@@ -1,20 +1,21 @@
 #!/usr/bin/env python
-"""bench.py -- decode tokens/s of the layer-sliced LLaMA forward on B200 (BASELINE.json's metric).
+"""bench.py -- decode tokens/s of the layer-sliced LLaMA forward on H100 (BASELINE.json's metric).
 
 A "step" is one pass of the hot path over one batch of synthetic input: ONE token (batch 1)
 propagated through every layer of the model's slice(s) with the KV cache at position p, p cycling
 through [256, 512) (seq_len 512) after a 256-token prefill.  Workload = BASELINE.json configs[1]
-(LLaMA-7B Q4_0, 1 slice on 1xB200) at N=1; at N>1 the same 32 layers are cut into N contiguous
+(LLaMA-7B Q4_0, 1 slice on 1xH100) at N=1; at N>1 the same 32 layers are cut into N contiguous
 slices, one rank per GPU, and the activation is handed from rank r to r+1 by one NCCL send/recv
 (configs[2] at N=4).
 
     python bench.py [--gpus N] [--steps K] [--warmup W]            # this framework
+    python bench.py [...] --dump-outputs DIR                        # + DIR/hidden.npy: the last timed step's output
     python bench.py --impl reference [...]                          # the reference's CPU path
 
 Prints ONE JSON line (rank 0).  `value` = tokens/s with the activation resident in HBM;
 `e2e` = the same metric through the reference-facing C ABI call b200_slice_forward() with HOST
 buffers (H2D + D2H inside the timed region); `roofline` = achieved HBM GB/s of the weight-matmul
-kernel vs the measured peak; `cpu_baseline` = the reference CPU path timed on this box's cores.
+kernel vs the HBM peak; `cpu_baseline` = the reference CPU path timed on this box's cores.
 """
 from __future__ import annotations
 
@@ -40,28 +41,8 @@ UNIT = "tokens/s"
 N_CTX = 512
 PREFILL = 256
 SEED = 0
-FALLBACK_HBM_GBS = 6650.0
-NCU_CAPTURE = os.path.join(ROOT, "profiles", "r02_decode_kernels_ncu_full.md")
-
-
-def ncu_traffic_per_launch():
-    """dram__bytes_read.sum + dram__bytes_write.sum per k_gemv launch, averaged over the launches of the committed
-    `ncu --set full` capture of a decode step (profiles/r02_decode_kernels_ncu_full.md, produced by scripts/summarize_ncu.py
-    from the .ncu-rep): parsed here, not a constant.  Returns (read + write bytes, read bytes, launches) or (None, None, 0)."""
-    try:
-        rd = wr = n = 0
-        cols = None
-        for line in open(NCU_CAPTURE):
-            f = [x.strip() for x in line.strip().strip("|").split("|")]
-            if "dram_rd_MB" in f:
-                cols = {name: i for i, name in enumerate(f)}
-            elif cols and f and f[0].startswith("void k_gemv<"):
-                rd += float(f[cols["dram_rd_MB"]]) * 1e6
-                wr += float(f[cols["dram_wr_MB"]]) * 1e6
-                n += 1
-        return ((rd + wr) / n, rd / n, n) if n else (None, None, 0)
-    except Exception:
-        return None, None, 0
+FALLBACK_HBM_GBS = 3350.0          # NVIDIA H100 SXM data sheet (HBM3, 700 W card)
+L2_BYTES = 50 * 1024 * 1024        # H100 SXM L2
 
 
 def model_dir() -> str:
@@ -92,7 +73,7 @@ def measured_peak():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return FALLBACK_HBM_GBS, "fallback (B200_PROFILING.md)"
+        return FALLBACK_HBM_GBS, "fallback (H100 SXM data sheet: 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -147,8 +128,8 @@ class ClockSampler:
 
 # ------------------------------------------------------------------------------------------- reference arm
 def cpu_reference_run(path: str, n_embd: int, steps: int, warmup: int, prompt: int = 16, want_outputs: bool = False):
-    """Time the reference's own CPU implementation (oracle/_ref, built from /root/reference in the build
-    container) on this box's host cores; falls back to the C port when oracle/_ref is absent."""
+    """Time the reference's own CPU implementation (oracle/_ref, built by oracle/Makefile where the reference sources
+    exist) on this box's host cores; falls back to the C port when oracle/_ref is absent."""
     from oracle import oracle
     try:
         avail = len(os.sched_getaffinity(0))
@@ -245,7 +226,7 @@ def run_reference(args):
     return 0
 
 
-# ------------------------------------------------------------------------------------------- B200 arm
+# ------------------------------------------------------------------------------------------- GPU arm
 def run_b200(args):
     from distributedllm_b200 import capi
 
@@ -332,6 +313,12 @@ def run_b200(args):
     barrier()
     wall_ms = 1e3 * (time.perf_counter() - t0)
     dev_ms = sl.mark_elapsed_ms()
+    if args.dump_outputs and rank == 0:
+        # the hidden state the last timed step handed back (on a ring: the last slice's output, returned to rank 0)
+        hidden = np.empty((1, E), np.float32)
+        _d2h(sl, hidden)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "hidden.npy"), hidden)
     launches = sl.launch_count() - launches0
     if dist is not None:
         import torch
@@ -448,7 +435,6 @@ def run_b200(args):
                         "note": "launches overlap under programmatic dependent launch, so per-class times can sum to more than the step"}
         except Exception as ex:
             in_graph = {"error": repr(ex)}
-        traffic, traffic_rd, traffic_n = ncu_traffic_per_launch()
         replay = {"achieved": achieved, "frac": achieved / peak, "avg_launch_us": 1e3 * only_ms / n_gemv,
                   "timing": "two CUDA events on the slice's stream around %d graph replays of the step's %d k_gemv launches with the "
                             "attention launch skipped (b200_debug_skip_attention): the matmul kernels back to back" % (reps, n_gemv)}
@@ -458,9 +444,6 @@ def run_b200(args):
                 # all): launch duration = last CTA exit - first CTA entry from in-kernel %globaltimer stamps
                 "achieved": in_step["achieved"] if in_step else achieved, "peak": peak, "unit": "GB/s",
                 "frac": (in_step["achieved"] if in_step else achieved) / peak, "peak_source": peak_src,
-                "traffic": traffic, "traffic_read_only": traffic_rd,
-                "traffic_source": "profiles/r02_decode_kernels_ncu_full.md: dram__bytes_read.sum + dram__bytes_write.sum averaged over its "
-                                  "%d k_gemv launches (ncu --set full, one decode step, cold caches)" % traffic_n,
                 "timing": ("in-step: %globaltimer stamps of every k_gemv launch inside the replayed decode graph, last of 3 steps"
                            if in_step else "matmul-only graph replay (in-step stamps unavailable)"),
                 "algorithmic_bytes_per_launch": wbytes / n_gemv,
@@ -564,14 +547,14 @@ def run_b200(args):
         barrier()
 
     # ---- prompt throughput of the same model (not the headline metric): one 512-token call, device-resident, exact mode and the
-    # opt-in tcgen05 fast mode (K2: dequant fused into a TMA-fed tcgen05 / TMEM tile kernel; tolerance-level parity)
+    # opt-in tensor-core fast mode (K2: dequant fused into a TMA-fed wgmma tile kernel; tolerance-level parity)
     prefill = None
     if world == 1:
         try:
             x512 = synth_inputs(N_CTX, E, 3)
             _h2d(sl, x512)
             prefill, outs = {}, {}
-            for name, fast in (("exact", False), ("tcgen05_fast", True)):
+            for name, fast in (("exact", False), ("wgmma_fast", True)):
                 sl.set_fast_prefill(fast, 32)
                 for rep in range(2):
                     sl.clear_context()
@@ -585,7 +568,7 @@ def run_b200(args):
                 outs[name] = o
             sl.set_fast_prefill(False, 32)
             sl.clear_context()
-            d = outs["tcgen05_fast"] - outs["exact"]
+            d = outs["wgmma_fast"] - outs["exact"]
             prefill["fast_vs_exact_rel_rms"] = float(np.sqrt(np.mean(d * d)) / np.sqrt(np.mean(outs["exact"] ** 2)))
             prefill["what"] = ("one %d-token prompt call through all 32 layers, activations resident in HBM; fast mode = fp16 tensor-core "
                                "matmuls (fastgemm2.cuh), off by default, decode is always exact" % N_CTX)
@@ -596,7 +579,7 @@ def run_b200(args):
         line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": K, "warmup": W,
                 "ms_per_step": dev_ms / K, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
                 "dtype": "q4_0*q8_0->f32", "data": "synthetic",
-                "config": {"workload": "LLaMA-7B Q4_0 (BASELINE.json configs[%d]): %d slice(s) x %s layers on %dxB200, "
+                "config": {"workload": "LLaMA-7B Q4_0 (BASELINE.json configs[%d]): %d slice(s) x %s layers on %dxH100, "
                                        "n_ctx=512 batch=1, one decoded token per step after a 256-token prefill; timed steps at "
                                        "positions %s" % (1 if world == 1 else 2, world,
                                                           "/".join(str(y - x + 1) for x, y in layer_ranges(32, world)), world,
@@ -607,7 +590,7 @@ def run_b200(args):
                            "parallelism": ("pp%d (layer slices; hand-off = %s)" % (world, "peer-memory store + flag over NVLink inside the step graph"
                                                                     if transport == "peer" else "one ncclSend/ncclRecv per hop")) if world > 1 else "pp1",
                            "handoff_transport": transport,
-                           "l2": "no flush: each step streams %.2f GB of weights, 29x the 126 MB L2" % (W_all / 1e9),
+                           "l2": "no flush: each step streams %.2f GB of weights, %.0fx the 50 MB L2" % (W_all / 1e9, W_all / L2_BYTES),
                            "timing": "CUDA events on the slice's stream around %d steps; wall %.1f ms" % (K, wall_ms)},
                 "clocks": clk, "e2e": e2e, "gpu_launches": launches, "roofline": roof, "step_roofline": step_roof,
                 "tokens_per_s_at_p511": at_p511["tokens_per_s"], "at_p511": at_p511, "prefill": prefill,
@@ -663,6 +646,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=8)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's output to DIR/hidden.npy (float32)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

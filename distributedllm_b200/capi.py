@@ -1,5 +1,5 @@
 """ctypes binding of libb200slice.so (include/b200_slice.h).  No torch, no CPU fallback:
-importing works anywhere, every call needs a B200."""
+importing works anywhere, every call needs an H100."""
 from __future__ import annotations
 
 import ctypes as C
@@ -229,7 +229,7 @@ class Slice:
         n = lib().b200_debug_trace_read(self._h, _ptr(buf), _ptr(cls), _ptr(ctas), max_launches)
         return buf[:n], cls[:n], ctas[:n]
 
-    def ptrace_read(self, n_sm: int = 148):
+    def ptrace_read(self, n_sm: int = 132):
         """-> stamps [n_cta][n_layer][16] uint64 ns of the last persistent step (B200_PTRACE=1)."""
         L = self.info.n_layer
         buf = np.zeros((n_sm, L, 16), np.uint64)

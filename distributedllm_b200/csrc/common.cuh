@@ -1,4 +1,4 @@
-// common.cuh -- error plumbing and sm_100a PTX helpers shared by the slice runtime.
+// common.cuh -- error plumbing and sm_90a PTX helpers shared by the slice runtime.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>

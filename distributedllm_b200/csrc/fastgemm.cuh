@@ -1,16 +1,16 @@
-// fastgemm.cuh -- K2: prefill weight matmul on the 5th-generation tensor cores ("fast mode").
+// fastgemm.cuh -- K2: prefill weight matmul on the Hopper tensor cores ("fast mode").
 //
 //   Y[token][row] = sum_k  W[row][k] * X[token][k]        W: Q4_0 (packed layout of kernels.cuh), X: activations
 //
-// tcgen05.mma (kind::f16, M=128, N=128, K=16, cta_group::1) with the fp32 accumulator in TENSOR MEMORY:
+// wgmma.mma_async (m64n128k16, f16 x f16 -> f32) with the fp32 accumulator in the registers of one warpgroup:
 //   * the producer lane streams the packed Q4_0 chunks of four 32-row tiles (= one 128-row M tile) with 1-D TMA bulk
 //     copies into a raw ring -- the same 18 B/block HBM traffic as the decode kernel, nothing is dequantised in HBM;
-//   * four dequant warps expand each 4-block quad to fp16 IN SHARED MEMORY, writing the K-major SWIZZLE_128B layout the
-//     UMMA shared-memory descriptor expects (fp16 magic-number nibble conversion, one HMUL2 by the block scale), and
-//     copy the matching activation tile; `fence.proxy.async` hands the tiles to the tensor core's async proxy;
-//   * ONE elected thread issues 8 tcgen05.mma per 128-wide K block and `tcgen05.commit`s to an mbarrier that recycles
-//     the stage; after the last K block the four warps read the accumulator back with tcgen05.ld (32 lanes x 16
-//     columns per instruction) and apply the fused epilogue (store | +residual | SiLU-gate).
+//   * the four warps of the consumer warpgroup expand each 4-block quad to fp16 IN SHARED MEMORY, writing the K-major
+//     SWIZZLE_128B layout the GMMA shared-memory descriptor expects (fp16 magic-number nibble conversion, one HMUL2 by
+//     the block scale), and copy the matching activation tile; `fence.proxy.async` hands the tiles to the async proxy;
+//   * the same warpgroup then issues 2 x 8 wgmma per 128-wide K block (rows 0..63 and 64..127, 128 accumulator registers
+//     a thread) and keeps one K block in flight while it dequantises the next; after the last K block it applies the
+//     fused epilogue straight from the accumulator registers (store | +residual | SiLU-gate).
 // Numerics ("fast mode", tolerance-checked, NOT bit-exact): activations go through the reference's Q8_0
 // quantisation (k_prep_q8_f16) and both operands are rounded to fp16 (<= 2^-11 relative each); products are exact
 // in fp32 and accumulated in fp32 in hardware order.  Measured: 2.7e-4 relative RMS on one matmul; ~5e-3 per layer on
@@ -60,27 +60,72 @@ __global__ void __launch_bounds__(256) k_prep_q8_f16(const PrepArgs a) {
     }
 }
 
-// ---- tcgen05 helpers -----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-    // K-major, SWIZZLE_128B, 8-row groups 1024 B apart (cute::UMMA::SmemDescriptor: start>>4 | LBO 1 | SBO 64 | version 1 | layout 2)
-    return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t) 1 << 16) | ((uint64_t) 64 << 32) | ((uint64_t) 1 << 46) | ((uint64_t) 2 << 61);
-}
-__device__ __forceinline__ uint32_t umma_idesc_f16_f32(int M, int N) {
-    // c_format F32 (1) at bit 4, a/b format F16 (0), K-major both, n_dim = N>>3 at bit 17, m_dim = M>>4 at bit 24
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{ .reg .pred p; setp.ne.b32 p, %4, 0; tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p; }"
-                 :: "r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t * bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(smem_u32(bar)) : "memory");
+// ---- wgmma helpers -------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint64_t gmma_desc_k_sw128(uint32_t smem_addr) {
+    // K-major, SWIZZLE_128B, 8-row groups 1024 B apart (sm_90 GMMA descriptor: start>>4 | LBO 1 | SBO 64 | layout 1 = 128B swizzle)
+    return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t) 1 << 16) | ((uint64_t) 64 << 32) | ((uint64_t) 1 << 62);
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after()  { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence()  { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+// keeps the compiler from touching accumulator registers across an in-flight wgmma
+__device__ __forceinline__ void acc_fence(float (&d)[64]) {
+    #pragma unroll
+    for (int i = 0; i < 64; i++) asm volatile("" : "+f"(d[i]) :: "memory");
+}
+// D[64 x 128] += A[64 x 16] * B[128 x 16]^T: fp16 operands K-major in shared memory, fp32 accumulator in the registers of
+// the issuing warpgroup (thread t holds rows 16*(t/32) + (t%32)/4 + {0, 8}, columns 8*j + 2*(t%4) + {0, 1} as d[4j + 2i + c])
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile("{ .reg .pred p; setp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+                 "%64, %65, p, 1, 1, 0, 0; }"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                   "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                   "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                   "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(da), "l"(db), "n"(1)
+                 : "memory");
+}
 
 enum { FG_STORE = 0, FG_RESID = 1, FG_GATE = 2 };
+
+// Epilogue of one 64 x 128 accumulator block (layout of wgmma_m64n128k16): this thread holds rows m0 and m0 + 8 of the
+// 128-row M tile (packed order) for the token pairs tok0 + 8j + {0, 1}.
+template <int EPI, class Args>
+__device__ __forceinline__ void gmma_epilogue(const Args & a, const float (&d)[64], int mt, int m0, int tok0) {
+    #pragma unroll
+    for (int j = 0; j < 16; j++) {
+        #pragma unroll
+        for (int c = 0; c < 2; c++) {
+            const int tok = tok0 + 8 * j + c;
+            if (tok >= a.N) continue;
+            if (EPI == FG_GATE) {
+                // packed G=2 order: row-groups alternate w1 / w3, so row m0 (w1, bit 3 clear) pairs with row m0 + 8 (w3)
+                const int row = (mt * 8 + (m0 >> 4)) * 8 + (m0 & 7);
+                if (row < a.out_rows) a.y[(size_t) tok * a.ldy + row] = fmul(h2f(a.tsilu[f2h(d[4 * j + c])]), d[4 * j + 2 + c]);
+            } else {
+                #pragma unroll
+                for (int i = 0; i < 2; i++) {
+                    const int row = mt * 128 + m0 + 8 * i;
+                    float val = d[4 * j + 2 * i + c];
+                    if (row < a.out_rows) {
+                        if (EPI == FG_RESID) val = fadd(val, a.resid[(size_t) tok * a.ldr + row]);
+                        a.y[(size_t) tok * a.ldy + row] = val;
+                    }
+                }
+            }
+        }
+    }
+}
 
 struct FastGemmArgs {
     PackedW W;                  // G=1 packing for STORE/RESID (TR = 4), G=2 packing (TR = 8) for GATE
@@ -96,8 +141,7 @@ __global__ void __launch_bounds__(160, 1) k_gemm_q4_tc(const FastGemmArgs a) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t * smem = (uint8_t *)(((uintptr_t) smem_raw + 1023) & ~(uintptr_t) 1023);       // SWIZZLE_128B tiles need 1 KB alignment
     uint64_t * bars = (uint64_t *)(smem + kFgStages * kFgStageBytes);
-    uint64_t * raw_full = bars, * ab_full = bars + 2, * stage_free = bars + 4, * acc_full = bars + 6;
-    uint32_t * tmem_slot = (uint32_t *)(bars + 8);
+    uint64_t * raw_full = bars, * stage_free = bars + 2;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int mt = blockIdx.x, nt = blockIdx.y;             // 128-row tile, 128-token tile
     const int nbq = a.W.nbq, K = a.W.K;
@@ -105,63 +149,42 @@ __global__ void __launch_bounds__(160, 1) k_gemm_q4_tc(const FastGemmArgs a) {
     const int tiles_per_m = 16 / TRp;                       // packed tiles per 128 rows (16 row-groups)
 
     if (tid == 0) {
-        for (int s = 0; s < kFgStages; s++) { mbar_init(&raw_full[s], 1); mbar_init(&ab_full[s], 4); mbar_init(&stage_free[s], 1); }
-        mbar_init(acc_full, 1);
+        for (int s = 0; s < kFgStages; s++) { mbar_init(&raw_full[s], 1); mbar_init(&stage_free[s], 1); }
         mbar_fence_init();
     }
-    if (warp == 4) {                                        // TMEM: 128 columns of fp32 accumulator
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 128;" :: "r"(smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == 4) {
         if (lane == 0) {
-            // ---------------------------------------------------------------- TMA producer + MMA issuer (one thread)
+            // ---------------------------------------------------------------- TMA producer (one thread)
             grid_dep_launch();
-            const uint32_t idesc = umma_idesc_f16_f32(kFgM, kFgN);
-            for (int kb = 0; kb < nbq + 1; kb++) {
-                if (kb < nbq) {                              // stream the raw quad of 128 rows for K block kb
-                    const int s = kb % kFgStages, use = kb / kFgStages;
-                    if (use > 0) mbar_wait(&stage_free[s], (use - 1) & 1);
-                    uint8_t * raw = smem + (size_t) s * kFgStageBytes;
-                    const uint32_t per_tile = (uint32_t) TRp * kQ4Chunk;
-                    mbar_arrive_expect_tx(&raw_full[s], (uint32_t) kFgRawBytes);
-                    for (int t = 0; t < tiles_per_m; t++) {
-                        const uint8_t * src = a.W.data + (long long)(mt * tiles_per_m + t) * a.W.tile_bytes + (size_t) kb * per_tile;
-                        bulk_g2s(raw + (size_t) t * per_tile, src, per_tile, &raw_full[s]);
-                    }
-                }
-                if (kb > 0) {                                // issue the MMAs of K block kb-1
-                    const int j = kb - 1, s = j % kFgStages;
-                    mbar_wait(&ab_full[s], (j / kFgStages) & 1);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(smem + (size_t) s * kFgStageBytes + kFgRawBytes);
-                    const uint32_t b_addr = a_addr + kFgABytes;
-                    #pragma unroll
-                    for (int k16 = 0; k16 < 8; k16++) {
-                        const uint32_t sub = (k16 >> 2) * (kFgM * 128), off = (k16 & 3) * 32;      // sub-tile of 64 K, 32 B per UMMA_K
-                        umma_f16(tmem_base, umma_desc_k_sw128(a_addr + sub + off), umma_desc_k_sw128(b_addr + sub + off),
-                                 idesc, (j > 0 || k16 > 0) ? 1u : 0u);
-                    }
-                    umma_commit(&stage_free[s]);
-                    if (j == nbq - 1) umma_commit(acc_full);
+            for (int kb = 0; kb < nbq; kb++) {               // stream the raw quad of 128 rows for K block kb
+                const int s = kb % kFgStages, use = kb / kFgStages;
+                if (use > 0) mbar_wait(&stage_free[s], (use - 1) & 1);
+                uint8_t * raw = smem + (size_t) s * kFgStageBytes;
+                const uint32_t per_tile = (uint32_t) TRp * kQ4Chunk;
+                mbar_arrive_expect_tx(&raw_full[s], (uint32_t) kFgRawBytes);
+                for (int t = 0; t < tiles_per_m; t++) {
+                    const uint8_t * src = a.W.data + (long long)(mt * tiles_per_m + t) * a.W.tile_bytes + (size_t) kb * per_tile;
+                    bulk_g2s(raw + (size_t) t * per_tile, src, per_tile, &raw_full[s]);
                 }
             }
         }
     } else {
-        // -------------------------------------------------------------------- dequant warps (128 threads)
+        // -------------------------------------------------------------------- dequant + MMA warpgroup (128 threads)
         grid_dep_wait();
+        float acc[2][64];                                    // rows 0..63 and 64..127 of the M tile
+        #pragma unroll
+        for (int h = 0; h < 2; h++)
+            #pragma unroll
+            for (int i = 0; i < 64; i++) acc[h][i] = 0.f;
         const int r8 = lane >> 2, w = lane & 3;
         for (int kb = 0; kb < nbq; kb++) {
             const int s = kb % kFgStages, use = kb / kFgStages;
             uint8_t * stage = smem + (size_t) s * kFgStageBytes;
             uint8_t * A = stage + kFgRawBytes, * B = A + kFgABytes;
             // B tile: tokens nt*128 .. +127, K block kb: [128 tokens][128 halfs] -> two SW128 sub-tiles (stage is free: the
-            // producer waited on stage_free before re-arming raw_full, and we wait on raw_full below before touching A)
+            // wgmma group that last read it, K block kb-2, was retired by wgmma_wait<1> at the end of K block kb-1)
             mbar_wait(&raw_full[s], use & 1);
             for (int c = tid; c < kFgN * 16; c += 128) {     // 16-byte chunks: 128 rows x 16 chunks
                 const int row = c >> 4, ch = c & 15, tok = nt * kFgN + row;
@@ -208,45 +231,28 @@ __global__ void __launch_bounds__(160, 1) k_gemm_q4_tc(const FastGemmArgs a) {
                 }
             }
             fence_proxy_async();                             // generic-proxy writes -> visible to the tensor core's async proxy
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&ab_full[s]);
-        }
-        // -------------------------------------------------------------------- epilogue: TMEM -> registers -> global
-        mbar_wait(acc_full, 0);
-        tc_fence_after();
-        const int m = warp * 32 + lane;                      // accumulator lane = row within the M tile (packed order)
-        #pragma unroll 1
-        for (int c0 = 0; c0 < kFgN; c0 += 16) {
-            uint32_t v[16];
-            const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t) c0;
-            asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                         : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                           "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                         : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+            named_bar_sync(1, 128);                          // A and B complete; the raw quad is consumed
+            if (tid == 0) mbar_arrive(&stage_free[s]);
+            const uint32_t a_addr = smem_u32(A), b_addr = smem_u32(B);
+            wgmma_fence();
+            acc_fence(acc[0]); acc_fence(acc[1]);
             #pragma unroll
-            for (int j = 0; j < 16; j++) {
-                const int tok = nt * kFgN + c0 + j;
-                float val = __uint_as_float(v[j]);
-                if (EPI == FG_GATE) {
-                    // packed G=2 order: row-groups alternate w1 / w3, so lane l (w1) pairs with lane l^8 (w3) of the same row
-                    const float other = __shfl_xor_sync(0xffffffffu, val, 8);
-                    const int row = (mt * 8 + (m >> 4)) * 8 + (m & 7);
-                    if (!(m & 8) && tok < a.N && row < a.out_rows)
-                        a.y[(size_t) tok * a.ldy + row] = fmul(h2f(a.tsilu[f2h(val)]), other);
-                } else {
-                    const int row = mt * kFgM + m;
-                    if (tok < a.N && row < a.out_rows) {
-                        if (EPI == FG_RESID) val = fadd(val, a.resid[(size_t) tok * a.ldr + row]);
-                        a.y[(size_t) tok * a.ldy + row] = val;
-                    }
-                }
+            for (int k16 = 0; k16 < 8; k16++) {
+                const uint32_t sub = (k16 >> 2) * (kFgM * 128), off = (k16 & 3) * 32;          // sub-tile of 64 K, 32 B per K step of 16
+                #pragma unroll
+                for (int h = 0; h < 2; h++)
+                    wgmma_m64n128k16(acc[h], gmma_desc_k_sw128(a_addr + sub + h * (64 * 128) + off), gmma_desc_k_sw128(b_addr + sub + off));
             }
+            wgmma_commit();
+            wgmma_wait<1>();
+            acc_fence(acc[0]); acc_fence(acc[1]);
         }
-        tc_fence_before();
+        wgmma_wait<0>();
+        acc_fence(acc[0]); acc_fence(acc[1]);
+        // -------------------------------------------------------------------- epilogue: registers -> global
+        #pragma unroll
+        for (int h = 0; h < 2; h++) gmma_epilogue<EPI>(a, acc[h], mt, h * 64 + warp * 16 + r8, nt * kFgN + 2 * w);
     }
-    __syncthreads();
-    if (warp == 4) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 128;" :: "r"(tmem_base) : "memory");
 }
 
 }  // namespace b200

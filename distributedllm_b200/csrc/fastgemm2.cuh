@@ -1,14 +1,15 @@
-// fastgemm2.cuh -- K2, second generation: the prefill weight matmul as a tcgen05 / TMEM tile kernel fed by TMA.
+// fastgemm2.cuh -- K2, second generation: the prefill weight matmul as a wgmma tile kernel fed by TMA.
 //
 //   Y[token][row] = sum_k  W[row][k] * X[token][k]      W: Q4_0 or Q8_0 (packed layout of kernels.cuh), X: fp16 activations
 //
-// What changed against fastgemm.cuh (round 1: 2.5-3.9 % tensor pipe; profiles/r01_tcgen05_prefill_ncu_full.md):
-//   * CTA tile 128 weight rows x 256 TOKENS (tcgen05.mma kind::f16, M = 128, N = 256, K = 16; 256 TMEM columns): every
-//     dequantised weight tile is used against twice as many tokens;
+// What changed against fastgemm.cuh:
+//   * CTA tile 128 weight rows x 256 TOKENS (two consumer warpgroups, each 64 rows x 256 tokens as two wgmma m64n128k16
+//     accumulators, 128 fp32 registers a thread): every dequantised weight tile is used against twice as many tokens;
 //   * the activation tile comes in through the TENSOR-MAP TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B: the hardware writes
-//     the K-major layout the UMMA descriptor expects), issued by the producer lane next to the 1-D bulk copy of the raw
+//     the K-major layout the GMMA descriptor expects), issued by the producer lane next to the 1-D bulk copy of the raw
 //     quantised weights -- the dequant warps no longer spend half their instructions copying activations;
-//   * 8 dequant warps instead of 4, a dedicated MMA-issuing warp next to the TMA warp, so the three roles overlap;
+//   * 8 dequant warps instead of 4; each warpgroup dequantises its own 64 rows, issues their wgmma and keeps one K block in
+//     flight while it dequantises the next, so dequantisation and tensor-core work overlap;
 //   * Q8_0 weights as well as Q4_0 (int8 -> fp16 through the 0x6400 magic, one HMUL2 by the block scale).
 // Numerics as fastgemm.cuh ("fast mode", tolerance-checked, NOT bit-exact): operands rounded to fp16, fp32 accumulation
 // in hardware order.  Reference for the operation: ggml_compute_forward_mul_mat (ggml.c:10577-10749); the CUDA analogue in
@@ -22,7 +23,7 @@ namespace b200 {
 
 constexpr int kF2M = 128, kF2K = 128;                      // token-tile width NT = 256 (wide matrices) or 128 (narrow ones: twice the CTAs)
 constexpr int kF2DqWarps = 8;
-constexpr int kF2Threads = (kF2DqWarps + 2) * 32;          // + TMA warp + MMA warp
+constexpr int kF2Threads = (kF2DqWarps + 1) * 32;          // + TMA warp
 constexpr int kF2ABytes = kF2M * kF2K * 2;                  // 32 KB: two [128 x 64] K-major SW128 sub-tiles
 __host__ __device__ constexpr int f2_raw_bytes(int wt) { return 16 * chunk_bytes(wt); }                   // one quad of 128 rows
 __host__ __device__ constexpr int f2_stage_bytes(int wt, int nt) { return ((f2_raw_bytes(wt) + 1023) & ~1023) + kF2ABytes + nt * kF2K * 2; }
@@ -49,8 +50,7 @@ __global__ void __launch_bounds__(kF2Threads, 1) k_gemm_tc2(const FastGemm2Args 
     constexpr int RAW = 16 * CB, RAWP = (RAW + 1023) & ~1023, STAGE = RAWP + kF2ABytes + kF2BBytes;
     extern __shared__ __align__(1024) uint8_t smem[];       // SWIZZLE_128B tiles need 1 KB alignment (no static shared memory in this kernel)
     uint64_t * bars = (uint64_t *)(smem + kF2Stages * STAGE);
-    uint64_t * tma_full = bars, * a_full = bars + 3, * stage_free = bars + 6, * acc_full = bars + 9;
-    uint32_t * tmem_slot = (uint32_t *)(bars + 10);
+    uint64_t * tma_full = bars, * stage_free = bars + 3;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int mt = blockIdx.x, nt = blockIdx.y;             // 128-row tile, 256-token tile
     const int nbq = a.W.nbq;
@@ -58,18 +58,11 @@ __global__ void __launch_bounds__(kF2Threads, 1) k_gemm_tc2(const FastGemm2Args 
     const int tiles_per_m = 16 / TRp;                       // packed tiles per 128 rows (16 row-groups)
 
     if (tid == 0) {
-        for (int s = 0; s < kF2Stages; s++) { mbar_init(&tma_full[s], 1); mbar_init(&a_full[s], kF2DqWarps); mbar_init(&stage_free[s], 1); }
-        mbar_init(acc_full, 1);
+        // a stage is free once both consumer warpgroups have retired the wgmma group that read it
+        for (int s = 0; s < kF2Stages; s++) { mbar_init(&tma_full[s], 1); mbar_init(&stage_free[s], 2); }
         mbar_fence_init();
     }
-    if (warp == kF2DqWarps + 1) {                           // TMEM: 256 columns of fp32 accumulator
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "n"(NT) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == kF2DqWarps) {
         // -------------------------------------------------------------------- TMA producer (one thread)
@@ -92,29 +85,14 @@ __global__ void __launch_bounds__(kF2Threads, 1) k_gemm_tc2(const FastGemm2Args 
                 tma_load_2d(B + kF2N * 128, &xmap, kb * kF2K + 64, nt * kF2N, &tma_full[s]);
             }
         }
-    } else if (warp == kF2DqWarps + 1) {
-        // -------------------------------------------------------------------- MMA issuer (one thread)
-        if (lane == 0) {
-            const uint32_t idesc = umma_idesc_f16_f32(kF2M, kF2N);
-            for (int kb = 0; kb < nbq; kb++) {
-                const int s = kb % kF2Stages, ph = (kb / kF2Stages) & 1;
-                mbar_wait(&tma_full[s], ph);                 // B tile landed (and the raw weights)
-                mbar_wait(&a_full[s], ph);                   // A tile dequantised
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(smem + (size_t) s * STAGE + RAWP);
-                const uint32_t b_addr = a_addr + kF2ABytes;
-                #pragma unroll
-                for (int k16 = 0; k16 < 8; k16++) {
-                    const uint32_t off = (k16 & 3) * 32;                                     // 32 B per UMMA_K inside the 128 B swizzle atom
-                    umma_f16(tmem_base, umma_desc_k_sw128(a_addr + (k16 >> 2) * (kF2M * 128) + off),
-                             umma_desc_k_sw128(b_addr + (k16 >> 2) * (kF2N * 128) + off), idesc, (kb > 0 || k16 > 0) ? 1u : 0u);
-                }
-                umma_commit(&stage_free[s]);
-                if (kb == nbq - 1) umma_commit(acc_full);
-            }
-        }
     } else {
-        // -------------------------------------------------------------------- dequant warps (256 threads), then epilogue
+        // -------------------------------------------------------------------- two dequant + MMA warpgroups (256 threads)
+        const int wg = warp >> 2;                            // warpgroup wg dequantises and multiplies rows 64*wg .. +63
+        float acc[NT / 128][64];
+        #pragma unroll
+        for (int n = 0; n < NT / 128; n++)
+            #pragma unroll
+            for (int i = 0; i < 64; i++) acc[n][i] = 0.f;
         const int r8 = lane >> 2, w = lane & 3;
         for (int kb = 0; kb < nbq; kb++) {
             const int s = kb % kF2Stages, use = kb / kF2Stages;
@@ -173,46 +151,34 @@ __global__ void __launch_bounds__(kF2Threads, 1) k_gemm_tc2(const FastGemm2Args 
                 }
             }
             fence_proxy_async();                             // generic-proxy writes -> visible to the tensor core's async proxy
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&a_full[s]);
-        }
-        // -------------------------------------------------------------------- epilogue: TMEM -> registers -> global
-        mbar_wait(acc_full, 0);
-        tc_fence_after();
-        const int q = warp & 3, half = warp >> 2;            // TMEM lane quarter of this warp; which half of the token columns
-        const int m = q * 32 + lane;                         // accumulator lane = row within the M tile (packed order)
-        #pragma unroll 1
-        for (int c0 = half * (NT / 2); c0 < half * (NT / 2) + NT / 2; c0 += 16) {
-            uint32_t v[16];
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t) c0;
-            asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                         : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                           "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                         : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+            named_bar_sync(1 + wg, 128);                     // this warpgroup's 64 rows of A are complete
+            // A stage is rewritten only after the wgmma group that last read it (K block kb - stages) was retired below
+            const uint32_t a_addr = smem_u32(A) + wg * (64 * 128), b_addr = smem_u32(stage + RAWP + kF2ABytes);
+            wgmma_fence();
             #pragma unroll
-            for (int j = 0; j < 16; j++) {
-                const int tok = nt * kF2N + c0 + j;
-                float val = __uint_as_float(v[j]);
-                if (EPI == FG_GATE) {
-                    // packed G=2 order: row-groups alternate w1 / w3, so lane l (w1) pairs with lane l^8 (w3) of the same row
-                    const float other = __shfl_xor_sync(0xffffffffu, val, 8);
-                    const int row = (mt * 8 + (m >> 4)) * 8 + (m & 7);
-                    if (!(m & 8) && tok < a.N && row < a.out_rows)
-                        a.y[(size_t) tok * a.ldy + row] = fmul(h2f(a.tsilu[f2h(val)]), other);
-                } else {
-                    const int row = mt * kF2M + m;
-                    if (tok < a.N && row < a.out_rows) {
-                        if (EPI == FG_RESID) val = fadd(val, a.resid[(size_t) tok * a.ldr + row]);
-                        a.y[(size_t) tok * a.ldy + row] = val;
-                    }
-                }
+            for (int n = 0; n < NT / 128; n++) acc_fence(acc[n]);
+            #pragma unroll
+            for (int k16 = 0; k16 < 8; k16++) {
+                const uint32_t off = (k16 & 3) * 32;                                         // 32 B per K step of 16 inside the 128 B swizzle atom
+                #pragma unroll
+                for (int n = 0; n < NT / 128; n++)
+                    wgmma_m64n128k16(acc[n], gmma_desc_k_sw128(a_addr + (k16 >> 2) * (kF2M * 128) + off),
+                                     gmma_desc_k_sw128(b_addr + (k16 >> 2) * (kF2N * 128) + n * (128 * 128) + off));
             }
+            wgmma_commit();
+            wgmma_wait<1>();                                 // K block kb-1 retired: its stage may be refilled
+            #pragma unroll
+            for (int n = 0; n < NT / 128; n++) acc_fence(acc[n]);
+            if (kb > 0 && (tid & 127) == 0) mbar_arrive(&stage_free[(kb - 1) % kF2Stages]);
         }
-        tc_fence_before();
+        wgmma_wait<0>();
+        #pragma unroll
+        for (int n = 0; n < NT / 128; n++) acc_fence(acc[n]);
+        // -------------------------------------------------------------------- epilogue: registers -> global
+        #pragma unroll
+        for (int n = 0; n < NT / 128; n++)
+            gmma_epilogue<EPI>(a, acc[n], mt, wg * 64 + (warp & 3) * 16 + r8, nt * kF2N + n * 128 + 2 * w);
     }
-    __syncthreads();
-    if (warp == kF2DqWarps + 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "n"(NT) : "memory");
 }
 
 }  // namespace b200

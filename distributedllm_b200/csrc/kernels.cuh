@@ -1,4 +1,4 @@
-// kernels.cuh -- the sm_100a kernels of the slice forward (exact mode).
+// kernels.cuh -- the sm_90a kernels of the slice forward (exact mode).
 //
 // "Exact mode" = every rounding point and accumulation order of the reference's CPU path
 // (ggml's AVX2+FMA+F16C build) is reproduced, so hidden states are bit-identical:
@@ -333,7 +333,7 @@ __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
                 for (int s = 0; s < n_stage; s++) {
                     // Only `pre_stages` of weights may be requested before the consumers have put their (tiny, latency-
                     // critical) prologue loads on the wire: a prologue load queued behind ~20 MB of bulk-copy requests
-                    // waits ~5 us (profiles/r01_timeline_*.txt); behind 2 stages per CTA it waits < 1 us.
+                    // waits for them, behind 2 stages per CTA it does not.
                     if (issued == a.pre_stages) mbar_wait(actbar + 1, 0);
                     issued++;
                     if (use > 0) mbar_wait(&empty[slot], (use - 1) & 1);
@@ -412,7 +412,7 @@ __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
                 const int rot = NC == 1 ? (tid & 7) : 0;
                 if (NC == 1) {
                     // one TMA bulk copy of the row instead of 1024 LDG.128 per CTA: under a saturated memory system the
-                    // LDGs took ~2.9 us (in-kernel timeline), the bulk copy of a same-sized activation ~0.5 us.  Each
+                    // LDGs queue behind the weight stream, one bulk copy of the same bytes does not.  Each
                     // thread then reads its block with 16-byte chunks rotated by its lane so the quarter-warps never
                     // collide on a bank; chunk (j + rot) & 7 lands in v[4j..4j+3].
                     if (tid == 0) { mbar_arrive_expect_tx(actbar, (uint32_t) K * 4); bulk_g2s(xs, x, (uint32_t) K * 4, actbar); }
@@ -632,8 +632,8 @@ __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
     }
     if (EPI == EPI_RESID_NQ) {
         // The output row feeds an RMSNorm + weight matmul next.  Instead of every CTA of that matmul re-reading and
-        // re-normalising the whole row (16 KB of LDGs that queue behind its own weight stream: ~3 us per kernel, and
-        // 20 % extra L2 traffic), THIS kernel finishes the job while the values are still on chip:
+        // re-normalising the whole row (16 KB of LDGs that queue behind its own weight stream, and 20 % extra L2
+        // traffic), THIS kernel finishes the job while the values are still on chip:
         //   every CTA owns exactly one 32-row tile = one Q8_0 block (the host guarantees gridDim.x == n_tiles);
         //   1. partial sum of squares of its block -> global;  2. grid-wide arrive + spin on a counter;
         //   3. every CTA adds the n_tiles partials in the same fixed order -> identical RMS scale everywhere;
@@ -685,8 +685,7 @@ __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
 // =============================================================================================
 // K1n: the NARROW matrices of a single-token step (wo, w2: 128 tiles of 32 rows for 7B = at most one CTA per SM).
 // With k_gemv's mapping (4 threads per row) such a CTA is 4 consumer warps = ONE warp per scheduler, and a lone warp
-// cannot hide its own latencies: measured IPC 0.39, ~19 cycles per block step, wo 2.6 us / w2 6.1 us of main loop for
-// 9.4 / 25.4 MB (1.5 / 3.9 us at the HBM rate).  The parallelism exact mode allows is rows x 8 AVX lanes (each lane's fma
+// cannot hide its own latencies.  The parallelism exact mode allows is rows x 8 AVX lanes (each lane's fma
 // chain is sequential in K), so this variant spends ALL of it: 8 threads per row, thread (r, l) owns AVX lane l alone.
 //   * 8 consumer warps per CTA, warp = 4 rows x 8 lanes, same 32-row tile, same packed layout, same TMA ring;
 //   * per block and thread: one shift+mask (lanes 0..3 take the low nibbles of word l, lanes 4..7 the high nibbles of
@@ -695,9 +694,7 @@ __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
 //     why the wide matrices (qkv, w1|w3: >= 2.3 warps per scheduler already) keep k_gemv.
 // Pre-quantised input only (PRO_PREQ: the attention / gate epilogue already produced Q8_0), one column, epilogues
 // + residual and + residual + send (EPI_RESID, EPI_RESID_SEND).  Arithmetic per lane chain is k_gemv's, operand for operand.
-// MEASURED (7B Q4_0, 64 steps, same box): 806 tok/s with this kernel against 823 with k_gemv -- twice the warps and half the
-// instructions per warp did NOT shorten wo / w2, so their main loops are not bound by the lone warp's issue rate after all;
-// opt-in (B200_N8=1), bit-exact (tests/test_gpu_parity.py::test_narrow_matrix_kernel_is_a_scheduling_choice).
+// Opt-in (B200_N8=1), bit-exact (tests/test_gpu_parity.py::test_narrow_matrix_kernel_is_a_scheduling_choice).
 // =============================================================================================
 constexpr int kN8Warps = 8;
 constexpr int kN8Consumers = kN8Warps * 32;
@@ -975,8 +972,8 @@ __global__ void __launch_bounds__(256) k_gemv_f16(const GemvF16Args a) {
 }
 
 // K1f-mc: the same F16 matmul for MULTI-token calls (prompt chunks, batched steps).  k_gemv_f16 takes one column per CTA, so
-// every token re-reads the whole matrix from L2 (405 MB per 7B layer and token: a 1024-token prompt ran at the L2 rate, 66 us per
-// token and layer, barely faster than decoding).  Here a CTA carries NC columns: the activations sit in shared memory as f32
+// every token re-reads the whole matrix from L2 (405 MB per 7B layer and token: a long prompt runs at the L2 rate, barely faster
+// than decoding).  Here a CTA carries NC columns: the activations sit in shared memory as f32
 // (the fp16-rounded value widened, what h2f() would produce per use) interleaved [k][NC], so one 16-byte weight load and one
 // conversion per weight feed NC fma chains (LDS.128 = 4 columns).  Per column the chain is k_gemv_f16's, chunk for chunk.
 template <int PRO, int EPI, int NC>
@@ -1634,7 +1631,7 @@ __global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(256) k_attn128(const
         const int l = tid >> 4, cg = tid & 15;
         float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         // four value rows in flight per thread (rows past the staged window come from L2 / HBM: one dependent-looking load
-        // per iteration made this loop 13 us at T ~ 1000); the FMAs stay in position order
+        // per iteration would serialise their latencies); the FMAs stay in position order
         for (int tb = 8 * g + l; tb < lim; tb += 128) {
             uint4 vv4[4];
             #pragma unroll

@@ -1,6 +1,6 @@
 // llm_module.cpp -- the CPython module `llm`, drop-in for the reference's module of the same name
 // (distllm/tensor_processor.cpp:1992-2275): the same nine functions with the same argument meaning, backed
-// by the B200 slice runtime through its C ABI (include/b200_slice.h) instead of llama.cpp on the CPU.
+// by the H100 slice runtime through its C ABI (include/b200_slice.h) instead of llama.cpp on the CPU.
 //
 //   load_slice(path) -> 0            propagate_forward(list[float]) -> list[float] (int status on eval failure)
 //   unload_slice() -> 0              clear_context() -> 0
@@ -370,6 +370,6 @@ static PyMethodDef Methods[] = {
     {"decode_token", py_decode_token, METH_VARARGS, "Convert a token id to text"},
     {nullptr, nullptr, 0, nullptr}};
 
-static struct PyModuleDef llmmodule = {PyModuleDef_HEAD_INIT, "llm", "B200 slice runtime behind DistributedLLM's llm module API", -1, Methods};
+static struct PyModuleDef llmmodule = {PyModuleDef_HEAD_INIT, "llm", "H100 slice runtime behind DistributedLLM's llm module API", -1, Methods};
 
 PyMODINIT_FUNC PyInit_llm(void) { return PyModule_Create(&llmmodule); }

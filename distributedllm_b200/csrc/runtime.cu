@@ -2,7 +2,7 @@
 //
 // Replaces TransformerSlice / llama_eval_internal / the loader of the reference
 // (distllm/tensor_processor.cpp:1488-1562, 474-809, 926-1086, 1203-1416) for a slice resident on
-// one B200.  One stream per slice; the N=1 decode step is a CUDA graph replayed per token with
+// one H100.  One stream per slice; the N=1 decode step is a CUDA graph replayed per token with
 // the position kept in device memory.
 #include "kernels.cuh"
 #include "persist.cuh"
@@ -43,7 +43,7 @@ struct GraphKey { const float * in; float * out; int host; bool operator<(const 
 using namespace b200;
 
 struct b200_slice {
-    int device = 0, n_sm = 148;
+    int device = 0, n_sm = 132;
     cudaStream_t stream = nullptr;
     int E = 0, H = 0, D = 0, FF = 0, L = 0, first_layer = 0, n_ctx = 512, wtype = 0;
     // sessions (SURVEY 8f N3): independent sequences sharing the weights, each with its own KV cache and position.
@@ -68,7 +68,7 @@ struct b200_slice {
     int64_t launches = 0, weight_bytes = 0;
     bool use_ring = true, use_graph = true, use_pdl = false, use_nq = true, f16_ring = true, use_tiled_attn = true, use_n8 = false, f16_mc = true; int f16_mc_cols = 4;
     bool skip_attention = false;   // measurement aid: replay only the weight matmuls of a step (bench.py roofline)
-    bool fast_prefill = false; int fast_min_tokens = 32; uint16_t * xh = nullptr;   // tcgen05 prefill (fast mode)
+    bool fast_prefill = false; int fast_min_tokens = 32; uint16_t * xh = nullptr;   // tensor-core prefill (fast mode)
     int fast_version = 2;                                                               // 2: fastgemm2.cuh (TMA tensor map, N = 256), 1: fastgemm.cuh
     int opt_ns = 0, opt_cta_per_sm = 0, opt_nc = 0, opt_pre = 3, opt_nomath = 0;   // read once at load (environment)
     float ema_token_ms = 0.f;              // host-buffer decode calls: smoothed device time of one token (sleep-then-poll wait)
@@ -344,7 +344,7 @@ static int launch_norm_quant(b200_slice * s, const float * x, int ldx, const flo
     return launch_simple(s, k_norm_quant<kWT_Q8_0>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
 }
 
-// ---------------------------------------------------------------- fast-mode prefill (tcgen05), see fastgemm.cuh
+// ---------------------------------------------------------------- fast-mode prefill (wgmma), see fastgemm.cuh
 template <bool NORM>
 static int launch_prep(b200_slice * s, const float * x, int ldx, const float * norm_w, int K, int N) {
     PrepArgs p{x, ldx, norm_w, s->xh, K, N};
@@ -364,7 +364,7 @@ static int launch_fast_gemm(b200_slice * s, const PackedW & W, const float * res
     return launch_simple(s, kern, dim3((groups + 15) / 16, (N + kFgN - 1) / kFgN, 1), dim3(160, 1, 1), kFgSmem, a);
 }
 
-// second-generation tcgen05 prefill matmul (fastgemm2.cuh): 128 x 256 tiles, activations through a tensor-map TMA
+// second-generation wgmma prefill matmul (fastgemm2.cuh): 128 x 256 tiles, activations through a tensor-map TMA
 typedef CUresult (*TensorMapEncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                       const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
                                       CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -1178,7 +1178,7 @@ static void destroy(b200_slice * s) {
 extern "C" {
 
 const char * b200_last_error(void) { return b200::last_error_ref().c_str(); }
-const char * b200_version(void) { return "b200-slice 0.1 (sm_100a, exact mode)"; }
+const char * b200_version(void) { return "b200-slice 0.1 (sm_90a, exact mode)"; }
 
 int b200_slice_load(const char * path, int device, int n_ctx, b200_slice_t ** out) {
     return b200_slice_load_ex(path, device, n_ctx, 1, out);
@@ -1194,7 +1194,7 @@ int b200_slice_load_ex(const char * path, int device, int n_ctx, int n_sessions,
     if (device < 0 || device >= ndev) return fail(B200_ENODEV, "device %d out of range (%d visible)", device, ndev);
     cudaDeviceProp prop;
     B200_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail(B200_ENODEV, "device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return fail(B200_ENODEV, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
     B200_CUDA(cudaSetDevice(device));
     b200_slice * s = new b200_slice();
     s->device = device; s->n_sm = prop.multiProcessorCount;
@@ -1211,7 +1211,7 @@ int b200_slice_load_ex(const char * path, int device, int n_ctx, int n_sessions,
     s->use_tiled_attn = env_int("B200_TILED_ATTN", 1) != 0;
     s->f16_mc = env_int("B200_F16_MC", 1) != 0;      // F16 slices, multi-token calls: 4 (8) columns per CTA share the weight loads
     s->f16_mc_cols = env_int("B200_F16_MC", 1) == 8 ? 8 : 4;
-    s->use_n8 = env_int("B200_N8", 0) != 0;          // single-token wo / w2: 8 threads per row (k_gemv_n8): exact, opt-in (slower: 806 vs 823 tok/s)  // prompt chunks: query-tiled attention (K / V staged once per 16 queries)
+    s->use_n8 = env_int("B200_N8", 0) != 0;          // single-token wo / w2: 8 threads per row (k_gemv_n8): exact, opt-in  // prompt chunks: query-tiled attention (K / V staged once per 16 queries)
     s->f16_ring = env_int("B200_F16_RING", 1) != 0;          // F16-weight slices: TMA-ring matmul for single-token steps
     s->use_persist = env_int("B200_PERSIST", 0) != 0;         // single-token step as ONE persistent kernel (persist.cuh)
     s->persist_tr = env_int("B200_PERSIST_TR", 4); s->persist_ns = env_int("B200_PERSIST_NS", 0); s->persist_ctas = env_int("B200_PERSIST_CTAS", 0);
@@ -2017,7 +2017,7 @@ int b200_extra_load(const char * path, int device, b200_extra_t ** out) {
     if (device < 0 || device >= ndev) return fail(B200_ENODEV, "device %d out of range", device);
     cudaDeviceProp prop;
     B200_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail(B200_ENODEV, "device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return fail(B200_ENODEV, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
     B200_CUDA(cudaSetDevice(device));
     std::unique_ptr<GgjtFile> fp;
     try { fp.reset(new GgjtFile(path, true)); }

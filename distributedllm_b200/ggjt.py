@@ -471,7 +471,7 @@ def write_fast_q4_slice(path: str, shape: ModelShape, layer_from: int, layer_to:
     """Large-model generator for benchmarks.  Quantising 6.5e9 Gaussians takes minutes, so Q4_0
     blocks are written directly: each matrix is a window (at a per-tensor pseudo-random block
     offset, wrapping) into a 36 MiB pool of random blocks built once per fan-in.  The file is the
-    ground truth for both the B200 path and the CPU reference, so the distribution only has to keep
+    ground truth for both the GPU path and the CPU reference, so the distribution only has to keep
     activations finite; any layer range of the same (shape, seed) is reproducible.  Returns bytes written.
     `wtype` = T_Q4_1 writes 20-byte Q4_1 blocks from _fast_q41_pool instead."""
     assert wtype in (T_Q4_0, T_Q4_1)

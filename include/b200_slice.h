@@ -1,5 +1,5 @@
 /*
- * b200_slice.h -- C ABI of libb200slice.so, the B200 (sm_100a) slice runtime.
+ * b200_slice.h -- C ABI of libb200slice.so, the H100 (sm_90a) slice runtime.
  *
  * Drop-in boundary: these entry points are what the reference's CPython module `llm`
  * (distllm/tensor_processor.cpp:2238-2260) binds for the per-slice forward path, with Python
@@ -11,7 +11,7 @@
  *     tensor_processor.cpp:523 and 798-799); the library owns weights, KV cache and n_past;
  *   - activations are row-major [n_tokens][n_embd] float32 (ggml ne0 = n_embd);
  *   - one handle = one slice on one GPU; calls on a handle are serialised by an internal mutex;
- *   - there is NO CPU fallback: every call fails with B200_ENODEV when no sm_100 device is present.
+ *   - there is NO CPU fallback: every call fails with B200_ENODEV when no sm_90 device is present.
  */
 #ifndef B200_SLICE_H
 #define B200_SLICE_H
@@ -30,7 +30,7 @@ enum {
     B200_OK       = 0,
     B200_EINVAL   = 1,   /* bad argument (null handle, n_tokens <= 0, ...) */
     B200_EFILE    = 2,   /* slice file missing / malformed / unsupported tensor type */
-    B200_ENODEV   = 3,   /* no CUDA device, or device is not sm_100 */
+    B200_ENODEV   = 3,   /* no CUDA device, or device is not sm_90 */
     B200_ECUDA    = 4,   /* a CUDA call or kernel failed */
     B200_ECONTEXT = 5,   /* n_past + n_tokens would exceed n_ctx */
     B200_ENCCL    = 6,   /* pipeline hand-off failed */
@@ -101,7 +101,7 @@ int b200_session_forward_device(b200_slice_t * s, int session, const float * d_i
 int b200_batch_forward(b200_slice_t * s, const int * sessions, int n_seq, const float * in, float * out);      /* host buffers */
 int b200_batch_forward_device(b200_slice_t * s, const int * sessions, int n_seq, const float * d_in, float * d_out, int sync);
 
-/* Fast mode for prefill calls (n_tokens >= min_tokens): the Q4_0 / Q8_0 weight matmuls run on the tcgen05 tensor cores with
+/* Fast mode for prefill calls (n_tokens >= min_tokens): the Q4_0 / Q8_0 weight matmuls run on the wgmma tensor cores with
  * the dequantisation fused in (csrc/fastgemm2.cuh; Q4_1 and F16 slices ignore the switch and stay exact).  NOT bit-exact: operands are rounded to fp16 after the reference's
  * Q8_0 activation quantisation; deviation from exact mode is bounded in tests/test_gpu_fast_prefill.py.  Off by default
  * (or B200_FAST_PREFILL=1); decode steps always run in exact mode. */
@@ -170,7 +170,7 @@ int b200_pipeline_step(b200_slice_t * s, const float * d_in, int n_tokens, int r
  * between the slices).  Every rank passes the same session list. */
 int b200_pipeline_step_session(b200_slice_t * s, int session, const float * d_in, int n_tokens, int ring);
 int b200_pipeline_step_batch(b200_slice_t * s, const int * sessions, int n_seq, const float * d_in, int ring);
-/* Peer-memory hand-off (the B200-native hop): every rank owns a MAILBOX in its HBM (sequence flags + two inbox slots of
+/* Peer-memory hand-off (the on-box GPU-native hop): every rank owns a MAILBOX in its HBM (sequence flags + two inbox slots of
  * [n_ctx][n_embd] f32) that its ring neighbours map over NVLink with cudaIpc.  After b200_pipeline_init, each rank
  * exports its 64-byte handle, the host gathers all of them (torch.distributed all_gather, a file, ...) and every rank
  * connects.  From then on b200_pipeline_step* hands the activation over with a store into the next rank's mailbox + a

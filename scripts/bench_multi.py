@@ -1,6 +1,6 @@
 """Multi-GPU measurements of BASELINE.json configs 4 and 5 (one process per GPU, launch with torch.distributed.run):
 
-  config 5  LLaMA-13B Q4_0, N slices across N B200s, n_ctx 512, S sessions in THROUGHPUT MODE:
+  config 5  LLaMA-13B Q4_0, N slices across N H100s, n_ctx 512, S sessions in THROUGHPUT MODE:
               serial      one session after another, each token waits for its ring result (what a bs=1 client does)
               batched     all S sessions in one batched step travelling through the slices (weights read once per slice)
               pipelined   sessions (or micro-batches of sessions) issued back to back with ring = 2 and collected later:
@@ -273,7 +273,7 @@ def config5():
         kv_pos = sh.n_layer * 2 * E * 2
         p_mid = PRE + 2 + K / 2
         single = peak_single = PEAK * 1e9 / (w_all + kv_pos * p_mid)
-        out = {"config": "BASELINE config 5: LLaMA-13B Q4_0, %d slice(s) x %s layers on %dxB200, n_ctx 512, %d sessions (throughput mode), "
+        out = {"config": "BASELINE config 5: LLaMA-13B Q4_0, %d slice(s) x %s layers on %dxH100, n_ctx 512, %d sessions (throughput mode), "
                          "decode at p~%d" % (world, "/".join(str(y - x + 1) for x, y in ranges), world, S, p_mid),
                "transport": transport, "modes": modes, "groups": G, "sessions": S, "steps_in_flight": LAG,
                "aggregate_tokens_per_s": max(m["tokens_per_s"] for m in modes.values()),
@@ -380,7 +380,7 @@ def config4():
         kv_pos = sh.n_layer * 2 * E * 2
         p_mid = PRE + 4 + K / 2
         bound = PEAK * 1e9 / (w_all + kv_pos * p_mid)
-        out = {"config": "BASELINE config 4: LLaMA-7B F16 (no quantisation), %d slice(s) x %s layers on %dxB200, n_ctx 2048 batch 1, "
+        out = {"config": "BASELINE config 4: LLaMA-7B F16 (no quantisation), %d slice(s) x %s layers on %dxH100, n_ctx 2048 batch 1, "
                          "decode at p~%d after a %d-token prefill" % (world, "/".join(str(y - x + 1) for x, y in ranges), world, p_mid, PRE),
                "transport": transport, "tokens_per_s": 1e3 / ms, "ms_per_step": ms, "us_per_layer_incl_handoff": 1e3 * ms / sh.n_layer,
                "roofline_tokens_per_s_one_gpu": bound, "frac_of_one_gpu": (1e3 / ms) / bound,

@@ -1,4 +1,4 @@
-// Micro-benchmark: issue rate of IDP.4A, FFMA, FADD, LOP3 and IMMA.16832.S8 on sm_100a (per SM per clock).
+// Micro-benchmark: issue rate of IDP.4A, FFMA, FADD, LOP3 and IMMA.16832.S8 on sm_90a (per SM per clock).
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -35,13 +35,13 @@ template <int OP> __global__ void k(int iters, int * out, long long * cyc) {
     if (threadIdx.x == 0) cyc[blockIdx.x] = t1 - t0;
 }
 template <int OP> void run(const char * name, int per_iter) {
-    int * out; long long * cyc; cudaMalloc(&out, 148 * 1024 * 4); cudaMalloc(&cyc, 148 * 8);
+    int * out; long long * cyc; cudaMalloc(&out, 132 * 1024 * 4); cudaMalloc(&cyc, 132 * 8);
     for (int warps : {4, 8, 16, 32}) {
         const int iters = 2000;
-        k<OP><<<148, warps * 32>>>(iters, out, cyc); cudaDeviceSynchronize();
-        k<OP><<<148, warps * 32>>>(iters, out, cyc); cudaDeviceSynchronize();
-        long long h[148]; cudaMemcpy(h, cyc, sizeof h, cudaMemcpyDeviceToHost);
-        double c = 0; for (int i = 0; i < 148; i++) c += h[i]; c /= 148;
+        k<OP><<<132, warps * 32>>>(iters, out, cyc); cudaDeviceSynchronize();
+        k<OP><<<132, warps * 32>>>(iters, out, cyc); cudaDeviceSynchronize();
+        long long h[132]; cudaMemcpy(h, cyc, sizeof h, cudaMemcpyDeviceToHost);
+        double c = 0; for (int i = 0; i < 132; i++) c += h[i]; c /= 132;
         printf("%-8s warps/SM %2d : %.2f warp-instr/clk/SM (%.2f per SMSP)\n", name, warps, (double) iters * per_iter * warps / c, (double) iters * per_iter * warps / c / 4);
     }
 }

@@ -1,4 +1,4 @@
-"""Prefill throughput of the 7B slice: exact mode (NC=8 dp4a columns) vs fast mode (tcgen05), N tokens in one call."""
+"""Prefill throughput of the 7B slice: exact mode (NC=8 dp4a columns) vs fast mode (wgmma), N tokens in one call."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -19,7 +19,7 @@ for mode in (0, 1):
     ms = min(ts[1:])
     flops = 2.0 * N * L * (4 * 4096 * 4096 + 3 * 4096 * 11008)
     print("%s prefill: %d tokens x %d layers  %.3f ms  -> %.0f tok/s (32-layer equiv %.0f tok/s), %.1f TFLOP/s" %
-          ("fast(tcgen05)" if mode else "exact(dp4a) ", N, L, ms, N / (ms / 1e3), N / (ms * 32 / L / 1e3), flops / (ms / 1e3) / 1e12))
+          ("fast(wgmma)  " if mode else "exact(dp4a) ", N, L, ms, N / (ms / 1e3), N / (ms * 32 / L / 1e3), flops / (ms / 1e3) / 1e12))
     sl.profile(True)
     sl.clear_context(); sl.forward_device(sl.dev_in, N, sl.dev_out)
     ms_c, cnt = sl.profile_read(); sl.profile(False)

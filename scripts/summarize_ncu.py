@@ -1,4 +1,4 @@
-"""Turn an .ncu-rep (ncu --set full) into a compact per-launch table for profiles/."""
+"""Turn an .ncu-rep (ncu --set full) into a compact per-launch table (profiles/ is git-ignored)."""
 import csv, io, subprocess, sys
 rep, out = sys.argv[1], sys.argv[2]
 raw = subprocess.run(["ncu", "-i", rep, "--page", "raw", "--csv"], capture_output=True, text=True).stdout

@@ -6,6 +6,8 @@
   extra.npz      reference get_inputs / get_llm_output / llama_tokenize on a synthetic extra-layers file
   tokenizer.json reference tokenisation of fixed strings with vendor/llama.cpp/models/ggml-vocab.bin's vocabulary
   protocol.json  frames produced by the reference's distllm/protocol.py for one instance of every message
+  ref_digests.json  SHA-256 of the reference's outputs (and its greedy ids) in the tests whose inputs are too large to store
+                 (`gen_golden.py digests` writes only this)
 
     python tests/golden/gen_golden.py          # needs /root/reference and a built oracle/_ref
 """
@@ -72,10 +74,107 @@ def gen_q4_1(tmp):
                         file_sha256=np.frombuffer(hashlib.sha256(open(extra, "rb").read()).digest(), np.uint8))
 
 
+def digest(a) -> str:
+    """SHA-256 of the float32 bit patterns: comparing digests is comparing every bit of the array."""
+    return hashlib.sha256(np.ascontiguousarray(a, np.float32).tobytes()).hexdigest()
+
+
+def gen_digests(tmp):
+    """ref_digests.json: what the reference computed in the tests that compare against it on inputs too large to store
+    (full-size layer shapes) -- the digest of every call's output and the greedy ids.  Each block replays the exact
+    inputs (files, seeds, schedules) of the test that reads it."""
+    import subprocess
+    out = {}
+    # tests/test_oracle.py::test_port_matches_live_reference
+    for shape, wt in [("tiny", ggjt.T_F32), ("tiny128", ggjt.T_F16), ("tiny3b", ggjt.T_Q8_0), ("tiny3b", ggjt.T_Q4_1)]:
+        path = os.path.join(tmp, "m.bin")
+        ggjt.write_synth_slice(path, ggjt.SHAPES[shape], 0, 1, wt, seed=3)
+        ref, rng = oracle.RefSlice(path, 3, 512), np.random.default_rng(5)
+        out["port/%s_%s" % (shape, ggjt.TYPE_NAME[wt])] = [
+            digest(ref.forward(rng.standard_normal((n, ggjt.SHAPES[shape].n_embd), dtype=np.float32))) for n in (34, 1, 2, 1)]
+        ref.close()
+    # tests/test_oracle.py::test_fast_q4_1_writer_files_are_valid_for_the_reference
+    sh = ggjt.SHAPES["tiny128"]
+    path = os.path.join(tmp, "fast_q4_1.bin")
+    ggjt.write_fast_q4_slice(path, sh, 0, 1, 0, wtype=ggjt.T_Q4_1)
+    ref, rng = oracle.RefSlice(path, 3, 512), np.random.default_rng(11)
+    out["fast_q4_1_writer"] = [digest(ref.forward(rng.standard_normal((n, sh.n_embd), dtype=np.float32))) for n in (20, 1, 1)]
+    ref.close()
+    # tests/test_ggjt_and_abi.py::test_q4_1_quantizer_is_the_reference_quantize_tool: the tool's Q4_1 tensors
+    sh = ggjt.SHAPES["tiny3b"]
+    full, fq = os.path.join(tmp, "f32.bin"), os.path.join(tmp, "q41.bin")
+    ggjt.write_synth_full(full, sh, ggjt.T_F32, seed=0)
+    subprocess.run([os.path.join(oracle.REF_DIR, "quantize"), full, fq, "q4_1"], check=True, capture_output=True)
+    b = ggjt.read_file(fq)
+    out["quantize_q4_1"] = {name: hashlib.sha256(b.read_raw(name)).hexdigest()
+                            for name, t in b.tensors.items() if t.ttype == ggjt.T_Q4_1}
+    # tests/test_gpu_llm_api.py::test_gpu_matches_live_reference
+    sh = ggjt.SHAPES["tiny128"]
+    path = os.path.join(tmp, "tiny128_q4_0_0_2_s5.bin")
+    ggjt.write_synth_slice(path, sh, 0, 2, ggjt.T_Q4_0, 5)
+    ref, rng = oracle.RefSlice(path, 3, 512), np.random.default_rng(8)
+    out["gpu_tiny128"] = [digest(ref.forward(rng.standard_normal((n, sh.n_embd), dtype=np.float32))) for n in (45, 1, 1, 1)]
+    ref.close()
+    # tests/test_gpu_full_size.py
+    threads = min(16, os.cpu_count() or 4)
+    sh = ggjt.SHAPES["3b"]
+    pa, pb, extra = (os.path.join(tmp, n) for n in ("a.bin", "b.bin", "extra.bin"))
+    ggjt.write_fast_q4_slice(pa, sh, 0, 16, seed=3)
+    ggjt.write_fast_q4_slice(pb, sh, 17, 25, seed=3)
+    ggjt.write_fast_q4_extra(extra, sh, seed=3)
+    refs = [oracle.RefSlice(pa, threads, 512), oracle.RefSlice(pb, threads, 512)]
+    toks, ids, hidden = [1 + (i * 7919) % 31999 for i in range(16)], [], []
+    for step in range(33):
+        y = oracle.ref_embed(extra, toks, sh.n_embd)
+        for s in refs:
+            y = s.forward(y)
+        hidden.append(digest(y))
+        toks = [oracle.ref_lib().ref_next_token(extra.encode(), y.ctypes.data, y.size)]
+        ids.append(toks[0])
+    out["config1"] = {"ids": ids, "hidden": hidden}
+    for s in refs:
+        s.close()
+    sh = ggjt.SHAPES["7b"]
+    p = os.path.join(tmp, "f16.bin")
+    ggjt.write_fast_f16_slice(p, sh, 0, 0, seed=4)
+    ref, rng = oracle.RefSlice(p, threads, 512), np.random.default_rng(9)
+    out["config4"] = [digest(ref.forward(rng.standard_normal((n, sh.n_embd), dtype=np.float32))) for n in (24, 1, 1, 9, 1)]
+    ref.close()
+    os.remove(p)
+    sh = ggjt.SHAPES["13b"]
+    p = os.path.join(tmp, "q4_13b.bin")
+    ggjt.write_fast_q4_slice(p, sh, 0, 0, seed=5)
+    refs, rng = [oracle.RefSlice(p, threads, 512) for _ in range(8)], np.random.default_rng(10)
+    prompt = [digest(refs[b].forward(rng.standard_normal((3 + 2 * b, sh.n_embd), dtype=np.float32))) for b in range(8)]
+    steps = []
+    for step in range(3):
+        x = rng.standard_normal((8, sh.n_embd), dtype=np.float32)
+        steps.append([digest(refs[b].forward(x[b:b + 1])[0]) for b in range(8)])
+    out["config5"] = {"prompt": prompt, "steps": steps}
+    for r in refs:
+        r.close()
+    sh = ggjt.SHAPES["7b"]
+    p = os.path.join(tmp, "q4_7b_2l.bin")
+    ggjt.write_fast_q4_slice(p, sh, 0, 1, seed=6)
+    ref, rng = oracle.RefSlice(p, threads, 512), np.random.default_rng(11)
+    chunks, pos = [], 0
+    while pos < 500:                     # the reference's arena caps a call at ~64 tokens
+        n = min(oracle.RefSlice.MAX_CHUNK, 500 - pos)
+        chunks.append([n, digest(ref.forward(rng.standard_normal((n, sh.n_embd), dtype=np.float32)))])
+        pos += n
+    out["config2"] = {"prefill": chunks,
+                      "decode": [digest(ref.forward(rng.standard_normal((1, sh.n_embd), dtype=np.float32))) for _ in range(500, 512)]}
+    ref.close()
+    json.dump(out, open(os.path.join(HERE, "ref_digests.json"), "w"), indent=1)
+
+
 def main():
     tmp = tempfile.mkdtemp()
     if sys.argv[1:] == ["q4_1"]:
         gen_q4_1(tmp)
+        return
+    if sys.argv[1:] == ["digests"]:
+        gen_digests(tmp)
         return
     gen_slices(tmp, CASES, "slices")
     gen_q4_1(tmp)

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 "fast mode" prefill (csrc/fastgemm.cuh) against exact mode.
+"""GPU: the wgmma "fast mode" prefill (csrc/fastgemm.cuh, csrc/fastgemm2.cuh) against exact mode.
 
 Fast mode is NOT bit-exact by design: the weight matmuls run as fp16 x fp16 -> fp32 tensor-core MMAs on operands
 that went through the reference's Q8_0 activation quantisation and one fp16 rounding each.  Stated tolerances:

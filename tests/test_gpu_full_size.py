@@ -1,11 +1,14 @@
-"""BASELINE.json's configurations at their FULL sizes, checked against the compiled reference itself (oracle/_ref,
-built from /root/reference by oracle/Makefile and shipped with the snapshot -- nothing here reads /root/reference).
+"""BASELINE.json's configurations at their FULL sizes, checked against what the compiled reference itself (oracle/_ref,
+built by oracle/Makefile) computed on the same files and inputs: tests/golden/ref_digests.json holds the SHA-256 of every
+output's float32 bits and the reference's greedy ids (tests/golden/gen_golden.py digests), so the comparison stays bit for bit.
 
   config 1  OpenLLaMA-3B shapes (n_embd 3200, d_head 100, n_ff 8640), two nodes: layers 0-16 / 17-25, single prompt,
             greedy decode: 16-token prompt + 32 generated tokens -- token ids AND hidden states bit-exact  (SURVEY 8d)
   config 4  LLaMA-7B F16 layer shapes at n_ctx 2048 (the reference is fixed at 512: compared on the positions it has)
   config 5  LLaMA-13B layer shapes, 8 sessions in one batched step vs the reference running each sequence alone
 Weights are synthetic (no network); the FILE is the ground truth both sides load."""
+import hashlib
+import json
 import os
 
 import numpy as np
@@ -14,22 +17,18 @@ import pytest
 from distributedllm_b200 import ggjt
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HAVE_REF = os.path.isfile(os.path.join(ROOT, "oracle", "_ref", "libllmref.so"))
-needs_ref = pytest.mark.skipif(not HAVE_REF, reason="compiled reference (oracle/_ref) not shipped")
-THREADS = min(16, os.cpu_count() or 4)
+REF = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_digests.json")))
+MAX_CHUNK = 32          # the reference's eval arena overflows for long calls (SURVEY 8a-Q3): its prefill went in these chunks
 
 
-def _bits(a):
-    return np.ascontiguousarray(a, dtype=np.float32).view(np.uint32)
+def _digest(a):
+    return hashlib.sha256(np.ascontiguousarray(a, dtype=np.float32).tobytes()).hexdigest()
 
 
-@needs_ref
 def test_config1_3b_two_nodes_greedy_decode(tmp_path):
     import sys
     from distributedllm_b200 import capi
     from distributedllm_b200.compute_node.slices import import_llm
-    from oracle import oracle
     llm = import_llm()
     sh = ggjt.SHAPES["3b"]
     pa, pb, extra = str(tmp_path / "a.bin"), str(tmp_path / "b.bin"), str(tmp_path / "extra.bin")
@@ -37,44 +36,36 @@ def test_config1_3b_two_nodes_greedy_decode(tmp_path):
     ggjt.write_fast_q4_slice(pb, sh, 17, 25, seed=3)
     ggjt.write_fast_q4_extra(extra, sh, seed=3)
     gpu = [capi.Slice(pa, 0, 512), capi.Slice(pb, 0, 512)]
-    ref = [oracle.RefSlice(pa, THREADS, 512), oracle.RefSlice(pb, THREADS, 512)]
     tokens = [1 + (i * 7919) % 31999 for i in range(16)]          # SURVEY 8d: token-level synthetic prompt
-    ids_gpu, ids_ref, bad = [], [], 0
-    tg, tr = list(tokens), list(tokens)
+    ids_gpu, bad_steps = [], []
+    tg = list(tokens)
     for step in range(33):
-        # GPU side: everything through the drop-in `llm` module + C ABI
+        # everything through the drop-in `llm` module + C ABI; the reference ran its own embedding lookup, slices and argmax
         x = np.array(llm.prepare_embeddings(extra, tg), np.float32).reshape(len(tg), sh.n_embd)
         for s in gpu:
             x = s.forward(x)
-        # reference side: its own embedding lookup, slices and argmax
-        y = oracle.ref_embed(extra, tr, sh.n_embd)
-        for s in ref:
-            y = s.forward(y)
-        bad += int((_bits(x) != _bits(y)).sum())
+        if _digest(x) != REF["config1"]["hidden"][step]:
+            bad_steps.append(step)
         a = llm.get_next_token(extra, x.ravel().tolist())
-        b = oracle.ref_lib().ref_next_token(extra.encode(), y.ctypes.data, y.size)
         ids_gpu.append(a)
-        ids_ref.append(b)
-        tg, tr = [a], [b]
-    assert ids_gpu == ids_ref
-    assert bad == 0, "%d hidden-state floats differ" % bad
+        tg = [a]
+    assert ids_gpu == REF["config1"]["ids"]
+    assert not bad_steps, "hidden states differ from the reference at steps %s" % bad_steps
     assert len(set(ids_gpu)) > 4                                   # the run is not degenerate
-    for s in gpu + ref:
+    for s in gpu:
         s.close()
 
 
-@needs_ref
 def test_config4_7b_f16_layer_at_n_ctx_2048(tmp_path):
     from distributedllm_b200 import capi
-    from oracle import oracle
     sh = ggjt.SHAPES["7b"]
     p = str(tmp_path / "f16.bin")
     ggjt.write_fast_f16_slice(p, sh, 0, 0, seed=4)
-    gpu, ref = capi.Slice(p, 0, 2048), oracle.RefSlice(p, THREADS, 512)
+    gpu = capi.Slice(p, 0, 2048)
     rng = np.random.default_rng(9)
-    for n in (24, 1, 1, 9, 1):
+    for i, n in enumerate((24, 1, 1, 9, 1)):
         x = rng.standard_normal((n, sh.n_embd), dtype=np.float32)
-        assert (_bits(gpu.forward(x)) == _bits(ref.forward(x))).all()
+        assert _digest(gpu.forward(x)) == REF["config4"][i], "call %d differs from the reference" % i
     # beyond the reference's 512 positions: the long context still runs and stays finite
     gpu.clear_context()
     x = rng.standard_normal((128, sh.n_embd), dtype=np.float32)
@@ -82,58 +73,49 @@ def test_config4_7b_f16_layer_at_n_ctx_2048(tmp_path):
         y = gpu.forward(x)
     assert gpu.n_past == 1280 and np.isfinite(y).all()
     gpu.close()
-    ref.close()
 
 
-@needs_ref
 def test_config5_13b_batch_of_8_sessions(tmp_path):
     from distributedllm_b200 import capi
-    from oracle import oracle
     sh = ggjt.SHAPES["13b"]
     p = str(tmp_path / "q4.bin")
     ggjt.write_fast_q4_slice(p, sh, 0, 0, seed=5)
     B = 8
     gpu = capi.Slice(p, 0, 512, n_sessions=B)
-    refs = [oracle.RefSlice(p, THREADS, 512) for _ in range(B)]
     rng = np.random.default_rng(10)
-    for b in range(B):
+    for b in range(B):                  # the reference ran each sequence alone, in its own context
         x = rng.standard_normal((3 + 2 * b, sh.n_embd), dtype=np.float32)
-        assert (_bits(gpu.session_forward(b, x)) == _bits(refs[b].forward(x))).all()
+        assert _digest(gpu.session_forward(b, x)) == REF["config5"]["prompt"][b], b
     for step in range(3):
         x = rng.standard_normal((B, sh.n_embd), dtype=np.float32)
         got = gpu.batch_forward(list(range(B)), x)
         for b in range(B):
-            assert (_bits(got[b]) == _bits(refs[b].forward(x[b:b + 1])[0])).all(), (step, b)
+            assert _digest(got[b]) == REF["config5"]["steps"][step][b], (step, b)
     gpu.close()
-    for r in refs:
-        r.close()
 
 
-@needs_ref
 def test_config2_7b_q4_decode_at_the_end_of_the_sequence(tmp_path):
     """The positions BASELINE's metric is quoted on: a 2-layer LLaMA-7B Q4_0 slice taken to p = 500 in prompt chunks,
     then decoded token by token at p = 500..511 (T up to 512 in attention: every staged-row / tail path of the decode
     kernels) -- hidden states bit-identical to the compiled reference at every step, including the chunked prefill."""
     from distributedllm_b200 import capi
-    from oracle import oracle
     sh = ggjt.SHAPES["7b"]
     p = str(tmp_path / "q4_7b_2l.bin")
     ggjt.write_fast_q4_slice(p, sh, 0, 1, seed=6)
-    gpu, ref = capi.Slice(p, 0, 512), oracle.RefSlice(p, THREADS, 512)
+    gpu = capi.Slice(p, 0, 512)
     rng = np.random.default_rng(11)
-    pos, bad = 0, 0
-    while pos < 500:                                               # the reference's arena caps a call at ~64 tokens
-        n = min(oracle.RefSlice.MAX_CHUNK, 500 - pos)
+    pos, bad = 0, []
+    for i, (n, want) in enumerate(REF["config2"]["prefill"]):     # the reference's prompt chunks
+        assert n == min(MAX_CHUNK, 500 - pos)
         x = rng.standard_normal((n, sh.n_embd), dtype=np.float32)
-        bad += int((_bits(gpu.forward(x)) != _bits(ref.forward(x))).sum())
+        if _digest(gpu.forward(x)) != want:
+            bad.append(i)
         pos += n
-    assert bad == 0, "%d floats differ in the chunked prefill" % bad
+    assert pos == 500 and not bad, "prefill chunks %s differ from the reference" % bad
     for pos in range(500, 512):
         x = rng.standard_normal((1, sh.n_embd), dtype=np.float32)
-        g, r = gpu.forward(x), ref.forward(x)
-        assert (_bits(g) == _bits(r)).all(), "decode step at position %d differs" % pos
+        assert _digest(gpu.forward(x)) == REF["config2"]["decode"][pos - 500], "decode step at position %d differs" % pos
     assert gpu.n_past == 512
     with pytest.raises(capi.B200Error):                            # position 512 does not exist at n_ctx 512
         gpu.forward(rng.standard_normal((1, sh.n_embd), dtype=np.float32))
     gpu.close()
-    ref.close()

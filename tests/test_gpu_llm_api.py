@@ -1,6 +1,5 @@
 """GPU: the reference-facing `llm` module, the resident extra layers, and the whole node/client stack with
-the slice forward on the B200 -- checked against goldens dumped from the reference (tests/golden) and, when the
-compiled reference travelled with the snapshot (oracle/_ref), against the live reference."""
+the slice forward on the H100 -- checked against goldens dumped from the reference (tests/golden)."""
 import gzip
 import io
 import json
@@ -168,19 +167,19 @@ def test_node_end_to_end_greedy_decode_matches_cpu_path(llm, tmp_path):
         llm.unload_slice()
 
 
-@pytest.mark.skipif(not os.path.isfile(os.path.join(os.path.dirname(os.path.dirname(__file__)), "oracle", "_ref", "libllmref.so")),
-                    reason="compiled reference (oracle/_ref) not shipped")
 def test_gpu_matches_live_reference(tmp_models):
+    """Hidden states against the compiled reference's outputs on the same file and inputs, kept as digests of their bits
+    (tests/golden/ref_digests.json) so the check runs without the reference sources."""
+    import hashlib
     from distributedllm_b200 import capi
-    from oracle import oracle
+    want = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "ref_digests.json")))["gpu_tiny128"]
     sh = ggjt.SHAPES["tiny128"]
     path = tmp_models("tiny128", ggjt.T_Q4_0, 0, 2, seed=5)
-    ref, gpu = oracle.RefSlice(path, 3, 512), capi.Slice(path, 0, 512)
+    gpu = capi.Slice(path, 0, 512)
     rng = np.random.default_rng(8)
-    for n in (45, 1, 1, 1):
+    for i, n in enumerate((45, 1, 1, 1)):
         x = rng.standard_normal((n, sh.n_embd), dtype=np.float32)
-        assert (_bits(ref.forward(x)) == _bits(gpu.forward(x))).all()
-    ref.close()
+        assert hashlib.sha256(_bits(gpu.forward(x)).tobytes()).hexdigest() == want[i], "call %d differs from the reference" % i
     gpu.close()
 
 

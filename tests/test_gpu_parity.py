@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a slice forward, called through the C ABI, against the CPU oracle.
+"""GPU parity: the sm_90a slice forward, called through the C ABI, against the CPU oracle.
 
 Bar (SURVEY.md Appendix B, "exact mode"): hidden states BIT-IDENTICAL to the reference CPU path
 for every weight type the slice path supports -- not a tolerance."""

@@ -2,7 +2,7 @@
 INTEGRATION.md section 1, on real hardware.
 
 `oracle/_ref/py/distllm` is a build output of oracle/Makefile (the reference's distllm/*.py copied next to the compiled
-reference; git-ignored, it travels with the snapshot -- nothing here reads /root/reference).  With
+reference; git-ignored, the tests skip without it -- nothing here reads the reference checkout).  With
 `distributedllm_b200/` first on sys.path, `import llm` inside the reference's code binds to csrc/llm_module.cpp:
 
   * distllm.compute_node.slices.GGMLSlice (slices.py:74-91)          llm.load_slice / propagate_forward / clear_context
