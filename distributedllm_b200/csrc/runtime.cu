@@ -68,6 +68,7 @@ struct b200_slice {
     int64_t launches = 0, weight_bytes = 0;
     bool use_ring = true, use_graph = true, use_pdl = false, use_nq = true, f16_ring = true, use_tiled_attn = true, use_n8 = false, f16_mc = true; int f16_mc_cols = 4;
     bool skip_attention = false;   // measurement aid: replay only the weight matmuls of a step (bench.py roofline)
+    bool attn_lut_smem = true;     // single-token attention stages the exp table in shared memory (decided at load)
     bool fast_prefill = false; int fast_min_tokens = 32; uint16_t * xh = nullptr;   // tensor-core prefill (fast mode)
     int fast_version = 2;                                                               // 2: fastgemm2.cuh (TMA tensor map, N = 256), 1: fastgemm.cuh
     int opt_ns = 0, opt_cta_per_sm = 0, opt_nc = 0, opt_pre = 3, opt_nomath = 0;   // read once at load (environment)
@@ -587,8 +588,8 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
                 s->cur_class = 2;
                 aa.n0 = 0;
                 if (s->trace && s->trace_next < 512) { aa.trace = s->trace + (size_t) s->trace_next * 1024 * 8; s->trace_next++; s->trace_cls.push_back(2); s->trace_ctas.push_back(4 * H); }
-                aa.lut_smem = 1;
-                if ((rc = launch_simple(s, k_attn128<true>, dim3(4 * H, 1, 1), dim3(256, 1, 1), asm_lut, aa))) return rc;
+                aa.lut_smem = s->attn_lut_smem;
+                if ((rc = launch_simple(s, k_attn128<true>, dim3(4 * H, 1, 1), dim3(256, 1, 1), aa.lut_smem ? asm_lut : asm_bytes, aa))) return rc;
             } else if (s->use_tiled_attn && s->past[s->cur] + N <= kAttnTMax) {
                 // prompt chunk whose whole context fits the staged window: query-tiled kernel, K / V read once per 16 queries
                 s->cur_class = 1;
@@ -1032,6 +1033,7 @@ static int load_locked(b200_slice * s, const char * path) {
     s->E = (int) f.n_embd; s->H = (int) f.n_head; s->D = s->E / s->H; s->L = (int) f.n_layer; s->first_layer = (int) f.first_layer;
     s->FF = (int)(((2 * (4 * f.n_embd) / 3 + f.n_mult - 1) / f.n_mult) * f.n_mult);   // tensor_processor.cpp:1250
     if (s->D > 128 || (s->D & 1)) return fail(B200_EFILE, "head size %d unsupported (<=128, even)", s->D);
+    size_t attn_smem = 0;                           // dynamic shared memory of the single-token attention kernel
     {
         // worst-case dynamic shared memory of the attention kernels at this n_ctx (scores f32 + probabilities f16 per
         // position, + staged rows / exp table / partials): reject the load instead of failing every forward later
@@ -1044,6 +1046,7 @@ static int load_locked(b200_slice * s, const char * path) {
             return fail(B200_EINVAL, "n_ctx %d needs %zu B of attention shared memory (limit %zu B): largest supported n_ctx for head size %d is %d",
                         s->n_ctx, need, limit, s->D, s->D == 128 ? (int)((limit - 2 * 128 * kAttnRow - 32 * 64 - 64 - 65536 - 16) / 6) & ~31
                                                                  : (int)((limit - (size_t) 4 * s->D * 32 - 64) / 6) & ~31);
+        attn_smem = need;
     }
     const uint32_t E = f.n_embd, FF = (uint32_t) s->FF;
     s->layers.resize(s->L);
@@ -1146,6 +1149,19 @@ static int load_locked(b200_slice * s, const char * path) {
     B200_CUDA(cudaFuncSetAttribute(k_attention, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
     B200_CUDA(cudaFuncSetAttribute(k_attn128<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     B200_CUDA(cudaFuncSetAttribute(k_attn128<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    if (s->D == 128) {
+        // The single-token attention runs one 4-CTA cluster per head, and each cluster can start only on four free SMs of
+        // one GPC.  With the exp table's 64 KB staged in shared memory a CTA takes most of an SM, and a device may hold
+        // fewer clusters than there are heads (H100 SXM, 7B: 30 of 32): the rest wait for a whole second wave, every
+        // layer.  Then the table is read through L2 instead (the same entries, so the same results).
+        cudaLaunchConfig_t cfg{};
+        cfg.gridDim = dim3(4 * s->H, 1, 1); cfg.blockDim = dim3(256, 1, 1); cfg.dynamicSmemBytes = attn_smem;
+        int clusters = 0;
+        B200_CUDA(cudaOccupancyMaxActiveClusters(&clusters, k_attn128<true>, &cfg));
+        s->attn_lut_smem = clusters >= s->H;
+        if (ltrace) fprintf(stderr, "[b200 load] single-token attention: %d of %d clusters resident with the exp table in shared memory: %s\n",
+                            clusters, s->H, s->attn_lut_smem ? "staged" : "read through L2");
+    }
     B200_CUDA(cudaEventCreate(&s->ev0));
     B200_CUDA(cudaEventCreate(&s->ev1));
     B200_CUDA(cudaDeviceSynchronize());
