@@ -14,7 +14,7 @@
 
 namespace b200 {
 
-enum GgmlType : uint32_t { GT_F32 = 0, GT_F16 = 1, GT_Q4_0 = 2, GT_Q4_1 = 3, GT_Q8_0 = 8, GT_Q6_K = 14 };
+enum GgmlType : uint32_t { GT_F32 = 0, GT_F16 = 1, GT_Q4_0 = 2, GT_Q4_1 = 3, GT_Q5_0 = 6, GT_Q5_1 = 7, GT_Q8_0 = 8, GT_Q6_K = 14 };
 
 struct GgjtTensor {
     std::string name;
@@ -38,6 +38,8 @@ struct GgjtFile {
             case GT_F16:  return nelem * 2;
             case GT_Q4_0: return nelem / 32 * 18;
             case GT_Q4_1: return nelem / 32 * 20;
+            case GT_Q5_0: return nelem / 32 * 22;
+            case GT_Q5_1: return nelem / 32 * 24;
             case GT_Q8_0: return nelem / 32 * 34;
             case GT_Q6_K: return nelem / 256 * 210;
             default: throw std::runtime_error("unrecognized tensor type " + std::to_string(type));

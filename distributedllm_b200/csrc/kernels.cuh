@@ -30,18 +30,55 @@ namespace b200 {
 // Q4_1 chunk (640 B = 20 B/block): the Q4_0 shape with the nibbles left UNSIGNED (0..15, no XOR) + 64 B of fp16 minima
 //       at 576 + 8*r.  ggml_vec_dot_q4_1_q8_1 (ggml.c:2700-2733): acc_l = fma(d0*d1, float(sum n*a), acc_l) with an
 //       f32 (unrounded) activation scale d1, plus a SCALAR chain summs += m * s (s = d1 * sum of the block's quants).
-// A warp reads a chunk with one conflict-free LDS.128 (+ one LDS.64) per lane.
+// Q5_0 chunk (704 B = 22 B/block): 512 B of file nibbles (unchanged, no XOR), 128 B of high bits, 64 B of fp16 d at 640 + 8*r.
+//       High-bit word of lane L = 4*r + w: byte bq = bits 4w..4w+3 of block 4q+bq's qh (lane w) in its low nibble and
+//       bits 16+4w..16+4w+3 (lane w+4) in its high nibble.  `(b * 0x10204080) & 0x80808080` spreads 4 bits b to bit 7
+//       of each byte; `(n<<3 | h<<7) ^ 0x80` is then 8*(n + 16h - 16) as a signed byte (the 1/8 is folded into the
+//       activation scale).  ggml_vec_dot_q5_0_q8_0 (ggml.c:2914-2936) has Q4_0's chain.
+// Q5_1 chunk (768 B = 24 B/block): the Q5_0 shape without the XOR (8*(n + 16h), unsigned) + 64 B of fp16 minima at
+//       704 + 8*r.  ggml_vec_dot_q5_1_q8_1 (ggml.c:3164-3189) has Q4_1's chain.
+// A warp reads a chunk with one conflict-free LDS.128 (+ one LDS.64, + one LDS.32 of high bits) per lane.
 // =============================================================================================
-constexpr int kWT_F16 = 1, kWT_Q4_0 = 2, kWT_Q4_1 = 3, kWT_Q8_0 = 8;
-constexpr int kQ4Chunk = 576, kQ41Chunk = 640, kQ8Chunk = 1088;
+constexpr int kWT_F16 = 1, kWT_Q4_0 = 2, kWT_Q4_1 = 3, kWT_Q5_0 = 6, kWT_Q5_1 = 7, kWT_Q8_0 = 8;
+constexpr int kQ4Chunk = 576, kQ41Chunk = 640, kQ50Chunk = 704, kQ51Chunk = 768, kQ8Chunk = 1088;
 constexpr int kWPC = 4;                 // consumer warps per CTA (8 rows x G groups each)
 constexpr int kConsumers = kWPC * 32;
 constexpr int kQS = 4;                  // quads per ring stage (nbq is padded to a multiple of kQS at pack time)
 constexpr float kMagic = 12582912.0f;   // 1.5 * 2^23: int->float through the dp4a accumulator
 constexpr int kMagicI = 0x4B400000;
 
-__host__ __device__ constexpr int chunk_bytes(int wt) { return wt == kWT_Q4_0 ? kQ4Chunk : (wt == kWT_Q4_1 ? kQ41Chunk : kQ8Chunk); }
-__host__ __device__ constexpr bool wt_nibbles(int wt) { return wt == kWT_Q4_0 || wt == kWT_Q4_1; }
+// The per-type facts of the block-quantised weight types, read by every dispatch site (an unknown type is not Q8_0).
+struct WtTraits {
+    int block_bytes;       // file bytes per 32-weight block
+    int chunk_bytes;       // packed bytes per chunk (8 rows x 4 blocks) = 32 * block_bytes
+    bool is_signed;        // packed weight bytes are signed (dp4a.s32.s32) or unsigned (dp4a.u32.s32)
+    bool min_plane;        // fp16 minima (Q4_1 / Q5_1: the scalar summs chain)
+    bool high_plane;       // 128 B of fifth bits (Q5_x)
+    bool q8_1;             // activations are Q8_1 (f32 scale + block-sum plane) instead of Q8_0
+    float act_scale;       // folded into the activation scale: 1 / (weight-byte scale of the packed form)
+};
+__host__ __device__ constexpr WtTraits wt_traits(int wt) {
+    return wt == kWT_Q4_0 ? WtTraits{18, kQ4Chunk, true, false, false, false, 0.0625f}
+         : wt == kWT_Q4_1 ? WtTraits{20, kQ41Chunk, false, true, false, true, 0.0625f}
+         : wt == kWT_Q5_0 ? WtTraits{22, kQ50Chunk, true, false, true, false, 0.125f}
+         : wt == kWT_Q5_1 ? WtTraits{24, kQ51Chunk, false, true, true, true, 0.125f}
+         : wt == kWT_Q8_0 ? WtTraits{34, kQ8Chunk, true, false, false, false, 1.0f}
+         :                  WtTraits{0, 0, false, false, false, false, 0.0f};
+}
+__host__ __device__ constexpr bool wt_block_quant(int wt) { return wt_traits(wt).block_bytes != 0; }
+__host__ __device__ constexpr int chunk_bytes(int wt) { return wt_traits(wt).chunk_bytes; }
+__host__ __device__ constexpr bool wt_nibbles(int wt) { return wt == kWT_Q4_0 || wt == kWT_Q4_1 || wt == kWT_Q5_0 || wt == kWT_Q5_1; }
+__host__ __device__ constexpr bool wt_q8_1(int wt) { return wt_traits(wt).q8_1; }
+__host__ __device__ constexpr float wt_act_scale(int wt) { return wt_traits(wt).act_scale; }
+// byte offsets inside a chunk: nibbles / Q8_0 quants at 0, high bits at 512, then the scales, then the minima
+__host__ __device__ constexpr int wt_scale_off(int wt) { return wt == kWT_Q8_0 ? 1024 : (wt_traits(wt).high_plane ? 640 : 512); }
+__host__ __device__ constexpr int wt_min_off(int wt) { return wt_scale_off(wt) + 64; }
+static_assert(chunk_bytes(kWT_Q4_0) == 32 * 18 && chunk_bytes(kWT_Q4_1) == 32 * 20 && chunk_bytes(kWT_Q5_0) == 32 * 22 &&
+              chunk_bytes(kWT_Q5_1) == 32 * 24 && chunk_bytes(kWT_Q8_0) == 32 * 34, "a chunk holds the file's bytes, nothing added");
+static_assert(kQ50Chunk % 16 == 0 && kQ51Chunk % 16 == 0, "a ring stage stays one bulk copy");
+
+// 4 bits b -> bit i at bit 8i+7 (no carries: the partial products never overlap)
+__device__ __forceinline__ uint32_t spread4_hi(uint32_t b) { return (b * 0x10204080u) & 0x80808080u; }
 
 struct PackedW {
     const uint8_t * data;
@@ -72,10 +109,41 @@ __global__ void k_repack(RepackArgs a) {
         if (a.mode == 1)      { const int gps = a.rows_per_src / 8; s = gi / gps; sg = gi % gps; }
         else if (a.mode == 2) { s = gi & 1; sg = gi >> 1; }
         else                  { s = 0; sg = gi; }
-        const int bsz = a.wtype == kWT_Q4_0 ? 18 : (a.wtype == kWT_Q4_1 ? 20 : 34);
+        const int bsz = wt_traits(a.wtype).block_bytes;
         uint32_t out = 0;
         const bool src_ok = s < 3 && a.src[s] != nullptr;
-        if (wt_nibbles(a.wtype)) {
+        if (wt_traits(a.wtype).high_plane) {                 // Q5_0 / Q5_1: [fp16 d][Q5_1: fp16 m][u8 qh[4]][u8 qs[16]]
+            const bool q51 = a.wtype == kWT_Q5_1;
+            const int qh_off = q51 ? 4 : 2, qs_off = qh_off + 4;
+            if (wi < 128) {                                  // nibble words, as the file stores them
+                const int lane = wi >> 2, bq = wi & 3, r = lane >> 2, w = lane & 3;
+                const int row = sg * 8 + r, b = q * 4 + bq;
+                if (src_ok && row < a.rows_per_src && b < a.nb) {
+                    const uint16_t * p = (const uint16_t *)(a.src[s] + ((long long) row * a.nb + b) * bsz + qs_off + 4 * w);
+                    out = (uint32_t) p[0] | ((uint32_t) p[1] << 16);
+                }
+            } else if (wi < 160) {                           // high-bit word of lane L = 4r + w: one byte per block
+                const int lane = wi - 128, r = lane >> 2, w = lane & 3, row = sg * 8 + r;
+                for (int bq = 0; bq < 4; bq++) {
+                    const int b = q * 4 + bq;
+                    if (src_ok && row < a.rows_per_src && b < a.nb) {
+                        const uint16_t * p = (const uint16_t *)(a.src[s] + ((long long) row * a.nb + b) * bsz + qh_off);
+                        const uint32_t qh = (uint32_t) p[0] | ((uint32_t) p[1] << 16);
+                        out |= (((qh >> (4 * w)) & 15u) | (((qh >> (16 + 4 * w)) & 15u) << 4)) << (8 * bq);
+                    }
+                }
+            } else {                                         // scales, then Q5_1 minima: 16 words = 8 rows x 4 halves
+                const int sel = (wi - 160) >> 4;             // 0: d at +0, 1: m at +2
+                const int h0 = ((wi - 160) & 15) * 2;
+                uint32_t v[2] = {0, 0};
+                for (int k = 0; k < 2; k++) {
+                    const int r = (h0 + k) >> 2, bq = (h0 + k) & 3, row = sg * 8 + r, b = q * 4 + bq;
+                    if (src_ok && row < a.rows_per_src && b < a.nb)
+                        v[k] = *(const uint16_t *)(a.src[s] + ((long long) row * a.nb + b) * bsz + 2 * sel);
+                }
+                out = v[0] | (v[1] << 16);
+            }
+        } else if (wt_nibbles(a.wtype)) {
             const bool q41 = a.wtype == kWT_Q4_1;
             if (wi < 128) {                                  // nibble words
                 const int lane = wi >> 2, bq = wi & 3, r = lane >> 2, w = lane & 3;
@@ -196,7 +264,7 @@ struct GemvArgs {
     const float * x;      int ldx;       // PRO_PLAIN / PRO_NORM: input [N][ldx], K valid per row
     const float * norm_w;                // PRO_NORM: weight [K]
     const int * aq_in; const float * da_in;   // PRO_PREQ: pre-quantised input, [N][nbq*32] words + [N][nbq*4] scales
-    int in_soff, out_soff;               // Q4_1 weights (Q8_1 activations): the block sums s live in a second plane, this many
+    int in_soff, out_soff;               // Q4_1 / Q5_1 weights (Q8_1 activations): the block sums s live in a second plane, this many
                                          // floats behind the scales (da_in / da_out); 0 for Q8_0 activations
     const float * resid;  int ldr;       // EPI_RESID
     float * y;            int ldy;       // output [N][ldy]
@@ -214,7 +282,7 @@ struct GemvArgs {
     uint2 * mb_peer_inbox; size_t mb_slot_elems;   // EPI_RESID_SEND: next rank's inbox (mapped peer memory), elements per slot
 };
 
-__host__ __device__ inline size_t act_bytes_per_col(int nbq, int wt) { return (size_t) nbq * (128 + 16 + (wt == kWT_Q4_1 ? 16 : 0)); }
+__host__ __device__ inline size_t act_bytes_per_col(int nbq, int wt) { return (size_t) nbq * (128 + 16 + (wt_q8_1(wt) ? 16 : 0)); }
 
 
 // (double) of a NON-NEGATIVE float, bit-exact, on the integer pipes: F2F.F64.F32 runs on the quarter-rate XU pipe and
@@ -262,17 +330,18 @@ __device__ __forceinline__ void warp_quant_block(float v, int lane, int * aq_col
 
 // quantise one 32-float block held in registers by ONE thread into shared memory
 // `rot`: v[4*w8 .. 4*w8+3] holds 16-byte chunk (w8 + rot) & 7 of the block (bank-conflict-free rotated smem reads)
-// WT == Q4_1: Q8_1 (f32 scale, block sum s into sn[b]); otherwise Q8_0.
+// wt_q8_1(WT) (Q4_1, Q5_1): Q8_1 (f32 scale, block sum s into sn[b]); otherwise Q8_0.
 template <int WT>
 __device__ __forceinline__ void thread_quant_block(const float (&v)[32], int * an, float * dn, int b, int rot = 0, float * sn = nullptr) {
+    constexpr bool Q81 = wt_q8_1(WT);
     float m[8];
     #pragma unroll
     for (int j = 0; j < 8; j++) m[j] = fmaxf(fmaxf(fabsf(v[j]), fabsf(v[j + 8])), fmaxf(fabsf(v[j + 16]), fabsf(v[j + 24])));
     const float amax = fmaxf(fmaxf(fmaxf(m[0], m[1]), fmaxf(m[2], m[3])), fmaxf(fmaxf(m[4], m[5]), fmaxf(m[6], m[7])));
     const float dq = __fdiv_rn(amax, 127.f);
-    const float d = (WT == kWT_Q4_1) ? dq : h2f(f2h(dq));
+    const float d = Q81 ? dq : h2f(f2h(dq));
     const float id = amax != 0.f ? __fdiv_rn(127.f, amax) : 0.f;
-    dn[b] = wt_nibbles(WT) ? fmul(d, 0.0625f) : d;          // the 1/16 of the nibble placement, folded (exact)
+    dn[b] = wt_nibbles(WT) ? fmul(d, wt_act_scale(WT)) : d; // the 1/16 (1/8 for Q5_x) of the weight-byte placement, folded (exact)
     int * dst = an + (b >> 2) * 32 + (b & 3) * 2;
     int qsum = 0;
     #pragma unroll
@@ -281,19 +350,21 @@ __device__ __forceinline__ void thread_quant_block(const float (&v)[32], int * a
         #pragma unroll
         for (int j = 0; j < 4; j++) {
             const int qv = rint_small(fmul(v[w*4 + j], id));
-            if (WT == kWT_Q4_1) qsum += qv;
+            if (Q81) qsum += qv;
             pk |= ((uint32_t)(qv & 0xFF)) << (8 * j);
         }
         const int ww = (w + rot) & 7;
         dst[(ww & 3) * 8 + (ww >> 2)] = (int) pk;
     }
-    if (WT == kWT_Q4_1) sn[b] = fmul(d, (float) qsum);
+    if (Q81) sn[b] = fmul(d, (float) qsum);
 }
 
 template <int WT, int G, int NC, int PRO, int EPI, bool RING>
 __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
     constexpr int CB = chunk_bytes(WT);
-    constexpr bool Q41 = WT == kWT_Q4_1;
+    constexpr bool Q41 = wt_q8_1(WT);                 // Q8_1 activations + the scalar min chain (Q4_1, Q5_1)
+    constexpr bool Q5 = wt_traits(WT).high_plane;
+    constexpr int SOFF = wt_scale_off(WT), MOFF = wt_min_off(WT);
     constexpr int TR = kWPC * G;
     extern __shared__ __align__(128) uint8_t smem[];
     const int nbq = a.W.nbq, K = a.W.K, nb = a.W.nb;
@@ -525,14 +596,15 @@ __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
             #pragma unroll
             for (int qi = 0; qi < kQS; qi++) {
                 const int Q = s * kQS + qi;
-                uint4 wv[G], wv2[G]; uint2 sc[G], mc[G];
+                uint4 wv[G], wv2[G]; uint2 sc[G], mc[G]; uint32_t hw[G];
                 #pragma unroll
                 for (int g = 0; g < G; g++) {
                     const uint8_t * ch = base + (size_t)(qi * TR + g) * CB;
                     wv[g] = *(const uint4 *)(ch + lane * 16);
-                    if (WT == kWT_Q8_0) { wv2[g] = *(const uint4 *)(ch + 512 + lane * 16); sc[g] = *(const uint2 *)(ch + 1024 + r * 8); }
-                    else sc[g] = *(const uint2 *)(ch + 512 + r * 8);
-                    mc[g] = Q41 ? *(const uint2 *)(ch + 576 + r * 8) : make_uint2(0u, 0u);
+                    if (WT == kWT_Q8_0) wv2[g] = *(const uint4 *)(ch + 512 + lane * 16);
+                    sc[g] = *(const uint2 *)(ch + SOFF + r * 8);
+                    mc[g] = Q41 ? *(const uint2 *)(ch + MOFF + r * 8) : make_uint2(0u, 0u);
+                    hw[g] = Q5 ? *(const uint32_t *)(ch + 512 + lane * 4) : 0u;
                 }
                 #pragma unroll
                 for (int n = 0; n < NC; n++) {
@@ -559,12 +631,20 @@ __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
                                 // summs += fp16->f32(m) * s first (ggml.c:2712), then the lane fma: two independent chains
                                 const uint16_t mh = (uint16_t)(mw[bq >> 1] >> (16 * (bq & 1)));
                                 summ[g][n] = fadd(summ[g][n], fmul(h2f(mh), sa[bq]));
-                                const uint32_t lo = (ww[bq] << 4) & 0xF0F0F0F0u, hi = ww[bq] & 0xF0F0F0F0u;
+                                uint32_t lo, hi;
+                                if (Q5) {                                  // 8 * (n | h << 4), unsigned
+                                    lo = ((ww[bq] << 3) & 0x78787878u) | spread4_hi((hw[g] >> (8 * bq)) & 15u);
+                                    hi = ((ww[bq] >> 1) & 0x78787878u) | spread4_hi((hw[g] >> (8 * bq + 4)) & 15u);
+                                } else { lo = (ww[bq] << 4) & 0xF0F0F0F0u; hi = ww[bq] & 0xF0F0F0F0u; }
                                 f0 = fadd(__int_as_float(dp4a_us(lo, alo[bq], kMagicI)), -kMagic);
                                 f1 = fadd(__int_as_float(dp4a_us(hi, ahi[bq], kMagicI)), -kMagic);
                             } else {
                                 int lo, hi;
                                 if (WT == kWT_Q4_0) { lo = (int)((ww[bq] << 4) & 0xF0F0F0F0u); hi = (int)(ww[bq] & 0xF0F0F0F0u); }
+                                else if (Q5) {                             // 8 * (n | h << 4) - 128 = 8 * (q - 16), signed
+                                    lo = (int)(((ww[bq] << 3) & 0x78787878u) | (spread4_hi((hw[g] >> (8 * bq)) & 15u) ^ 0x80808080u));
+                                    hi = (int)(((ww[bq] >> 1) & 0x78787878u) | (spread4_hi((hw[g] >> (8 * bq + 4)) & 15u) ^ 0x80808080u));
+                                }
                                 else                { lo = (int) ww[bq]; hi = (int) ww2[bq]; }
                                 f0 = fadd(__int_as_float(__dp4a(lo, alo[bq], kMagicI)), -kMagic);
                                 f1 = fadd(__int_as_float(__dp4a(hi, ahi[bq], kMagicI)), -kMagic);
@@ -838,8 +918,8 @@ __global__ void __launch_bounds__(kN8Consumers + 32) k_gemv_n8(const GemvArgs a)
 // =============================================================================================
 struct NormQuantArgs {
     const float * x; int ldx; const float * norm_w; int K;
-    int * aq; float * da; int nbq;            // [N][nbq*32] words, [N][nbq*4] scales (x 1/16 for Q4_0 / Q4_1 weights)
-    int soff;                                 // Q4_1: block sums s at da + soff
+    int * aq; float * da; int nbq;            // [N][nbq*32] words, [N][nbq*4] scales (x wt_act_scale)
+    int soff;                                 // Q4_1 / Q5_1: block sums s at da + soff
 };
 
 template <int WT>
@@ -1419,7 +1499,7 @@ struct Attn128Args {
     const float2 * cs; const uint16_t * texp;
     float * out;                  // [N][E]
     int * aq_out; float * da_out; int out_nbq; float out_dscale;   // optional: Q8_0-quantised output for the wo matmul
-    int out_soff;                                                    // Q4_1 weights: Q8_1 instead, block sums at da_out + out_soff
+    int out_soff;                                                    // Q4_1 / Q5_1 weights: Q8_1 instead, block sums at da_out + out_soff
     int n_ctx; float kq_scale;
     unsigned long long * trace;
     const int2 * cols; size_t sess_stride;   // batched step (FUSE only): column n = (session, position); each column is an N = 1 step

@@ -250,9 +250,14 @@ static int launch_gemv_nc(b200_slice * s, const GemvArgs & a) {
 
 template <int G, int PRO, int EPI>
 static int launch_gemv(b200_slice * s, const GemvArgs & a) {
-    if (a.W.wtype == kWT_Q4_0) return launch_gemv_nc<kWT_Q4_0, G, PRO, EPI>(s, a);
-    if (a.W.wtype == kWT_Q4_1) return launch_gemv_nc<kWT_Q4_1, G, PRO, EPI>(s, a);
-    return launch_gemv_nc<kWT_Q8_0, G, PRO, EPI>(s, a);
+    switch (a.W.wtype) {
+    case kWT_Q4_0: return launch_gemv_nc<kWT_Q4_0, G, PRO, EPI>(s, a);
+    case kWT_Q4_1: return launch_gemv_nc<kWT_Q4_1, G, PRO, EPI>(s, a);
+    case kWT_Q5_0: return launch_gemv_nc<kWT_Q5_0, G, PRO, EPI>(s, a);
+    case kWT_Q5_1: return launch_gemv_nc<kWT_Q5_1, G, PRO, EPI>(s, a);
+    case kWT_Q8_0: return launch_gemv_nc<kWT_Q8_0, G, PRO, EPI>(s, a);
+    default: return fail(B200_EINVAL, "no block-quantised matmul for weight type %d", a.W.wtype);
+    }
 }
 
 template <typename K, typename A>
@@ -340,9 +345,14 @@ static int launch_f16(b200_slice * s, GemvF16Args a) {
 
 static int launch_norm_quant(b200_slice * s, const float * x, int ldx, const float * norm_w, int N) {
     NormQuantArgs q{x, ldx, norm_w, s->E, s->aq_x, s->da_x, s->nbqE, s->soffE};
-    if (s->wtype == kWT_Q4_0) return launch_simple(s, k_norm_quant<kWT_Q4_0>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
-    if (s->wtype == kWT_Q4_1) return launch_simple(s, k_norm_quant<kWT_Q4_1>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
-    return launch_simple(s, k_norm_quant<kWT_Q8_0>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
+    switch (s->wtype) {
+    case kWT_Q4_0: return launch_simple(s, k_norm_quant<kWT_Q4_0>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
+    case kWT_Q4_1: return launch_simple(s, k_norm_quant<kWT_Q4_1>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
+    case kWT_Q5_0: return launch_simple(s, k_norm_quant<kWT_Q5_0>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
+    case kWT_Q5_1: return launch_simple(s, k_norm_quant<kWT_Q5_1>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
+    case kWT_Q8_0: return launch_simple(s, k_norm_quant<kWT_Q8_0>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
+    default: return fail(B200_EINVAL, "no activation quantiser for weight type %d", s->wtype);
+    }
 }
 
 // ---------------------------------------------------------------- fast-mode prefill (wgmma), see fastgemm.cuh
@@ -482,7 +492,7 @@ static int launch_persistent(b200_slice * s, const float * in, float * out) {
     a.n_past = s->d_npast + s->cur;
     a.qkv = s->qkv; a.att = s->att; a.ffin = s->ffin;
     a.aq_att = s->aq_att; a.da_att = s->da_att; a.aq_gate = s->aq_gate; a.da_gate = s->da_gate;
-    a.dscale = s->wtype == kWT_Q4_0 ? 0.0625f : 1.0f;
+    a.dscale = wt_act_scale(s->wtype);
     a.cs = s->cs; a.texp = s->texp; a.tsilu = s->tsilu;
     a.cnt = s->p_cnt;
     a.kq_scale = 1.0f / sqrtf((float) s->E / (float) s->H);
@@ -574,7 +584,7 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
             aa.cs = s->cs; aa.texp = s->texp; aa.out = s->att;
             aa.n_ctx = s->n_ctx; aa.kq_scale = 1.0f / sqrtf((float) E / (float) H);
             const bool preq = s->wtype != kWT_F16;
-            const float dsc = wt_nibbles(s->wtype) ? 0.0625f : 1.0f;
+            const float dsc = wt_act_scale(s->wtype);
             if (preq) { aa.aq_out = s->aq_att; aa.da_out = s->da_att; aa.out_nbq = s->nbqE; aa.out_dscale = dsc; aa.out_soff = s->soffE; }
             if (s->cols) {
                 // every column is an independent N = 1 step: the fused (RoPE + append) kernel, one cluster row per column
@@ -652,7 +662,7 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
             if ((rc = launch_prep<false>(s, s->gate, FF, nullptr, FF, N))) return rc;
             if ((rc = launch_fast_any<FG_RESID>(s, Lw.w2, s->ffin, E, nxt, E, N, E))) return rc;
         } else {
-            const float dsc = wt_nibbles(s->wtype) ? 0.0625f : 1.0f;
+            const float dsc = wt_act_scale(s->wtype);
             s->cur_class = 3;
             GemvArgs o{}; o.W = Lw.wo; o.x = s->att; o.ldx = E; o.resid = cur; o.ldr = E; o.y = s->ffin; o.ldy = E;
             o.N = N; o.out_rows = E; o.tsilu = s->tsilu; o.aq_in = s->aq_att; o.da_in = s->da_att; o.in_soff = s->soffE; o.out_soff = s->soffE;
@@ -688,7 +698,10 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
                 if (gemv8_applicable(s, Lw.w2, N)) rc = launch_gemv8<EPI_RESID_SEND>(s, w);
                 else if (s->wtype == kWT_Q4_0) rc = launch_gemv_t<kWT_Q4_0, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
                 else if (s->wtype == kWT_Q4_1) rc = launch_gemv_t<kWT_Q4_1, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
-                else                           rc = launch_gemv_t<kWT_Q8_0, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
+                else if (s->wtype == kWT_Q5_0) rc = launch_gemv_t<kWT_Q5_0, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
+                else if (s->wtype == kWT_Q5_1) rc = launch_gemv_t<kWT_Q5_1, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
+                else if (s->wtype == kWT_Q8_0) rc = launch_gemv_t<kWT_Q8_0, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
+                else rc = fail(B200_EINVAL, "no pipelined matmul for weight type %d", s->wtype);
                 if (rc) return rc;
             } else if (gemv8_applicable(s, Lw.w2, N)) { if ((rc = launch_gemv8<EPI_RESID>(s, w))) return rc; }
             else if ((rc = launch_gemv<1, PRO_PREQ, EPI_RESID>(s, w))) return rc;
@@ -1056,8 +1069,8 @@ static int load_locked(b200_slice * s, const char * path) {
     try {
         const std::string p0 = "layers." + std::to_string(s->first_layer);
         s->wtype = (int) f.get(p0 + ".attention.wq.weight", {E, E}).type;
-        if (s->wtype != kWT_Q4_0 && s->wtype != kWT_Q4_1 && s->wtype != kWT_Q8_0 && s->wtype != kWT_F16)
-            return fail(B200_EFILE, "weight type %d unsupported (Q4_0, Q4_1, Q8_0, F16)", s->wtype);
+        if (!wt_block_quant(s->wtype) && s->wtype != kWT_F16)
+            return fail(B200_EFILE, "weight type %d unsupported (Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, F16)", s->wtype);
         float * d_norms = nullptr;
         if ((rc = dev_alloc(s, &d_norms, (size_t) s->L * 2 * E))) return rc;
         norms.resize((size_t) s->L * 2 * E);
@@ -1120,8 +1133,8 @@ static int load_locked(b200_slice * s, const char * path) {
     if (s->wtype != kWT_F16) {
         s->nbqE = s->layers[0].wo.nbq; s->nbqF = s->layers[0].w2.nbq;
         const size_t nq = (size_t) s->n_ctx;
-        // Q4_1: every scale array carries a second plane (Q8_1's block sums s) right behind the scales
-        const size_t pl = s->wtype == kWT_Q4_1 ? 2 : 1;
+        // Q4_1 / Q5_1: every scale array carries a second plane (Q8_1's block sums s) right behind the scales
+        const size_t pl = wt_q8_1(s->wtype) ? 2 : 1;
         if (pl == 2) { s->soffE = (int)(nq * s->nbqE * 4); s->soffF = (int)(nq * s->nbqF * 4); }
         if ((rc = dev_alloc(s, &s->aq_att, nq * s->nbqE * 32)) || (rc = dev_alloc(s, &s->da_att, pl * nq * s->nbqE * 4)) ||
             (rc = dev_alloc(s, &s->aq_gate, nq * s->nbqF * 32)) || (rc = dev_alloc(s, &s->da_gate, pl * nq * s->nbqF * 4))) return rc;
@@ -1929,6 +1942,15 @@ __global__ void k_embed_rows(const uint8_t * emb, int type, int E, const int32_t
             const float d = h2f(*(const uint16_t *) blk), m = h2f(*(const uint16_t *)(blk + 2));
             const int j = i & 31, q = blk[4 + (j & 15)];
             v = fadd(fmul((float)(j < 16 ? (q & 0x0F) : (q >> 4)), d), m);
+        } else if (type == kWT_Q5_0 || type == kWT_Q5_1) {  // dequantize_row_q5_0 / _q5_1, ggml.c:1564-1611
+            const bool q51 = type == kWT_Q5_1;
+            const uint8_t * blk = emb + ((size_t) t * (E / 32) + i / 32) * (q51 ? 24 : 22);
+            const float d = h2f(*(const uint16_t *) blk);
+            const uint8_t * qh = blk + (q51 ? 4 : 2);
+            const int j = i & 31, q = qh[4 + (j & 15)];
+            const int x = (j < 16 ? (q & 0x0F) : (q >> 4)) | (((qh[j >> 3] >> (j & 7)) & 1) << 4);
+            if (q51) v = fadd(fmul((float) x, d), h2f(*(const uint16_t *)(blk + 2)));   // x * d, then + m (two roundings)
+            else     v = fmul((float)(x - 16), d);
         } else if (type == kWT_Q8_0) {
             const uint8_t * blk = emb + ((size_t) t * (E / 32) + i / 32) * 34;
             v = fmul((float)((const int8_t *)(blk + 2))[i & 31], h2f(*(const uint16_t *) blk));
@@ -2067,10 +2089,10 @@ int b200_extra_load(const char * path, int device, b200_extra_t ** out) {
         const GgjtTensor & tn = f.get("norm.weight", {E});
         const GgjtTensor & to = f.get("output.weight", {E, V});
         e->emb_type = (int) te.type; e->out_type = (int) to.type;
-        if (te.type != GT_Q4_0 && te.type != GT_Q4_1 && te.type != GT_Q8_0 && te.type != GT_F16 && te.type != GT_F32)
+        if (!wt_block_quant((int) te.type) && te.type != GT_F16 && te.type != GT_F32)
             return fail(B200_EFILE, "tok_embeddings type %u unsupported", te.type);
-        if (to.type != GT_Q4_0 && to.type != GT_Q4_1 && to.type != GT_Q8_0 && to.type != GT_F16 && to.type != GT_Q6_K)
-            return fail(B200_EFILE, "output.weight type %u unsupported (Q4_0, Q4_1, Q8_0, F16, Q6_K)", to.type);
+        if (!wt_block_quant((int) to.type) && to.type != GT_F16 && to.type != GT_Q6_K)
+            return fail(B200_EFILE, "output.weight type %u unsupported (Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, F16, Q6_K)", to.type);
         if (to.type == GT_Q6_K && E % 256) return fail(B200_EFILE, "Q6_K output.weight needs n_embd %% 256 == 0");
         if (tn.type != GT_F32) return fail(B200_EFILE, "norm.weight must be F32");
         if ((rc = dev_alloc(s, &e->emb_raw, te.nbytes)) || (rc = dev_alloc(s, &e->norm_w, (size_t) E))) return rc;
