@@ -535,10 +535,13 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
     if (persist) { int rc = launch_persistent(s, in, out); if (rc) return rc; }
     for (int il = 0; il < (persist ? 0 : s->L); il++) {
         LayerW & Lw = s->layers[il];
-        // grid-barrier norm+quant epilogue: decode only (every CTA of wo / w2 must be co-resident: 1 tile per CTA)
-        const bool fast = s->fast_prefill && N >= s->fast_min_tokens && (s->wtype == kWT_Q4_0 || (s->wtype == kWT_Q8_0 && s->fast_version >= 2)) &&
+        // fast mode is for prefill calls only: a single-token step or a batched step (cols: one token of each of N sessions)
+        // stays exact, so decode and batch_forward keep the reference's bits whatever min_tokens is
+        const bool fast = s->fast_prefill && N > 1 && !s->cols && N >= s->fast_min_tokens &&
+                          (s->wtype == kWT_Q4_0 || (s->wtype == kWT_Q8_0 && s->fast_version >= 2)) &&
                           (Lw.qkv.n_tiles * Lw.qkv.TR) % 16 == 0 &&
                           (Lw.wo.n_tiles * Lw.wo.TR) % 16 == 0 && (Lw.w13.n_tiles * Lw.w13.TR) % 16 == 0;
+        // grid-barrier norm+quant epilogue: decode only (every CTA of wo / w2 must be co-resident: 1 tile per CTA)
         const bool nq = s->use_nq && N == 1 && !s->cols && s->wtype != kWT_F16 && Lw.wo.n_tiles <= 256 && Lw.wo.n_tiles <= s->n_sm * 2;
         float * nxt = (il == s->L - 1) ? out : ((il & 1) ? s->xb : s->xa);
         // cols mode (batched independent sequences): the kernels add session * sess_stride themselves
@@ -1510,11 +1513,12 @@ int b200_debug_trace_read(b200_slice_t * s, unsigned long long * out, int * cls,
 }
 
 /* Test hook: copy `count` 32-bit words of an internal activation buffer to the host after a
- * forward (0 qkv, 1 att, 2 ffin, 3 gate, 4 xa, 5 xb, 6 q16, 7 k-cache, 8 v-cache). */
+ * forward (0 qkv, 1 att, 2 ffin, 3 gate, 4 xa, 5 xb, 6 q16, 7 k-cache, 8 v-cache, 9 xh: the fp16 activations of the
+ * last fast-mode matmul). */
 int b200_debug_read(b200_slice_t * s, int which, size_t offset_words, size_t count, void * out) {
     if (!s || !out) return fail(B200_EINVAL, "null argument");
-    const void * src[9] = {s->qkv, s->att, s->ffin, s->gate, s->xa, s->xb, s->q16, s->kc, s->vc};
-    if (which < 0 || which > 8) return fail(B200_EINVAL, "bad buffer id %d", which);
+    const void * src[10] = {s->qkv, s->att, s->ffin, s->gate, s->xa, s->xb, s->q16, s->kc, s->vc, s->xh};
+    if (which < 0 || which > 9) return fail(B200_EINVAL, "bad buffer id %d", which);
     B200_CUDA(cudaSetDevice(s->device));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     B200_CUDA(cudaMemcpy(out, (const uint32_t *) src[which] + offset_words, count * 4, cudaMemcpyDeviceToHost));

@@ -203,6 +203,14 @@ def quantize_q8_0(x: np.ndarray) -> np.ndarray:
     return out
 
 
+def dequantize_q8_0(blocks: np.ndarray) -> np.ndarray:
+    """[rows, nb, 34] u8 -> [rows, nb*32] f32: q * d, one rounding (ggml.c dequantize_row_q8_0)."""
+    rows, nb, _ = blocks.shape
+    d = blocks[..., 0:2].copy().view(np.float16).astype(np.float32)
+    q = np.ascontiguousarray(blocks[..., 2:]).view(np.int8).astype(np.float32)
+    return (q * d).astype(np.float32).reshape(rows, nb * QK)
+
+
 def encode_tensor(x: np.ndarray, ttype: int) -> bytes:
     if ttype == T_F32:
         return np.ascontiguousarray(x, dtype=np.float32).tobytes()
@@ -564,6 +572,20 @@ def _fast_q5_pool(seed: int, k: int, wtype: int) -> np.ndarray:
     return blocks
 
 
+def _fast_q8_pool(seed: int, k: int) -> np.ndarray:
+    """Q8_0 twin of _fast_q4_pool: 34-byte blocks of uniform int8 quants in [-127, 127] (the range the reference's
+    quantiser writes) and fp16 scale +-mag*(1 + j/512), mag = 1/(73.6*sqrt(fan_in)) (a uniform quant has std ~73.6),
+    so weights have std ~ 1/sqrt(fan_in)."""
+    rng = np.random.default_rng([seed, k, 84])
+    blocks = rng.integers(0, 256, size=(_POOL_BLOCKS, 34), dtype=np.uint8)
+    blocks[:, 2:][blocks[:, 2:] == 0x80] = 0x81                 # -128 -> -127
+    mag = 1.0 / (73.6 * np.sqrt(k))
+    d = (mag * (1.0 + (blocks[:, 1].astype(np.float32) - 128.0) / 512.0)).astype(np.float16)
+    d = d.view(np.uint16) | ((blocks[:, 0] & 1).astype(np.uint16) << 15)
+    blocks[:, 0:2] = d.view(np.uint8).reshape(-1, 2)
+    return blocks
+
+
 def write_fast_q4_slice(path: str, shape: ModelShape, layer_from: int, layer_to: int, seed: int = 0,
                         wtype: int = T_Q4_0) -> int:
     """Large-model generator for benchmarks.  Quantising 6.5e9 Gaussians takes minutes, so Q4_0
@@ -572,8 +594,8 @@ def write_fast_q4_slice(path: str, shape: ModelShape, layer_from: int, layer_to:
     ground truth for both the GPU path and the CPU reference, so the distribution only has to keep
     activations finite; any layer range of the same (shape, seed) is reproducible.  Returns bytes written.
     `wtype` = T_Q4_1 writes 20-byte Q4_1 blocks from _fast_q41_pool instead, T_Q5_0 / T_Q5_1 22- / 24-byte blocks
-    from _fast_q5_pool."""
-    assert wtype in (T_Q4_0, T_Q4_1, T_Q5_0, T_Q5_1)
+    from _fast_q5_pool, T_Q8_0 34-byte blocks from _fast_q8_pool."""
+    assert wtype in (T_Q4_0, T_Q4_1, T_Q5_0, T_Q5_1, T_Q8_0)
     bsz = TYPE_BLOCK[wtype][1]
     vocab = default_vocab(shape.n_vocab)
     hp = HParams(shape.n_vocab, shape.n_embd, shape.n_mult, shape.n_head, layer_to - layer_from + 1,
@@ -585,6 +607,8 @@ def write_fast_q4_slice(path: str, shape: ModelShape, layer_from: int, layer_to:
     if wtype in (T_Q5_0, T_Q5_1):
         def make_pool(sd, k):
             return _fast_q5_pool(sd, k, wtype)
+    elif wtype == T_Q8_0:
+        make_pool = _fast_q8_pool
     else:
         make_pool = _fast_q4_pool if wtype == T_Q4_0 else _fast_q41_pool
     pools = {k: memoryview(make_pool(seed, k)).cast("B") for k in sorted({e, ff})}

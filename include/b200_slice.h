@@ -102,9 +102,12 @@ int b200_batch_forward(b200_slice_t * s, const int * sessions, int n_seq, const 
 int b200_batch_forward_device(b200_slice_t * s, const int * sessions, int n_seq, const float * d_in, float * d_out, int sync);
 
 /* Fast mode for prefill calls (n_tokens >= min_tokens): the Q4_0 / Q8_0 weight matmuls run on the wgmma tensor cores with
- * the dequantisation fused in (csrc/fastgemm2.cuh; Q4_1, Q5_0, Q5_1 and F16 slices ignore the switch and stay exact).  NOT bit-exact: operands are rounded to fp16 after the reference's
- * Q8_0 activation quantisation; deviation from exact mode is bounded in tests/test_gpu_fast_prefill.py.  Off by default
- * (or B200_FAST_PREFILL=1); decode steps always run in exact mode. */
+ * the dequantisation fused in (csrc/fastgemm2.cuh; Q4_1, Q5_0, Q5_1 and F16 slices ignore the switch and stay exact).
+ * NOT bit-exact: operands are rounded to fp16 after the reference's Q8_0 activation quantisation and summed in fp32.
+ * Each matmul output is within TAU * sum_k |w16 * x16| of the float64 sum of the same fp16 operands (TAU <= 2^-16, see
+ * tests/test_gpu_fast_prefill.py, which also bounds the deviation from exact mode).  Off by default (or
+ * B200_FAST_PREFILL=1).  Fast mode never applies to a single-token step or to a batched step (b200_batch_forward),
+ * whatever min_tokens is: decode always runs in exact mode. */
 int b200_slice_set_fast_prefill(b200_slice_t * s, int on, int min_tokens);
 
 /* Block until everything queued on the slice's stream has finished. */
@@ -134,7 +137,8 @@ float * b200_slice_dev_in(b200_slice_t * s);
 float * b200_slice_dev_out(b200_slice_t * s);
 
 /* Test hook: copy `count` 32-bit words of an internal activation buffer to the host after a forward
- * (0 qkv, 1 att, 2 ffin, 3 gate, 4 xa, 5 xb, 6 q16, 7 k-cache, 8 v-cache).  Not part of the drop-in surface. */
+ * (0 qkv, 1 att, 2 ffin, 3 gate, 4 xa, 5 xb, 6 q16, 7 k-cache, 8 v-cache, 9 xh: the [n_tokens][K] fp16 activations of
+ * the last fast-mode matmul, i.e. w2's input after a fast prefill).  Not part of the drop-in surface. */
 int b200_debug_read(b200_slice_t * s, int which, size_t offset_words, size_t count, void * out);
 
 /* Measurement aid (bench.py roofline): while on, a decode step launches only its weight-matmul kernels. */

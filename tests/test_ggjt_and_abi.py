@@ -149,3 +149,54 @@ def test_q4_1_quantizer_is_the_reference_quantize_tool(tmp_path):
         src = np.frombuffer(a.read_raw(name), np.float32).reshape(t.ne[1], t.ne[0])
         assert hashlib.sha256(ggjt.quantize_q4_1(src).tobytes()).hexdigest() == digest, name
     assert len(want) == 2 + 7 * sh.n_layer
+
+
+def test_q8_0_dequantizer_is_q_times_d():
+    """ggjt.dequantize_q8_0 (ggml.c dequantize_row_q8_0): element j of a block is int8 q_j * fp16 d, one fp32 rounding;
+    it inverts quantize_q8_0 to within half a step plus the fp16 rounding of the scale (127 * 2^-12 steps)."""
+    rng = np.random.default_rng(1)
+    x = rng.standard_normal((3, 96)).astype(np.float32)
+    q = ggjt.quantize_q8_0(x)
+    y = ggjt.dequantize_q8_0(q)
+    assert y.shape == (3, 96) and y.dtype == np.float32
+    d = q[..., :2].copy().view(np.float16).astype(np.float32)             # [3, 3, 1]
+    qs = q[..., 2:].copy().view(np.int8).astype(np.float32)               # [3, 3, 32]
+    assert np.array_equal(y, (qs * d).astype(np.float32).reshape(3, 96))
+    step = np.repeat(d[..., 0], 32, axis=1)
+    assert (np.abs(x - y) <= (0.5 + 127 * 2 ** -12) * step).all()
+    # a hand-made block: d = -0.25, q = -127, -119, ..., 113 and 127
+    blk = np.zeros((1, 1, 34), np.uint8)
+    blk[0, 0, :2] = np.array([-0.25], np.float16).view(np.uint8)
+    vals = np.array(list(range(-127, 120, 8)) + [127], np.int8)
+    blk[0, 0, 2:] = vals.view(np.uint8)
+    assert np.array_equal(ggjt.dequantize_q8_0(blk)[0], vals.astype(np.float32) * np.float32(-0.25))
+
+
+def test_fast_writer_q8_0_blocks(tmp_path):
+    """write_fast_q4_slice(wtype=T_Q8_0): reference-format Q8_0 tensors of the right size, deterministic per layer,
+    quants in the reference quantiser's range [-127, 127], weights with std ~ 1/sqrt(fan_in); the C restatement
+    runs the file."""
+    from oracle import oracle
+    sh = ggjt.ModelShape(512, 256, 32, 2, 3)
+    p, p2 = str(tmp_path / "q8.bin"), str(tmp_path / "q8b.bin")
+    n = ggjt.write_fast_q4_slice(p, sh, 1, 2, seed=5, wtype=ggjt.T_Q8_0)
+    assert n == os.path.getsize(p)
+    f = ggjt.read_file(p, sliced=True)
+    assert f.hparams.ftype == ggjt.FTYPE_Q8_0 and f.hparams.n_layer == 2 and len(f.tensors) == 18
+    for name in ("layers.2.feed_forward.w2.weight", "layers.1.attention.wq.weight"):
+        t = f.tensors[name]
+        k, rows = t.ne
+        assert t.ttype == ggjt.T_Q8_0 and t.offset % 32 == 0 and t.nbytes == rows * k // 32 * 34
+        blocks = np.frombuffer(f.read_raw(name), np.uint8).reshape(rows, k // 32, 34)
+        assert (blocks[..., 2:].view(np.int8) != -128).all()
+        w = ggjt.dequantize_q8_0(blocks)
+        assert np.isfinite(w).all() and 0.8 < w.std() * np.sqrt(k) < 1.25, (name, w.std() * np.sqrt(k))
+    ggjt.write_fast_q4_slice(p2, sh, 2, 2, seed=5, wtype=ggjt.T_Q8_0)
+    g = ggjt.read_file(p2, sliced=True)
+    a, b = open(p, "rb").read(), open(p2, "rb").read()
+    t1, t2 = f.tensors["layers.2.feed_forward.w1.weight"], g.tensors["layers.2.feed_forward.w1.weight"]
+    assert a[t1.offset:t1.offset + t1.nbytes] == b[t2.offset:t2.offset + t2.nbytes]
+    s = oracle.PortSlice(p, 32)
+    y = s.forward(np.random.default_rng(0).standard_normal((3, 256), dtype=np.float32))
+    s.close()
+    assert np.isfinite(y).all() and np.abs(y).max() < 100
