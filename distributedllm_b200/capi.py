@@ -77,7 +77,6 @@ def lib() -> C.CDLL:
         L.b200_pipeline_result.argtypes = [vp]
         L.b200_pipeline_result.restype = vp
         L.b200_device_init.argtypes = [ci]
-        L.b200_debug_ptrace_read.argtypes = [vp, vp, C.c_size_t]
         for name, args in (("b200_pipeline_unique_id", [vp]), ("b200_pipeline_init", [vp, ci, ci, vp]),
                            ("b200_pipeline_step", [vp, vp, ci, ci]),
                            ("b200_pipeline_mailbox_export", [vp, vp]), ("b200_pipeline_mailbox_connect", [vp, vp, ci]),
@@ -228,13 +227,6 @@ class Slice:
         ctas = np.zeros(max_launches, np.int32)
         n = lib().b200_debug_trace_read(self._h, _ptr(buf), _ptr(cls), _ptr(ctas), max_launches)
         return buf[:n], cls[:n], ctas[:n]
-
-    def ptrace_read(self, n_sm: int = 132):
-        """-> stamps [n_cta][n_layer][16] uint64 ns of the last persistent step (B200_PTRACE=1)."""
-        L = self.info.n_layer
-        buf = np.zeros((n_sm, L, 16), np.uint64)
-        n = lib().b200_debug_ptrace_read(self._h, _ptr(buf), buf.size)
-        return buf[: n // L] if L else buf[:0]
 
     def last_ms(self) -> float:
         return float(lib().b200_slice_last_ms(self._h))

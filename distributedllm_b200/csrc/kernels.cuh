@@ -763,153 +763,6 @@ __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
 }
 
 // =============================================================================================
-// K1n: the NARROW matrices of a single-token step (wo, w2: 128 tiles of 32 rows for 7B = at most one CTA per SM).
-// With k_gemv's mapping (4 threads per row) such a CTA is 4 consumer warps = ONE warp per scheduler, and a lone warp
-// cannot hide its own latencies.  The parallelism exact mode allows is rows x 8 AVX lanes (each lane's fma
-// chain is sequential in K), so this variant spends ALL of it: 8 threads per row, thread (r, l) owns AVX lane l alone.
-//   * 8 consumer warps per CTA, warp = 4 rows x 8 lanes, same 32-row tile, same packed layout, same TMA ring;
-//   * per block and thread: one shift+mask (lanes 0..3 take the low nibbles of word l, lanes 4..7 the high nibbles of
-//     word l-4), one dp4a, the magic-number int->float, one fma -- 8 instead of 15 instructions on the warp's critical path;
-//   * the scale product D = d_w * d_a is now computed by 8 threads instead of 4 (+27 % instructions in total), which is
-//     why the wide matrices (qkv, w1|w3: >= 2.3 warps per scheduler already) keep k_gemv.
-// Pre-quantised input only (PRO_PREQ: the attention / gate epilogue already produced Q8_0), one column, epilogues
-// + residual and + residual + send (EPI_RESID, EPI_RESID_SEND).  Arithmetic per lane chain is k_gemv's, operand for operand.
-// Opt-in (B200_N8=1), bit-exact (tests/test_gpu_parity.py::test_narrow_matrix_kernel_is_a_scheduling_choice).
-// =============================================================================================
-constexpr int kN8Warps = 8;
-constexpr int kN8Consumers = kN8Warps * 32;
-
-template <int WT, int EPI>
-__global__ void __launch_bounds__(kN8Consumers + 32) k_gemv_n8(const GemvArgs a) {
-    static_assert(WT == kWT_Q4_0 || WT == kWT_Q8_0, "narrow variant: Q4_0 / Q8_0");
-    constexpr int CB = chunk_bytes(WT);
-    constexpr int TR = 4;                                   // row-groups of 8 rows per tile (= k_gemv with G = 1)
-    constexpr int stage_bytes = kQS * TR * CB;
-    extern __shared__ __align__(128) uint8_t smem[];
-    const int nbq = a.W.nbq, NS = a.NS;
-    // smem: [ring NS*stage][act words nbq*128][act scales nbq*16][full 16][empty 16][act bar 2]
-    uint8_t * ring = smem;
-    int * a_s = (int *)(smem + (size_t) NS * stage_bytes);
-    float * da_s = (float *)((uint8_t *) a_s + (size_t) nbq * 128);
-    uint64_t * full = (uint64_t *)((uint8_t *) da_s + (size_t) nbq * 16);
-    uint64_t * empty = full + 16;
-    uint64_t * actbar = empty + 16;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int n_stage = nbq / kQS;
-
-    if (tid == 0) {
-        B200_TRACE(a.trace, 0);
-        for (int s = 0; s < NS; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], kN8Warps); }
-        mbar_init(actbar, 1);
-        mbar_init(actbar + 1, kN8Warps);
-        mbar_fence_init();
-    }
-    __syncthreads();
-
-    if (warp == kN8Warps) {
-        // producer warp: k_gemv's, including the gate on the consumers' prologue copies and the late dependent trigger
-        if (lane == 0) {
-            int slot = 0, use = 0, issued = 0;
-            for (int tile = blockIdx.x; tile < a.W.n_tiles; tile += gridDim.x) {
-                const uint8_t * src = a.W.data + (long long) tile * a.W.tile_bytes;
-                for (int s = 0; s < n_stage; s++) {
-                    if (issued == a.pre_stages) mbar_wait(actbar + 1, 0);
-                    issued++;
-                    if (use > 0) mbar_wait(&empty[slot], (use - 1) & 1);
-                    mbar_arrive_expect_tx(&full[slot], (uint32_t) stage_bytes);
-                    bulk_g2s(ring + (size_t) slot * stage_bytes, src + (size_t) s * stage_bytes, (uint32_t) stage_bytes, &full[slot]);
-                    if (++slot == NS) { slot = 0; use++; }
-                }
-            }
-            if (issued <= a.pre_stages) mbar_wait(actbar + 1, 0);
-            grid_dep_launch();
-            B200_TRACE(a.trace, 4);
-        }
-        return;
-    }
-
-    grid_dep_wait();                                        // the quantised activation comes from the previous kernel
-    if (tid == 0) {
-        B200_TRACE(a.trace, 1);
-        const uint32_t b1 = (uint32_t) nbq * 128, b2 = (uint32_t) nbq * 16;
-        mbar_arrive_expect_tx(actbar, b1 + b2);
-        bulk_g2s(a_s, a.aq_in, b1, actbar);
-        bulk_g2s(da_s, a.da_in, b2, actbar);
-    }
-    if (lane == 0) mbar_arrive(actbar + 1);
-    mbar_wait(actbar, 0);
-    if (tid == 0) B200_TRACE(a.trace, 2);
-
-    const int rg = warp >> 1;                               // row-group of the tile
-    const int r = (warp & 1) * 4 + (lane >> 3), l = lane & 7;   // row in the group, AVX lane
-    const int sh = (WT == kWT_Q4_0 && l < 4) ? 4 : 0;
-    const uint32_t w_off = (uint32_t)((WT == kWT_Q8_0 ? (l >> 2) * 512 : 0) + (4 * r + (l & 3)) * 16);
-    const uint32_t s_off = (uint32_t)((WT == kWT_Q8_0 ? 1024 : 512) + r * 8);
-    const int * a_l = a_s + (l & 3) * 8 + (l >> 2);         // words [Q][l&3][bq][l>>2]
-    uint2 * send_slot = nullptr; int send_seq = 0;
-    if (EPI == EPI_RESID_SEND) {
-        send_seq = a.mb_mine->seq_out + 1;
-        if (lane == 0) mb_wait_slot_free(a.mb_mine, send_seq);
-        __syncwarp();
-        send_slot = a.mb_peer_inbox + (size_t)(send_seq & (kMbSlots - 1)) * a.mb_slot_elems;
-    }
-    int slot = 0, phase = 0;
-#ifdef B200_TRACE_WAITS
-    long long dbg_wait = 0, dbg_t0 = a.trace ? clock64() : 0;
-#endif
-    for (int tile = blockIdx.x; tile < a.W.n_tiles; tile += gridDim.x) {
-        float acc = 0.f;
-        for (int s = 0; s < n_stage; s++) {
-#ifdef B200_TRACE_WAITS
-            if (a.trace) { const long long c0 = clock64(); mbar_wait(&full[slot], phase); dbg_wait += clock64() - c0; }
-            else
-#endif
-            mbar_wait(&full[slot], phase);
-            const uint8_t * base = ring + (size_t) slot * stage_bytes + (size_t) rg * CB;
-            if (!a.dbg_nomath)
-            #pragma unroll
-            for (int qi = 0; qi < kQS; qi++) {
-                const int Q = s * kQS + qi;
-                const uint8_t * ch = base + (size_t) qi * TR * CB;
-                const uint4 wv = *(const uint4 *)(ch + w_off);
-                const uint2 sc = *(const uint2 *)(ch + s_off);
-                const float4 dav = *(const float4 *)(da_s + Q * 4);
-                const int av[4] = {a_l[Q * 32], a_l[Q * 32 + 2], a_l[Q * 32 + 4], a_l[Q * 32 + 6]};
-                const uint32_t ww[4] = {wv.x, wv.y, wv.z, wv.w};
-                const uint32_t sw[2] = {sc.x, sc.y};
-                const float da[4] = {dav.x, dav.y, dav.z, dav.w};
-                #pragma unroll
-                for (int bq = 0; bq < 4; bq++) {
-                    const uint16_t dh = (uint16_t)(sw[bq >> 1] >> (16 * (bq & 1)));
-                    const float D = fmul(h2f(dh), da[bq]);
-                    const int v = WT == kWT_Q4_0 ? (int)((ww[bq] << sh) & 0xF0F0F0F0u) : (int) ww[bq];
-                    const float f = fadd(__int_as_float(__dp4a(v, av[bq], kMagicI)), -kMagic);
-                    acc = ffma(D, f, acc);
-                }
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty[slot]);
-            if (++slot == NS) { slot = 0; phase ^= 1; }
-        }
-        // hsum_float_8: (a_l + a_l+4), then + lane^2, then + lane^1
-        float t = fadd(acc, __shfl_xor_sync(0xffffffffu, acc, 4));
-        t = fadd(t, __shfl_xor_sync(0xffffffffu, t, 2));
-        t = fadd(t, __shfl_xor_sync(0xffffffffu, t, 1));
-        const int row = (tile * TR + rg) * 8 + r;
-        if (l == 0 && row < a.out_rows) {
-            const float v = fadd(t, a.resid[row]);
-            a.y[row] = v;
-            if (EPI == EPI_RESID_SEND) st_ll(send_slot + row, v, send_seq);
-        }
-    }
-    if (tid == 0) B200_TRACE(a.trace, 3);
-#ifdef B200_TRACE_WAITS
-    if (tid == 0 && a.trace)
-        a.trace[(size_t) blockIdx.x * 8 + 7] = ((unsigned long long) dbg_wait << 32) | (unsigned long long)((clock64() - dbg_t0) & 0xFFFFFFFFll);
-#endif
-}
-
-// =============================================================================================
 // K3: RMSNorm * weight -> Q8_0 act-quant of whole rows, once per token, for MULTI-token calls (prefill chunks, batched
 // steps).  With several columns per CTA the fused PRO_NORM prologue would repeat this for every 32-row tile (480x for
 // qkv) behind one dependent global round trip per column; here it is done once and the matmul CTAs fetch the quantised

@@ -5,7 +5,6 @@
 // one H100.  One stream per slice; the N=1 decode step is a CUDA graph replayed per token with
 // the position kept in device memory.
 #include "kernels.cuh"
-#include "persist.cuh"
 #include "fastgemm.cuh"
 #include "fastgemm2.cuh"
 #include "ggjt_file.hpp"
@@ -29,7 +28,6 @@ constexpr int kSmemLimit = 226 * 1024;   // opt-in dynamic limit is 227 KB minus
 
 struct LayerW {
     PackedW qkv{}, wo{}, w13{}, w2{};
-    PackedW wo_p{}, w2_p{};      // persistent-kernel copies of the narrow matrices with fewer row-groups per tile (B200_PERSIST_TR)
     // F16-weight slices
     uint16_t * f_q = nullptr, * f_k = nullptr, * f_v = nullptr, * f_o = nullptr, * f_1 = nullptr, * f_2 = nullptr, * f_3 = nullptr;
     float * attn_norm = nullptr, * ffn_norm = nullptr;
@@ -66,7 +64,7 @@ struct b200_slice {
     std::map<GraphKey, cudaGraphExec_t> graphs;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr; bool timed = false;
     int64_t launches = 0, weight_bytes = 0;
-    bool use_ring = true, use_graph = true, use_pdl = false, use_nq = true, f16_ring = true, use_tiled_attn = true, use_n8 = false, f16_mc = true; int f16_mc_cols = 4;
+    bool use_ring = true, use_graph = true, use_pdl = false, use_nq = true, f16_ring = true, use_tiled_attn = true, f16_mc = true; int f16_mc_cols = 4;
     bool skip_attention = false;   // measurement aid: replay only the weight matmuls of a step (bench.py roofline)
     bool attn_lut_smem = true;     // single-token attention stages the exp table in shared memory (decided at load)
     bool fast_prefill = false; int fast_min_tokens = 32; uint16_t * xh = nullptr;   // tensor-core prefill (fast mode)
@@ -90,9 +88,6 @@ struct b200_slice {
     // as they are computed, no k_peer_send launch on the critical path
     bool fold_send = false, use_fold = true;
     std::map<GraphKey, cudaGraphExec_t> pp_graphs;
-    // persistent single-token step (persist.cuh)
-    bool use_persist = false; int persist_tr = 4, persist_ns = 0, persist_ctas = 0;
-    int * p_cnt = nullptr; std::map<GraphKey, PLayer *> p_tables; unsigned long long * p_trace = nullptr;
 };
 
 namespace b200 {
@@ -178,58 +173,6 @@ static int launch_gemv_t(b200_slice * s, GemvArgs a) {
     prof_end(s);
     s->launches++;
     return 0;
-}
-
-// narrow matrices of a single-token step: 8 threads per row (k_gemv_n8), one CTA per tile, deep ring
-template <int WT, int EPI>
-static int launch_gemv8_t(b200_slice * s, GemvArgs a) {
-    constexpr int CB = chunk_bytes(WT);
-    auto kern = k_gemv_n8<WT, EPI>;
-    static bool attr_set[16] = {false};
-    const size_t stage = (size_t) kQS * 4 * CB;
-    const size_t act = (size_t) a.W.nbq * 144 + 34 * 8 + 64;
-    // every tile gets a co-resident CTA (13B: 160 tiles -> two CTAs on some SMs, each with half the ring)
-    const int need = (a.W.n_tiles + s->n_sm - 1) / s->n_sm;
-    const size_t budget = (size_t) kSmemLimit / need - 1024;
-    int NS = s->opt_ns > 0 ? s->opt_ns : (budget > act ? (int)((budget - act) / stage) : 2);
-    if (NS > 16) NS = 16;
-    if (NS < 2) NS = 2;
-    const size_t smem = NS * stage + act;
-    if (smem > (size_t) kSmemLimit) return fail(B200_EINVAL, "gemv8 needs %zu B of shared memory (K=%d)", smem, a.W.K);
-    if (!attr_set[s->device & 15]) {
-        B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-        B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-        attr_set[s->device & 15] = true;
-    }
-    a.NS = NS; a.dbg_nomath = s->opt_nomath; a.pre_stages = s->opt_pre;
-    a.trace = nullptr;
-    if (s->trace && s->trace_next < 512) { a.trace = s->trace + (size_t) s->trace_next * 1024 * 8; s->trace_next++; s->trace_cls.push_back(s->cur_class); }
-    const int gx = a.W.n_tiles;
-    if (a.trace) s->trace_ctas.push_back(gx);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(gx, 1, 1);
-    cfg.blockDim = dim3(kN8Consumers + 32, 1, 1);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = s->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = s->use_pdl ? 1 : 0;
-    prof_begin(s);
-    B200_CUDA(cudaLaunchKernelEx(&cfg, kern, a));
-    prof_end(s);
-    s->launches++;
-    return 0;
-}
-// applies to: one column, ring on, Q4_0 / Q8_0, the matrix is narrow enough that k_gemv would run <= 1 CTA per SM
-static bool gemv8_applicable(const b200_slice * s, const PackedW & W, int N) {
-    return s->use_n8 && N == 1 && !s->cols && s->use_ring && (W.wtype == kWT_Q4_0 || W.wtype == kWT_Q8_0) && W.TR == 4 &&
-           W.n_tiles <= s->n_sm * 3 / 2;
-}
-template <int EPI>
-static int launch_gemv8(b200_slice * s, const GemvArgs & a) {
-    if (a.W.wtype == kWT_Q4_0) return launch_gemv8_t<kWT_Q4_0, EPI>(s, a);
-    return launch_gemv8_t<kWT_Q8_0, EPI>(s, a);
 }
 
 template <int WT, int G, int PRO, int EPI>
@@ -440,100 +383,12 @@ static int launch_fast_any(b200_slice * s, const PackedW & W, const float * resi
     return launch_fast_gemm<EPI>(s, W, resid, ldr, y, ldy, N, out_rows);
 }
 
-// ---------------------------------------------------------------- persistent single-token step (persist.cuh)
-static bool persist_applicable(const b200_slice * s, int N) {
-    return s->use_persist && N == 1 && !s->cols && s->D == 128 && (s->wtype == kWT_Q4_0 || s->wtype == kWT_Q8_0) && !s->skip_attention &&
-           !s->profiling && s->E / 32 <= kPConsumers && s->p_cnt != nullptr;
-}
-
-static PMat pmat_of(const PackedW & W, int G) {
-    PMat m{};
-    m.data = W.data; m.n_tiles = W.n_tiles; m.nbq = W.nbq; m.TR = W.TR; m.tile_bytes = W.tile_bytes;
-    m.sq = kQS / G;                           // quads per ring stage: one stage = 16 chunks = one slot
-    return m;
-}
-
-// The layer table of a step (weights + this call's buffers) lives in device memory; it depends on (in, out, session), so
-// it is built once per such triple -- OUTSIDE any stream capture, which is why forward paths call this before capturing.
-static int persist_prepare(b200_slice * s, const float * in, float * out) {
-    GraphKey key{in, out, s->cur};
-    if (s->p_tables.count(key)) return 0;
-    std::vector<PLayer> tab(s->L);
-    const float * cur = in;
-    const int E = s->E;
-    const size_t sess_off = (size_t) s->cur * s->sess_stride;
-    for (int il = 0; il < s->L; il++) {
-        LayerW & Lw = s->layers[il];
-        PLayer & P = tab[il];
-        P.qkv = pmat_of(Lw.qkv, 1);
-        P.wo = pmat_of(Lw.wo, 1);
-        P.w13 = pmat_of(Lw.w13, 2);
-        P.w2 = pmat_of(Lw.w2, 1);
-        P.attn_norm = Lw.attn_norm; P.ffn_norm = Lw.ffn_norm;
-        float * nxt = (il == s->L - 1) ? out : ((il & 1) ? s->xb : s->xa);
-        P.x_in = cur; P.x_out = nxt;
-        P.kc = s->kc + sess_off + (size_t) il * s->n_ctx * E; P.vc = s->vc + sess_off + (size_t) il * s->n_ctx * E;
-        cur = nxt;
-    }
-    PLayer * d = nullptr;
-    int rc = dev_alloc(s, &d, (size_t) s->L);
-    if (rc) return rc;
-    B200_CUDA(cudaMemcpy(d, tab.data(), tab.size() * sizeof(PLayer), cudaMemcpyHostToDevice));
-    s->p_tables[key] = d;
-    return 0;
-}
-
-static int launch_persistent(b200_slice * s, const float * in, float * out) {
-    auto it = s->p_tables.find(GraphKey{in, out, s->cur});
-    if (it == s->p_tables.end()) return fail(B200_EINVAL, "persistent step: layer table not prepared");
-    PersistArgs a{};
-    a.layers = it->second; a.L = s->L;
-    a.E = s->E; a.FF = s->FF; a.H = s->H; a.n_ctx = s->n_ctx; a.nb_E = s->E / 32; a.nbqE = s->nbqE; a.nbqF = s->nbqF;
-    a.n_past = s->d_npast + s->cur;
-    a.qkv = s->qkv; a.att = s->att; a.ffin = s->ffin;
-    a.aq_att = s->aq_att; a.da_att = s->da_att; a.aq_gate = s->aq_gate; a.da_gate = s->da_gate;
-    a.dscale = wt_act_scale(s->wtype);
-    a.cs = s->cs; a.texp = s->texp; a.tsilu = s->tsilu;
-    a.cnt = s->p_cnt;
-    a.kq_scale = 1.0f / sqrtf((float) s->E / (float) s->H);
-    a.trace = s->p_trace;
-    const int nbq_max = s->nbqF > s->nbqE ? s->nbqF : s->nbqE;
-    const size_t limit = 227 * 1024;
-    int NS = s->persist_ns > 0 ? s->persist_ns : 48;          // ring slots of the CTA: all the shared memory that is left
-    while (NS > 4 && p_smem_layout(s->wtype, NS, nbq_max, s->E, s->n_ctx).total > limit) NS--;
-    const PSmem lay = p_smem_layout(s->wtype, NS, nbq_max, s->E, s->n_ctx);
-    if (lay.total > limit) return fail(B200_EINVAL, "persistent step needs %zu B of shared memory", lay.total);
-    a.NS = NS;
-    static bool attr_set[16] = {false};
-    if (!attr_set[s->device & 15]) {
-        B200_CUDA(cudaFuncSetAttribute(k_decode_persistent<kWT_Q4_0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) limit));
-        B200_CUDA(cudaFuncSetAttribute(k_decode_persistent<kWT_Q8_0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) limit));
-        attr_set[s->device & 15] = true;
-    }
-    // progress counters start at zero every step
-    B200_CUDA(cudaMemsetAsync(s->p_cnt, 0, (size_t) s->L * kPPhases * 4, s->stream));
-    int grid = s->persist_ctas > 0 ? s->persist_ctas : s->n_sm;      // one CTA per SM, all co-resident (they wait on each other)
-    if (grid > s->n_sm) grid = s->n_sm;
-    if (grid < s->H) return fail(B200_EINVAL, "persistent step needs at least n_head (%d) CTAs", s->H);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid, 1, 1); cfg.blockDim = dim3(kPThreads, 1, 1); cfg.dynamicSmemBytes = lay.total; cfg.stream = s->stream;
-    s->cur_class = 0;
-    prof_begin(s);
-    if (s->wtype == kWT_Q4_0) B200_CUDA(cudaLaunchKernelEx(&cfg, k_decode_persistent<kWT_Q4_0>, a));
-    else                      B200_CUDA(cudaLaunchKernelEx(&cfg, k_decode_persistent<kWT_Q8_0>, a));
-    prof_end(s);
-    s->launches++;
-    return 0;
-}
-
 // ---------------------------------------------------------------- one forward over the slice
 // Enqueue every layer for N tokens at device-side position *d_npast (tensor_processor.cpp:537-766).
 static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) {
     const int E = s->E, FF = s->FF, H = s->H, D = s->D;
     const float * cur = in;
-    const bool persist = persist_applicable(s, N);
-    if (persist) { int rc = launch_persistent(s, in, out); if (rc) return rc; }
-    for (int il = 0; il < (persist ? 0 : s->L); il++) {
+    for (int il = 0; il < s->L; il++) {
         LayerW & Lw = s->layers[il];
         // fast mode is for prefill calls only: a single-token step or a batched step (cols: one token of each of N sessions)
         // stays exact, so decode and batch_forward keep the reference's bits whatever min_tokens is
@@ -672,7 +527,6 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
             o.nq_norm_w = Lw.ffn_norm; o.nq_counter = s->nq_counter; o.nq_partial = s->nq_partial; o.aq_out = s->aq_x; o.da_out = s->da_x; o.out_nbq = s->nbqE; o.out_dscale = dsc;
             if (D == 128) {
                 if (nq) { if ((rc = launch_gemv<1, PRO_PREQ, EPI_RESID_NQ>(s, o))) return rc; }
-                else if (gemv8_applicable(s, Lw.wo, N)) { if ((rc = launch_gemv8<EPI_RESID>(s, o))) return rc; }
                 else    { if ((rc = launch_gemv<1, PRO_PREQ, EPI_RESID>(s, o))) return rc; }
             } else {
                 if (nq) { if ((rc = launch_gemv<1, PRO_PLAIN, EPI_RESID_NQ>(s, o))) return rc; }
@@ -698,16 +552,14 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
             } else if (s->fold_send && il == s->L - 1) {
                 w.mb_mine = (MailboxHdr *) s->mb_block;
                 w.mb_peer_inbox = (uint2 *)(s->mb_next + sizeof(MailboxHdr)); w.mb_slot_elems = s->mb_slot_floats;
-                if (gemv8_applicable(s, Lw.w2, N)) rc = launch_gemv8<EPI_RESID_SEND>(s, w);
-                else if (s->wtype == kWT_Q4_0) rc = launch_gemv_t<kWT_Q4_0, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
+                if (s->wtype == kWT_Q4_0) rc = launch_gemv_t<kWT_Q4_0, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
                 else if (s->wtype == kWT_Q4_1) rc = launch_gemv_t<kWT_Q4_1, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
                 else if (s->wtype == kWT_Q5_0) rc = launch_gemv_t<kWT_Q5_0, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
                 else if (s->wtype == kWT_Q5_1) rc = launch_gemv_t<kWT_Q5_1, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
                 else if (s->wtype == kWT_Q8_0) rc = launch_gemv_t<kWT_Q8_0, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
                 else rc = fail(B200_EINVAL, "no pipelined matmul for weight type %d", s->wtype);
                 if (rc) return rc;
-            } else if (gemv8_applicable(s, Lw.w2, N)) { if ((rc = launch_gemv8<EPI_RESID>(s, w))) return rc; }
-            else if ((rc = launch_gemv<1, PRO_PREQ, EPI_RESID>(s, w))) return rc;
+            } else if ((rc = launch_gemv<1, PRO_PREQ, EPI_RESID>(s, w))) return rc;
         }
         cur = nxt;
     }
@@ -740,8 +592,7 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
 static int run_decode_graph(b200_slice * s, const float * in, float * out, bool host) {
     GraphKey key{in, out, (host ? 1 : 0) | (s->skip_attention ? 2 : 0) | (s->send_pending ? 4 : 0) | (s->cur << 3)};
     auto it = s->graphs.find(key);
-    const int per_step = persist_applicable(s, 1) ? 2 : (s->D == 128 ? 5 : 6) * s->L + 1;
-    if (persist_applicable(s, 1)) { int rc = persist_prepare(s, host ? s->d_in : in, host ? s->d_out : out); if (rc) return rc; }
+    const int per_step = (s->D == 128 ? 5 : 6) * s->L + 1;
     if (it == s->graphs.end()) {
         const int64_t before = s->launches;
         cudaGraph_t g = nullptr;
@@ -797,7 +648,6 @@ static int forward_locked(b200_slice * s, const float * in, int N, float * out, 
             memcpy(out, s->h_out, (size_t) s->E * 4);
         } else {
             B200_CUDA(cudaMemcpyAsync(s->d_in, in, (size_t) N * s->E * 4, cudaMemcpyHostToDevice, s->stream));
-            if (persist_applicable(s, N) && (rc = persist_prepare(s, s->d_in, s->d_out))) return rc;
             if ((rc = enqueue_layers(s, s->d_in, N, s->d_out))) return rc;
             B200_CUDA(cudaEventRecord(s->ev1, s->stream));
             B200_CUDA(cudaMemcpyAsync(out, s->d_out, (size_t) N * s->E * 4, cudaMemcpyDeviceToHost, s->stream));
@@ -805,10 +655,7 @@ static int forward_locked(b200_slice * s, const float * in, int N, float * out, 
         }
     } else {
         if (N == 1 && s->use_graph && !s->profiling) { if ((rc = run_decode_graph(s, in, out, false))) return rc; }
-        else {
-            if (persist_applicable(s, N) && (rc = persist_prepare(s, in, out))) return rc;
-            if ((rc = enqueue_layers(s, in, N, out))) return rc;
-        }
+        else if ((rc = enqueue_layers(s, in, N, out))) return rc;
         B200_CUDA(cudaEventRecord(s->ev1, s->stream));
     }
     s->timed = true;
@@ -867,7 +714,6 @@ struct LoadJob {
     int kind = 0;                 // 0: block-quantised matrix (k_repack), 1: F16 (k_repack_f16), 2: raw copy, 3: Q6_K (k_repack_q6k)
     int mode = 0, G = 1;
     PackedW * out = nullptr;      // kind 0
-    PackedW * out2 = nullptr; int TR2 = 0;   // kind 0: a second packing of the same matrix with TR2 row-groups per tile
     uint16_t ** outf = nullptr; uint16_t * into = nullptr;   // kind 1
     uint8_t * raw_dst = nullptr;  // kind 2
     size_t bytes() const { size_t n = 0; for (int i = 0; i < nsrc; i++) n += (src[i]->nbytes + 255) & ~(size_t) 255; return n; }
@@ -966,18 +812,6 @@ static int run_load_jobs(b200_slice * s, const GgjtFile & f, std::vector<LoadJob
             PackedW * out = job.out;
             out->data = dst; out->wtype = wt; out->rows = rows_per * job.nsrc; out->K = K; out->nb = nb; out->nbq = nbq; out->TR = TR;
             out->n_tiles = n_tiles; out->tile_bytes = tile_bytes;
-            if (job.out2 && job.TR2 > 0) {
-                const int TR2 = job.TR2, n_tiles2 = (total_groups + TR2 - 1) / TR2;
-                // quads per ring stage of the persistent kernel: sq * TR2 <= 16; pad nbq so a whole number of stages fits
-                int sq = 16 / TR2; while (sq > 4 && nbq % sq) sq >>= 1;
-                const long long tile_bytes2 = (long long) nbq * TR2 * chunk_bytes(wt);
-                uint8_t * dst2 = nullptr;
-                if ((rc = dev_alloc(s, &dst2, (size_t) n_tiles2 * tile_bytes2))) break;
-                ra.TR = TR2; ra.n_tiles = n_tiles2; ra.dst = dst2;
-                k_repack<<<s->n_sm * 8, 256, 0, s->stream>>>(ra);
-                PackedW * o2 = job.out2;
-                *o2 = *out; o2->data = dst2; o2->TR = TR2; o2->n_tiles = n_tiles2; o2->tile_bytes = tile_bytes2;
-            }
         } else if (job.kind == 1) {
             const GgjtTensor & t = *job.src[0];
             const int K = (int) t.ne[0], rows = (int) t.ne[1];
@@ -1143,8 +977,6 @@ static int load_locked(b200_slice * s, const char * path) {
             (rc = dev_alloc(s, &s->aq_gate, nq * s->nbqF * 32)) || (rc = dev_alloc(s, &s->da_gate, pl * nq * s->nbqF * 4))) return rc;
         if ((rc = dev_alloc(s, &s->aq_x, nq * s->nbqE * 32)) || (rc = dev_alloc(s, &s->da_x, pl * nq * s->nbqE * 4)) ||
             (rc = dev_alloc(s, &s->nq_counter, 2 * nq)) || (rc = dev_alloc(s, &s->nq_partial, nq * 256))) return rc;
-        if ((rc = dev_alloc(s, &s->p_cnt, (size_t) s->L * kPPhases + 32))) return rc;
-        B200_CUDA(cudaMemset(s->p_cnt, 0, ((size_t) s->L * kPPhases + 32) * 4));
         B200_CUDA(cudaMemset(s->aq_x, 0, nq * s->nbqE * 128)); B200_CUDA(cudaMemset(s->da_x, 0, pl * nq * s->nbqE * 16));
         B200_CUDA(cudaMemset(s->nq_counter, 0, 2 * nq * 4));
         B200_CUDA(cudaMemset(s->aq_att, 0, nq * s->nbqE * 128));  B200_CUDA(cudaMemset(s->da_att, 0, pl * nq * s->nbqE * 16));
@@ -1240,37 +1072,16 @@ int b200_slice_load_ex(const char * path, int device, int n_ctx, int n_sessions,
     s->use_nq    = env_int("B200_NQ", 0) != 0;   // grid-barrier norm+quant epilogue in wo / w2 (decode): exact, opt-in (its barrier costs what it saves)
     s->opt_ns = env_int("B200_NS", 0); s->opt_cta_per_sm = env_int("B200_CTA_PER_SM", 0); s->opt_nc = env_int("B200_NC", 0);
     s->opt_pre = env_int("B200_PRE", 3); s->opt_nomath = env_int("B200_DBG_NOMATH", 0);
-    s->use_tiled_attn = env_int("B200_TILED_ATTN", 1) != 0;
+    s->use_tiled_attn = env_int("B200_TILED_ATTN", 1) != 0;   // prompt chunks: query-tiled attention (K / V staged once per 16 queries)
     s->f16_mc = env_int("B200_F16_MC", 1) != 0;      // F16 slices, multi-token calls: 4 (8) columns per CTA share the weight loads
     s->f16_mc_cols = env_int("B200_F16_MC", 1) == 8 ? 8 : 4;
-    s->use_n8 = env_int("B200_N8", 0) != 0;          // single-token wo / w2: 8 threads per row (k_gemv_n8): exact, opt-in  // prompt chunks: query-tiled attention (K / V staged once per 16 queries)
     s->f16_ring = env_int("B200_F16_RING", 1) != 0;          // F16-weight slices: TMA-ring matmul for single-token steps
-    s->use_persist = env_int("B200_PERSIST", 0) != 0;         // single-token step as ONE persistent kernel (persist.cuh)
-    s->persist_tr = env_int("B200_PERSIST_TR", 4); s->persist_ns = env_int("B200_PERSIST_NS", 0); s->persist_ctas = env_int("B200_PERSIST_CTAS", 0);
-    if (s->persist_tr != 1 && s->persist_tr != 2 && s->persist_tr != 4) s->persist_tr = 4;
-    const bool want_ptrace = env_int("B200_PTRACE", 0) != 0;
     cudaError_t e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
     if (e != cudaSuccess) { delete s; return fail(B200_ECUDA, "cudaStreamCreate failed: %s", cudaGetErrorString(e)); }
     int rc = load_locked(s, path);
     if (rc) { destroy(s); return rc; }
-    if (want_ptrace) {
-        const size_t n = (size_t) s->n_sm * s->L * kPTraceSlots;
-        if ((rc = dev_alloc(s, &s->p_trace, n))) { destroy(s); return rc; }
-        cudaMemset(s->p_trace, 0, n * 8);
-    }
     *out = s;
     return 0;
-}
-
-/* Debug timeline of the persistent step (B200_PTRACE=1 at load): [cta][layer][16] %globaltimer stamps of the LAST step. */
-int b200_debug_ptrace_read(b200_slice_t * s, unsigned long long * out, size_t cap_words) {
-    if (!s || !s->p_trace || !out) return 0;
-    cudaSetDevice(s->device);
-    cudaStreamSynchronize(s->stream);
-    size_t n = (size_t) s->n_sm * s->L * kPTraceSlots;
-    if (n > cap_words) n = cap_words;
-    cudaMemcpy(out, s->p_trace, n * 8, cudaMemcpyDeviceToHost);
-    return (int)(n / kPTraceSlots);
 }
 
 int b200_slice_unload(b200_slice_t * s) {
@@ -1617,10 +1428,9 @@ static int pipeline_step_peer(b200_slice * s, const float * d_in, int n_rows, in
     if (!sessions) { s->cur = session; s->cols = nullptr; }
     // fold the send into the slice's last matmul for plain single-token steps of quantised, head-size-128 slices
     const bool fold = s->use_fold && sends && !sessions && n_rows == 1 && s->D == 128 && s->wtype != kWT_F16 && s->use_ring && !s->use_nq &&
-                      !persist_applicable(s, 1) && !s->skip_attention;
+                      !s->skip_attention;
     const float * in = recv_in ? s->d_in : d_in;
     int rc = 0;
-    if (!sessions && persist_applicable(s, n_rows) && (rc = persist_prepare(s, in, s->d_out))) return rc;
     auto body = [&]() -> int {
         int e;
         s->cur_class = 6;
@@ -1664,7 +1474,7 @@ static int pipeline_step_peer(b200_slice * s, const float * d_in, int n_rows, in
             it = s->pp_graphs.emplace(key, ge).first;
         }
         B200_CUDA(cudaGraphLaunch(it->second, s->stream));
-        s->launches += (persist_applicable(s, 1) ? 2 : (s->D == 128 ? 5 : 6) * s->L + 1) + (recv_in ? 1 : 0) + (sends ? 1 : 0) + (recv_final ? 1 : 0);
+        s->launches += (s->D == 128 ? 5 : 6) * s->L + 1 + (recv_in ? 1 : 0) + (sends ? 1 : 0) + (recv_final ? 1 : 0);
         s->past[session] += 1;
     } else {
         s->cur = session; s->cols = nullptr;

@@ -150,10 +150,6 @@ int b200_debug_skip_attention(b200_slice_t * s, int on);
 int b200_debug_trace_enable(b200_slice_t * s, int on);
 int b200_debug_trace_read(b200_slice_t * s, unsigned long long * out, int * cls, int * ctas, int max_launches);
 
-/* Timeline of the persistent single-token step (csrc/persist.cuh; B200_PERSIST=1 and B200_PTRACE=1 at load): 16 stamps per
- * (CTA, layer) of the most recent step; returns the number of (CTA, layer) records written. */
-int b200_debug_ptrace_read(b200_slice_t * s, unsigned long long * out, size_t cap_words);
-
 /* ---- layer-slice pipeline over NVLink (one process per GPU) --------------------------- */
 
 /* Join a pipeline of `nranks` slices (rank r holds layer range r of the nodes_map).  `nccl_id`

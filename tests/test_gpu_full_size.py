@@ -17,12 +17,19 @@ import pytest
 from distributedllm_b200 import ggjt
 
 pytestmark = pytest.mark.gpu
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HAVE_REF = os.path.isfile(os.path.join(ROOT, "oracle", "_ref", "libllmref.so"))
+THREADS = min(16, os.cpu_count() or 4)
 REF = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_digests.json")))
 MAX_CHUNK = 32          # the reference's eval arena overflows for long calls (SURVEY 8a-Q3): its prefill went in these chunks
 
 
 def _digest(a):
     return hashlib.sha256(np.ascontiguousarray(a, dtype=np.float32).tobytes()).hexdigest()
+
+
+def _bits(a):
+    return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
 def test_config1_3b_two_nodes_greedy_decode(tmp_path):
@@ -119,3 +126,29 @@ def test_config2_7b_q4_decode_at_the_end_of_the_sequence(tmp_path):
     with pytest.raises(capi.B200Error):                            # position 512 does not exist at n_ctx 512
         gpu.forward(rng.standard_normal((1, sh.n_embd), dtype=np.float32))
     gpu.close()
+
+
+def test_7b_and_13b_layers_decode_after_a_chunked_prefill(tmp_path):
+    """7B (E 4096, 32 heads) and 13B (E 5120, 40 heads) layer shapes taken to position 290 in 32-token chunks, then
+    device-resident decode steps deep in the context, against the compiled reference (the C port where it is absent)."""
+    from distributedllm_b200 import capi
+    from oracle import oracle
+    for name, layers, seed in (("7b", 2, 21), ("13b", 1, 22)):
+        sh = ggjt.SHAPES[name]
+        p = str(tmp_path / ("%s.bin" % name))
+        ggjt.write_fast_q4_slice(p, sh, 0, layers - 1, seed=seed)
+        gpu = capi.Slice(p, 0, 512)
+        ref = oracle.RefSlice(p, THREADS, 512) if HAVE_REF else oracle.PortSlice(p, 512)
+        rng = np.random.default_rng(seed)
+        pos = 0
+        while pos < 290:
+            n = min(MAX_CHUNK, 290 - pos)
+            x = rng.standard_normal((n, sh.n_embd), dtype=np.float32)
+            assert (_bits(gpu.forward(x)) == _bits(ref.forward(x))).all()
+            pos += n
+        for step in range(6):
+            x = rng.standard_normal((1, sh.n_embd), dtype=np.float32)
+            g, r = gpu.forward(x), ref.forward(x)
+            assert (_bits(g) == _bits(r)).all(), "%s step %d: %d floats differ" % (name, step, int((_bits(g) != _bits(r)).sum()))
+        gpu.close()
+        ref.close()

@@ -56,7 +56,8 @@ def test_ring_and_simple_kernels_agree(tmp_models, monkeypatch):
         assert bad == 0, "ring=%s: %d of %d floats differ" % (ring, bad, tot)
 
 
-@pytest.mark.parametrize("shape,wtype", [("tiny", ggjt.T_Q4_0), ("tiny128", ggjt.T_Q4_0), ("tiny128", ggjt.T_Q4_1)])
+@pytest.mark.parametrize("shape,wtype", [("tiny", ggjt.T_Q4_0), ("tiny128", ggjt.T_Q4_0), ("tiny128", ggjt.T_Q4_1),
+                                         ("tiny128", ggjt.T_Q8_0)])
 def test_decode_only_long(tmp_models, shape, wtype):
     sh = ggjt.SHAPES[shape]
     path = tmp_models(shape, wtype, 0, 2)
@@ -88,11 +89,9 @@ def test_f16_multi_column_kernel_is_a_scheduling_choice(tmp_models, monkeypatch,
     assert bad == 0, "%d of %d floats differ" % (bad, tot)
 
 
-@pytest.mark.parametrize("n8", ["1", "0"])
 @pytest.mark.parametrize("shape,wtype", [("tiny128", ggjt.T_Q4_0), ("tiny3b", ggjt.T_Q8_0), ("tiny", ggjt.T_Q8_0)])
-def test_narrow_matrix_kernel_is_a_scheduling_choice(tmp_models, monkeypatch, n8, shape, wtype):
-    """Single-token wo / w2 run 8 threads per row (k_gemv_n8, one AVX lane per thread) instead of 4: the same lane chains."""
-    monkeypatch.setenv("B200_N8", n8)
+def test_narrow_matrix_kernel_is_a_scheduling_choice(tmp_models, shape, wtype):
+    """Single-token wo / w2 (the narrow matrices: one CTA per SM with a deep ring) between prompt chunks."""
     sh = ggjt.SHAPES[shape]
     path = tmp_models(shape, wtype, 0, 2)
     bad, tot = _run_pair(path, [5, 1, 1, 1, 1, 30, 1, 1], sh)

@@ -81,10 +81,9 @@ def test_q5_scheduling_choices_are_exact(tmp_models, monkeypatch, env, wtype):
 
 
 @pytest.mark.parametrize("wtype", Q5, ids=IDS)
-@pytest.mark.parametrize("switch", ["B200_FAST_PREFILL", "B200_PERSIST", "B200_N8"])
+@pytest.mark.parametrize("switch", ["B200_FAST_PREFILL"])
 def test_q5_ignores_paths_it_does_not_take(tmp_models, monkeypatch, switch, wtype):
-    """The wgmma prefill, the persistent step and k_gemv_n8 cover Q4_0 / Q8_0 only: with their switches on, a Q5 slice
-    stays on the exact kernels."""
+    """The wgmma prefill covers Q4_0 / Q8_0 only: with its switch on, a Q5 slice stays on the exact kernels."""
     monkeypatch.setenv(switch, "1")
     sh = ggjt.SHAPES["tiny128"]
     path = tmp_models("tiny128", wtype, 0, 2)

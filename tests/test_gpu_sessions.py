@@ -79,3 +79,23 @@ def test_session_zero_is_the_reference_context_and_errors(tmp_models):
     assert e.value.code == 5 and a.session_n_past(0) == 0 and a.session_n_past(1) == 64
     a.close()
     b.close()
+
+
+def test_single_token_steps_interleaved_across_sessions(tmp_models):
+    """Each session's single-token step is its own graph replay: interleaved steps of three sessions at three different
+    positions equal three private slices."""
+    from distributedllm_b200 import capi
+    sh = ggjt.SHAPES["tiny128"]
+    path = tmp_models("tiny128", ggjt.T_Q4_0, 0, 1, seed=9)
+    gpu = capi.Slice(path, 0, 64, n_sessions=3)
+    priv = [capi.Slice(path, 0, 64) for _ in range(3)]
+    rng = np.random.default_rng(2)
+    for k, n in enumerate((3, 1, 6)):
+        x = rng.standard_normal((n, sh.n_embd), dtype=np.float32)
+        assert (_bits(gpu.session_forward(k, x)) == _bits(priv[k].forward(x))).all()
+    for step in range(5):
+        for k in (2, 0, 1):
+            x = rng.standard_normal((1, sh.n_embd), dtype=np.float32)
+            assert (_bits(gpu.session_forward(k, x)) == _bits(priv[k].forward(x))).all(), (step, k)
+    for s in priv + [gpu]:
+        s.close()
