@@ -117,15 +117,28 @@ static void prof_end(b200_slice * s) {
 }
 
 // ---------------------------------------------------------------- kernel dispatch
+// Dynamic shared memory of a k_gemv launch: `act` bytes for the NC columns' activations (plus the f32 input row of a
+// one-column PRO_NORM launch) and barriers, and `stage` bytes per ring stage; a launch with NS stages needs bytes(NS).
+struct GemvSmem {
+    size_t stage, act;
+    size_t bytes(int NS) const { return (size_t) NS * stage + act; }
+};
+
+template <int WT, int G, int NC, int PRO>
+static GemvSmem gemv_smem(const PackedW & W) {
+    GemvSmem m;
+    m.stage = (size_t) kQS * kWPC * G * chunk_bytes(WT);
+    m.act = (size_t) NC * act_bytes_per_col(W.nbq, WT) + 34 * 8 + kWPC * 8 + (size_t) NC * 128 + 64 +
+            ((NC == 1 && PRO == PRO_NORM) ? (size_t) W.K * 4 : 0);
+    return m;
+}
+
 template <int WT, int G, int NC, int PRO, int EPI, bool RING>
 static int launch_gemv_t(b200_slice * s, GemvArgs a) {
-    constexpr int CB = chunk_bytes(WT);
-    constexpr int TR = kWPC * G;
     auto kern = k_gemv<WT, G, NC, PRO, EPI, RING>;
     static bool attr_set[16] = {false};
-    const size_t stage = (size_t) kQS * TR * CB;
-    const size_t act = (size_t) NC * act_bytes_per_col(a.W.nbq, WT) + 34 * 8 + kWPC * 8 + (size_t) NC * 128 + 64 +
-                       ((NC == 1 && PRO == PRO_NORM) ? (size_t) a.W.K * 4 : 0);
+    const GemvSmem sm = gemv_smem<WT, G, NC, PRO>(a.W);
+    const size_t stage = sm.stage, act = sm.act;
     // Ring depth: as deep as possible while EVERY tile of the matrix still gets a co-resident CTA (no second wave):
     // wide matrices (qkv 384 tiles, w1|w3 688) run 3-5 small-ring CTAs per SM, narrow ones (wo, w2: 128 tiles) one
     // CTA per SM with a deep ring.  B200_NS overrides.
@@ -140,7 +153,7 @@ static int launch_gemv_t(b200_slice * s, GemvArgs a) {
         if (NS > 16) NS = 16;
         while (NS > 2 && NS * stage + act > (size_t) kSmemLimit) NS--;
     }
-    const size_t smem = NS * stage + act;
+    const size_t smem = sm.bytes(NS);
     if (smem > (size_t) kSmemLimit) return fail(B200_EINVAL, "gemv needs %zu B of shared memory (K=%d, NC=%d)", smem, a.W.K, NC);
     if (!attr_set[s->device & 15]) {
         B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
@@ -184,10 +197,15 @@ static int launch_gemv_nc(b200_slice * s, const GemvArgs & a) {
     // over a narrow matrix (wo / w2: 128-160 tiles) would then run ONE 4-warp CTA per SM.  Take the widest column
     // group that still puts >= 3 CTAs on every SM; the extra column groups re-read the tile from L2, not from HBM
     // (they are co-resident and walk the tiles in the same order).
+    // A group is taken only if its launch fits in shared memory with a two-stage ring: at LLaMA-65B (w2: K = 22016) eight
+    // columns of activations plus two stages exceed it for Q8_0, Q4_1 and Q5_1 weights, whose w2 launches take four.
+    // B200_NC forces a group, as an upper bound.
     const int want = 3 * s->n_sm, nt = a.W.n_tiles;
-    const int force = s->opt_nc;
-    if (force == 8 || (!force && nt * ((a.N + 7) / 8) >= want)) return launch_gemv_t<WT, G, 8, PRO, EPI, true>(s, a);
-    if (force == 4 || (!force && nt * ((a.N + 3) / 4) >= want)) return launch_gemv_t<WT, G, 4, PRO, EPI, true>(s, a);
+    const int force = s->opt_nc, cap = force > 0 ? force : 8;
+    if (cap >= 8 && gemv_smem<WT, G, 8, PRO>(a.W).bytes(2) <= (size_t) kSmemLimit && (force || nt * ((a.N + 7) / 8) >= want))
+        return launch_gemv_t<WT, G, 8, PRO, EPI, true>(s, a);
+    if (cap >= 4 && gemv_smem<WT, G, 4, PRO>(a.W).bytes(2) <= (size_t) kSmemLimit && (force || nt * ((a.N + 3) / 4) >= want))
+        return launch_gemv_t<WT, G, 4, PRO, EPI, true>(s, a);
     return launch_gemv_t<WT, G, 2, PRO, EPI, true>(s, a);
 }
 

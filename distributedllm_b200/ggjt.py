@@ -443,6 +443,8 @@ SHAPES = {
     "3b":     ModelShape(32000, 3200, 216, 32, 26),  # OpenLLaMA-3B: n_ff 8640
     "7b":     ModelShape(32000, 4096, 256, 32, 32),
     "13b":    ModelShape(32000, 5120, 256, 40, 40),
+    "30b":    ModelShape(32000, 6656, 256, 52, 60),  # n_ff 17920
+    "65b":    ModelShape(32000, 8192, 256, 64, 80),  # n_ff 22016
 }
 
 

@@ -67,6 +67,39 @@ def test_fast_generator_writes_a_loadable_slice(tmp_path):
     assert np.isfinite(y).all() and np.abs(y).max() < 100
 
 
+@pytest.mark.parametrize("name,n_embd,n_head,n_ff,n_layer", [("30b", 6656, 52, 17920, 60), ("65b", 8192, 64, 22016, 80)])
+def test_30b_and_65b_shapes(tmp_path, name, n_embd, n_head, n_ff, n_layer):
+    """LLaMA-30B and 65B: n_ff from n_mult 256 as the reference's loader derives it, head size 128, and a slice file of
+    the shape carries those dimensions in its header and tensors."""
+    sh = ggjt.SHAPES[name]
+    assert (sh.n_embd, sh.n_head, sh.n_ff, sh.n_layer) == (n_embd, n_head, n_ff, n_layer)
+    assert sh.n_embd // sh.n_head == 128 and sh.n_embd % sh.n_head == 0
+    p = str(tmp_path / "l.bin")
+    ggjt.write_fast_q4_slice(p, sh, n_layer - 1, n_layer - 1, seed=0)
+    f = ggjt.read_file(p, sliced=True)
+    assert (f.hparams.n_embd, f.hparams.n_head, f.hparams.n_ff, f.hparams.first_layer) == (n_embd, n_head, n_ff, n_layer - 1)
+    assert tuple(f.tensors["layers.%d.feed_forward.w2.weight" % (n_layer - 1)].ne) == (n_ff, n_embd)
+
+
+def test_large_shape_digests_match_their_generator():
+    """tests/golden/ref_digests_large.json holds, next to each case's digests, the parameters its inputs and weight file
+    are made from; they must be what gen_golden_large.py defines, or the GPU test would replay other inputs."""
+    import json
+    import sys
+    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+    import gen_golden_large
+    stored = json.load(open(os.path.join(ROOT, "tests", "golden", "ref_digests_large.json")))
+    want = gen_golden_large.case_list()
+    assert list(stored) == list(want)
+    for name, case in want.items():
+        assert {k: v for k, v in stored[name].items() if not k.endswith("digests")} == case, name
+        if case["kind"] == "schedule":
+            assert len(stored[name]["digests"]) == len(case["schedule"])
+        else:
+            assert len(stored[name]["prompt_digests"]) == len(case["sessions"])
+            assert [len(s) for s in stored[name]["step_digests"]] == [len(case["sessions"])] * case["n_steps"]
+
+
 def _header_symbols():
     text = open(os.path.join(ROOT, "include", "b200_slice.h")).read()
     text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)

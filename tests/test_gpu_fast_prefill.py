@@ -4,7 +4,8 @@ restatement of each matmul (tests/fast_ref.py).
 Fast mode is NOT bit-exact by design: the weight matmuls run as fp16 x fp16 -> fp32 tensor-core MMAs on operands
 that went through the reference's Q8_0 activation quantisation and one fp16 rounding each.  Stated tolerances:
   * each weight matmul (qkv, wo + residual, w1|w3 + SiLU gate, w2 + residual) against the float64 sum of the same fp16
-    operands: |y - y_ref| <= TAU * sum_k |w16 * x16| (+ one fp32 ulp of |y| for a residual add), TAU below;
+    operands: |y - y_ref| <= TAU * sum_k |w16 * x16| (+ one fp32 ulp of |y| for a residual add), TAU below (TAU_LONG
+    for K > 13824);
   * one weight matmul against exact mode (qkv of the first layer): relative RMS error <= 1e-3 (measured 2.7e-4: fp16
     operand rounding + fp32 accumulation order);
   * slice output (hidden states, 2 layers): relative RMS error <= 1.5e-2.  Most of it is not the tensor core: every
@@ -31,9 +32,25 @@ pytestmark = pytest.mark.gpu
 # The error grows with K (2.5e-7 at K = 512, 7e-7 at 4096, 1.7e-6 at 13824): the tensor core adds each k16 product
 # group into the fp32 accumulator with less than round-to-nearest accuracy (the same fp16 products summed in fp32
 # by a CPU BLAS stay below 5e-8 at K = 11008).  TAU is 4x the largest, rounded up to a power of two.  At TAU, zeroing one 32-wide activation block puts >= 99.05 % of a token's outputs outside the bound.
+# The longer K of LLaMA-30B / 65B (same GPU, same power limit), largest per case, every time in w2:
+#   30b q4_0 v2 1.80e-6   30b q8_0 v2 1.95e-6   65b q4_0 v2 2.17e-6   65b q8_0 v2 1.99e-6
+# The matmuls with K <= 6656 .. 8192 stay below 9.5e-7.  By the same rule the matmuls with K > LONG_K (w2 of 30B and
+# 65B, K = 17920 and 22016) get TAU_LONG, the others keep TAU.  Zeroing one of the 560 / 688 activation blocks moves a
+# smaller share of such a sum: at these shapes it put >= 96.78 % of a token's outputs outside the bound (30b q8_0 w2;
+# >= 98.95 % for the matmuls with K <= 8192), so they are held to LOST_BLOCK_LARGE.
 MEASURED = 1.73e-6
 TAU = 2.0 ** -17
+LONG_K = 13824
+MEASURED_LONG = 2.17e-6
+TAU_LONG = 2.0 ** -16
 assert TAU <= 2.0 ** -16 and TAU == 2.0 ** np.ceil(np.log2(4 * MEASURED))
+assert TAU_LONG <= 2.0 ** -16 and TAU_LONG == 2.0 ** np.ceil(np.log2(4 * MEASURED_LONG))
+LOST_BLOCK = 0.99
+LOST_BLOCK_LARGE = 0.95          # the 30b / 65b cases
+
+
+def tau(k: int) -> float:
+    return TAU if k <= LONG_K else TAU_LONG
 
 
 def _bits(a):
@@ -59,7 +76,8 @@ def big_models(tmp_path_factory):
 _V = {(2, ggjt.T_Q4_0): "v2-tma-n256-q4_0", (2, ggjt.T_Q8_0): "v2-tma-n256-q8_0", (1, ggjt.T_Q4_0): "v1-q4_0"}
 _LAYER_CASES = [pytest.param("tiny128b", n, v, wt, id="%d-%s" % (n, _V[(v, wt)]))
                 for (v, wt) in _V for n in (128, 200, 33, 300)]
-_LAYER_CASES += [pytest.param("7b", 512, 2, wt, id="7b-512-%s" % _V[(2, wt)]) for wt in (ggjt.T_Q4_0, ggjt.T_Q8_0)]
+_LAYER_CASES += [pytest.param(shape, 512, 2, wt, id="%s-512-%s" % (shape, _V[(2, wt)]))
+                 for shape in ("7b", "30b", "65b") for wt in (ggjt.T_Q4_0, ggjt.T_Q8_0)]
 
 
 @pytest.mark.parametrize("shape,n_tokens,version,wtype", _LAYER_CASES)
@@ -162,6 +180,10 @@ MATMUL_CASES = [
     ("7b", ggjt.T_Q4_0, 1, (300,)),
     ("13b", ggjt.T_Q4_0, 2, (300,)),
     ("3b", ggjt.T_Q4_0, 2, (300,)),                # w2: K = 8640, 67.5 quads of 128
+    ("30b", ggjt.T_Q4_0, 2, (300,)),               # w2: K = 17920
+    ("30b", ggjt.T_Q8_0, 2, (300,)),
+    ("65b", ggjt.T_Q4_0, 2, (300,)),               # w2: K = 22016
+    ("65b", ggjt.T_Q8_0, 2, (300,)),
     ("tiny128b", ggjt.T_Q4_0, 2, (128, 300)),
     ("tiny128b", ggjt.T_Q8_0, 2, (128, 300)),
     ("tiny128b", ggjt.T_Q4_0, 1, (128, 300)),
@@ -212,8 +234,8 @@ def _stacked_rows(path, names, per, sample):
     return np.concatenate(parts)
 
 
-def _outside_fraction(err_of_mutated) -> float:
-    return float(np.mean(err_of_mutated > TAU))
+def _outside_fraction(err_of_mutated, bound: float) -> float:
+    return float(np.mean(err_of_mutated > bound))
 
 
 @pytest.mark.parametrize("shape,wtype,version,ns", MATMUL_CASES, ids=_CASE_IDS)
@@ -222,7 +244,7 @@ def test_each_fast_matmul_is_within_the_float64_bound(tmp_models, big_models, mo
     the four matmuls of one layer, against fast_ref's float64 sum of the same fp16 operands.  The fp16 activations the
     kernels read are proven bit-exact through the w2 input left in xh.  Also checks, in numpy only, that the bound is
     tight enough to see one lost 32-wide K block: zeroing one activation block of one token in the reference must put
-    >= 99 % of that token's outputs outside it."""
+    >= 99 % (95 % at 30B / 65B) of that token's outputs outside it."""
     from distributedllm_b200 import capi
     monkeypatch.setenv("B200_FAST_V", str(version))
     sh = ggjt.SHAPES[shape]
@@ -278,15 +300,19 @@ def test_each_fast_matmul_is_within_the_float64_bound(tmp_models, big_models, mo
                 worst[(n, mat)] = float(e.max())
             print("\n[fast-matmul] %s %s v%d N=%d  max normalised error  %s" % (
                 shape, ggjt.TYPE_NAME[wtype], version, n, "  ".join("%s %.3g" % (m, worst[(n, m)]) for m in errs)))
+            bound = {mat: tau(FF if mat == "w2" else E) for mat in errs}
             for mat, e in errs.items():
-                assert e.max() <= TAU, "%s N=%d: normalised error %.3g > TAU %.3g at %d outputs" % (
-                    mat, n, e.max(), TAU, int((e > TAU).sum()))
+                assert e.max() <= bound[mat], "%s N=%d: normalised error %.3g > TAU %.3g at %d outputs" % (
+                    mat, n, e.max(), bound[mat], int((e > bound[mat]).sum()))
+            floor = LOST_BLOCK_LARGE if shape in ("30b", "65b") else LOST_BLOCK
             for mat, (xa, err_of) in moved.items():
                 xm = xa[t:t + 1].copy()
                 blk = (xm.shape[1] // 32) // 3
                 xm[0, blk * 32:(blk + 1) * 32] = 0
-                frac = _outside_fraction(err_of(xm))
-                assert frac >= 0.99, "%s N=%d: a lost K block moves only %.3f of the outputs outside the bound" % (mat, n, frac)
+                frac = _outside_fraction(err_of(xm), bound[mat])
+                print("[fast-matmul] %s %s v%d N=%d  %s: a lost K block moves %.4f of the outputs outside the bound" % (
+                    shape, ggjt.TYPE_NAME[wtype], version, n, mat, frac))
+                assert frac >= floor, "%s N=%d: a lost K block moves only %.3f of the outputs outside the bound" % (mat, n, frac)
     finally:
         gpu.close()
     print("[fast-matmul] %s %s v%d  largest %.3g (2^%.2f)  %.1f s" % (

@@ -135,6 +135,45 @@ def test_q4_1_dot_is_scale_chain_plus_min_chain():
     assert (np.abs(ggjt.dequantize_q4_1(blk) - xw).reshape(4, 2, 32).max(2) <= step * 0.51 + 2e-3).all()
 
 
+@pytest.mark.skipif(not oracle.have_ref(), reason="oracle/_ref is not built (it needs the reference sources)")
+@pytest.mark.parametrize("wtype", [ggjt.T_Q4_0, ggjt.T_Q8_0], ids=["q4_0", "q8_0"])
+def test_port_matches_live_reference_at_65b(wtype, tmp_path):
+    """One LLaMA-65B layer (n_embd 8192, 64 heads, n_ff 22016): the C restatement against the compiled reference, bit for
+    bit, on a prompt, a multi-token call and single-token steps -- the C port is the GPU tests' fallback checker."""
+    sh = ggjt.SHAPES["65b"]
+    path = str(tmp_path / "l.bin")
+    ggjt.write_fast_q4_slice(path, sh, 0, 0, seed=3, wtype=wtype)
+    port, ref = oracle.PortSlice(path, 64), oracle.RefSlice(path, min(16, os.cpu_count() or 4), 64)
+    rng = np.random.default_rng(12)
+    try:
+        for i, n in enumerate((9, 1, 3, 1)):
+            x = rng.standard_normal((n, sh.n_embd), dtype=np.float32)
+            a, b = port.forward(x), ref.forward(x)
+            assert np.isfinite(b).all()
+            assert (_bits(a) == _bits(b)).all(), "call %d (N=%d): %d floats differ" % (i, n, int((_bits(a) != _bits(b)).sum()))
+    finally:
+        port.close()
+        ref.close()
+
+
+@pytest.mark.parametrize("name", ["65b_q4_0", "65b_q8_0"])
+def test_port_matches_reference_digests_at_65b(name, tmp_path):
+    """The same, without the reference built: the C restatement reproduces the reference's digests of a whole 65B case of
+    tests/golden/ref_digests_large.json (a 32-token prompt, calls of 9, 17 and 5 tokens, then 8 single-token steps)."""
+    import sys
+    sys.path.insert(0, GOLD)
+    import gen_golden_large as large
+    case = json.load(open(os.path.join(GOLD, "ref_digests_large.json")))[name]
+    path = str(tmp_path / "l.bin")
+    large.write_slice(path, case["shape"], case["wtype"], case["seed"])
+    port = oracle.PortSlice(path, case["n_ctx"])
+    try:
+        for i, x in enumerate(large.case_inputs(case)):
+            assert _digest(port.forward(x)) == case["digests"][i], "call %d (N=%d) differs from the reference" % (i, len(x))
+    finally:
+        port.close()
+
+
 def test_fast_q4_1_writer_files_are_valid_for_the_reference(tmp_path):
     """The benchmark generator's Q4_1 files (random 20-byte blocks, ggjt.write_fast_q4_slice) load in the compiled reference
     and the C restatement agrees with it on them, prompt and single-token steps."""
