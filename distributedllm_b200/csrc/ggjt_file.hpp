@@ -14,7 +14,8 @@
 
 namespace b200 {
 
-enum GgmlType : uint32_t { GT_F32 = 0, GT_F16 = 1, GT_Q4_0 = 2, GT_Q4_1 = 3, GT_Q5_0 = 6, GT_Q5_1 = 7, GT_Q8_0 = 8, GT_Q6_K = 14 };
+enum GgmlType : uint32_t { GT_F32 = 0, GT_F16 = 1, GT_Q4_0 = 2, GT_Q4_1 = 3, GT_Q5_0 = 6, GT_Q5_1 = 7, GT_Q8_0 = 8,
+                         GT_Q2_K = 10, GT_Q3_K = 11, GT_Q4_K = 12, GT_Q5_K = 13, GT_Q6_K = 14 };
 
 struct GgjtTensor {
     std::string name;
@@ -41,6 +42,10 @@ struct GgjtFile {
             case GT_Q5_0: return nelem / 32 * 22;
             case GT_Q5_1: return nelem / 32 * 24;
             case GT_Q8_0: return nelem / 32 * 34;
+            case GT_Q2_K: return nelem / 256 * 84;
+            case GT_Q3_K: return nelem / 256 * 110;
+            case GT_Q4_K: return nelem / 256 * 144;
+            case GT_Q5_K: return nelem / 256 * 176;
             case GT_Q6_K: return nelem / 256 * 210;
             default: throw std::runtime_error("unrecognized tensor type " + std::to_string(type));
         }

@@ -5,6 +5,7 @@
 // one H100.  One stream per slice; the N=1 decode step is a CUDA graph replayed per token with
 // the position kept in device memory.
 #include "kernels.cuh"
+#include "kquant.cuh"
 #include "fastgemm.cuh"
 #include "fastgemm2.cuh"
 #include "ggjt_file.hpp"
@@ -28,6 +29,9 @@ constexpr int kSmemLimit = 226 * 1024;   // opt-in dynamic limit is 227 KB minus
 
 struct LayerW {
     PackedW qkv{}, wo{}, w13{}, w2{};
+    // k-quant slices: wq / wk / wv of different types are packed per run of one type (qkv holds the first run); the
+    // other runs write rows qkv_row[i] onward of the same qkv output
+    PackedW qkv_more[2]{}; int qkv_row[2] = {0, 0};
     // F16-weight slices
     uint16_t * f_q = nullptr, * f_k = nullptr, * f_v = nullptr, * f_o = nullptr, * f_1 = nullptr, * f_2 = nullptr, * f_3 = nullptr;
     float * attn_norm = nullptr, * ffn_norm = nullptr;
@@ -87,6 +91,8 @@ struct b200_slice {
     // single-token steps fold the send into the slice's last matmul (EPI_RESID_SEND): rows leave for the next rank's inbox
     // as they are computed, no k_peer_send launch on the critical path
     bool fold_send = false, use_fold = true;
+    // k-quant slices: the Q8_K input of the next matmul, quantised once per column (k_quant_q8k, PRO_PREQ)
+    int * kq_aq = nullptr; float * kq_ad = nullptr;
     std::map<GraphKey, cudaGraphExec_t> pp_graphs;
 };
 
@@ -127,6 +133,11 @@ struct GemvSmem {
 template <int WT, int G, int NC, int PRO>
 static GemvSmem gemv_smem(const PackedW & W) {
     GemvSmem m;
+    if constexpr (wt_kquant(WT)) {
+        m.stage = (size_t) kKQS * kWPC * G * kq_chunk_bytes(WT);
+        m.act = kq_act_bytes(W.nbq, NC) + 34 * 8 + 64;
+        return m;
+    }
     m.stage = (size_t) kQS * kWPC * G * chunk_bytes(WT);
     m.act = (size_t) NC * act_bytes_per_col(W.nbq, WT) + 34 * 8 + kWPC * 8 + (size_t) NC * 128 + 64 +
             ((NC == 1 && PRO == PRO_NORM) ? (size_t) W.K * 4 : 0);
@@ -134,8 +145,14 @@ static GemvSmem gemv_smem(const PackedW & W) {
 }
 
 template <int WT, int G, int NC, int PRO, int EPI, bool RING>
+static constexpr auto gemv_kernel() {
+    if constexpr (wt_kquant(WT)) return k_gemv_kq<WT, G, NC, PRO, EPI, RING>;
+    else return k_gemv<WT, G, NC, PRO, EPI, RING>;
+}
+
+template <int WT, int G, int NC, int PRO, int EPI, bool RING>
 static int launch_gemv_t(b200_slice * s, GemvArgs a) {
-    auto kern = k_gemv<WT, G, NC, PRO, EPI, RING>;
+    auto kern = gemv_kernel<WT, G, NC, PRO, EPI, RING>();
     static bool attr_set[16] = {false};
     const GemvSmem sm = gemv_smem<WT, G, NC, PRO>(a.W);
     const size_t stage = sm.stage, act = sm.act;
@@ -219,6 +236,29 @@ static int launch_gemv(b200_slice * s, const GemvArgs & a) {
     case kWT_Q8_0: return launch_gemv_nc<kWT_Q8_0, G, PRO, EPI>(s, a);
     default: return fail(B200_EINVAL, "no block-quantised matmul for weight type %d", a.W.wtype);
     }
+}
+
+// Q4_K / Q6_K matrices (kquant.cuh): the type is per matrix, the activations are always Q8_K, quantised in the prologue
+template <int G, int PRO, int EPI>
+static int launch_gemv_kq(b200_slice * s, const GemvArgs & a) {
+    switch (a.W.wtype) {
+    case kWT_Q4_K: return launch_gemv_nc<kWT_Q4_K, G, PRO, EPI>(s, a);
+    case kWT_Q6_K: return launch_gemv_nc<kWT_Q6_K, G, PRO, EPI>(s, a);
+    default: return fail(B200_EINVAL, "no k-quant matmul for weight type %d", a.W.wtype);
+    }
+}
+
+template <typename K, typename A>
+static int launch_simple(b200_slice * s, K kern, dim3 grid, dim3 block, size_t smem, const A & args);
+
+// The input of a k-quant matmul: [RMSNorm * norm_w ->] Q8_K of its N columns, once per column (k_quant_q8k), into the
+// slice's Q8_K buffer, from which the matmul's CTAs fetch it (PRO_PREQ).
+static int quant_kq(b200_slice * s, GemvArgs & a, bool norm) {
+    const int nbq = a.W.nbq;
+    QuantKArgs q{a.x, a.ldx, a.norm_w, a.W.K, s->kq_aq, s->n_ctx * nbq * 64, s->kq_ad, nbq};
+    a.aq_in = s->kq_aq; a.in_soff = q.soff; a.da_in = s->kq_ad;
+    return norm ? launch_simple(s, k_quant_q8k<true>, dim3(a.N, 1, 1), dim3(256, 1, 1), 0, q)
+                : launch_simple(s, k_quant_q8k<false>, dim3(a.N, 1, 1), dim3(256, 1, 1), 0, q);
 }
 
 template <typename K, typename A>
@@ -415,7 +455,9 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
                           (Lw.qkv.n_tiles * Lw.qkv.TR) % 16 == 0 &&
                           (Lw.wo.n_tiles * Lw.wo.TR) % 16 == 0 && (Lw.w13.n_tiles * Lw.w13.TR) % 16 == 0;
         // grid-barrier norm+quant epilogue: decode only (every CTA of wo / w2 must be co-resident: 1 tile per CTA)
-        const bool nq = s->use_nq && N == 1 && !s->cols && s->wtype != kWT_F16 && Lw.wo.n_tiles <= 256 && Lw.wo.n_tiles <= s->n_sm * 2;
+        // k-quant slices (Q4_K / Q6_K in any mix) take the exact kernels of kquant.cuh: no fast mode, no NQ epilogue
+        const bool kq = wt_kquant(s->wtype);
+        const bool nq = s->use_nq && N == 1 && !s->cols && s->wtype != kWT_F16 && !kq && Lw.wo.n_tiles <= 256 && Lw.wo.n_tiles <= s->n_sm * 2;
         float * nxt = (il == s->L - 1) ? out : ((il & 1) ? s->xb : s->xa);
         // cols mode (batched independent sequences): the kernels add session * sess_stride themselves
         const size_t sess_off = s->cols ? 0 : (size_t) s->cur * s->sess_stride;
@@ -427,6 +469,14 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
             GemvF16Args f{}; f.K = E; f.x = cur; f.ldx = E; f.norm_w = Lw.attn_norm; f.N = N; f.tsilu = s->tsilu;
             f.rows = 3 * E; f.ldy = 3 * E;       // wq | wk | wv are packed back to back: one launch, one RMSNorm prologue
             f.W = Lw.f_q; f.y = s->qkv;         if ((rc = launch_f16<PRO_NORM, EPI_STORE>(s, f))) return rc;
+        } else if (kq) {
+            GemvArgs g{}; g.W = Lw.qkv; g.x = cur; g.ldx = E; g.norm_w = Lw.attn_norm; g.y = s->qkv; g.ldy = 3 * E;
+            g.N = N; g.out_rows = Lw.qkv.rows; g.tsilu = s->tsilu;
+            if ((rc = quant_kq(s, g, true)) || (rc = launch_gemv_kq<1, PRO_PREQ, EPI_STORE>(s, g))) return rc;
+            for (int i = 0; i < 2 && Lw.qkv_more[i].data; i++) {       // wq | wk and wv of different types: same input and rows, exact
+                g.W = Lw.qkv_more[i]; g.y = s->qkv + Lw.qkv_row[i]; g.out_rows = Lw.qkv_more[i].rows;
+                if ((rc = launch_gemv_kq<1, PRO_PREQ, EPI_STORE>(s, g))) return rc;
+            }
         } else if (fast) {
             if ((rc = launch_prep<true>(s, cur, E, Lw.attn_norm, E, N))) return rc;
             if ((rc = launch_fast_any<FG_STORE>(s, Lw.qkv, nullptr, 0, s->qkv, 3 * E, N, 3 * E))) return rc;
@@ -459,8 +509,8 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
             aa.cols = s->cols; aa.sess_stride = s->sess_stride;
             aa.cs = s->cs; aa.texp = s->texp; aa.out = s->att;
             aa.n_ctx = s->n_ctx; aa.kq_scale = 1.0f / sqrtf((float) E / (float) H);
-            const bool preq = s->wtype != kWT_F16;
-            const float dsc = wt_act_scale(s->wtype);
+            const bool preq = s->wtype != kWT_F16 && !kq;       // k-quant wo quantises the f32 s->att itself
+            const float dsc = preq ? wt_act_scale(s->wtype) : 0.f;
             if (preq) { aa.aq_out = s->aq_att; aa.da_out = s->da_att; aa.out_nbq = s->nbqE; aa.out_dscale = dsc; aa.out_soff = s->soffE; }
             if (s->cols) {
                 // every column is an independent N = 1 step: the fused (RoPE + append) kernel, one cluster row per column
@@ -527,6 +577,26 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
             GemvF16Args w{}; w.K = FF; w.x = s->gate; w.ldx = FF; w.N = N; w.tsilu = s->tsilu;
             w.rows = E; w.W = Lw.f_2; w.resid = s->ffin; w.ldr = E; w.y = nxt; w.ldy = E;
             if ((rc = launch_f16<PRO_PLAIN, EPI_RESID>(s, w))) return rc;
+        } else if (kq) {
+            s->cur_class = 3;
+            GemvArgs o{}; o.W = Lw.wo; o.x = s->att; o.ldx = E; o.resid = cur; o.ldr = E; o.y = s->ffin; o.ldy = E;
+            o.N = N; o.out_rows = E; o.tsilu = s->tsilu;
+            if ((rc = quant_kq(s, o, false)) || (rc = launch_gemv_kq<1, PRO_PREQ, EPI_RESID>(s, o))) return rc;
+            s->cur_class = 4;
+            GemvArgs g{}; g.W = Lw.w13; g.x = s->ffin; g.ldx = E; g.norm_w = Lw.ffn_norm; g.y = s->gate; g.ldy = FF;
+            g.N = N; g.out_rows = FF; g.tsilu = s->tsilu;
+            if ((rc = quant_kq(s, g, true)) || (rc = launch_gemv_kq<2, PRO_PREQ, EPI_GATE>(s, g))) return rc;
+            s->cur_class = 5;
+            GemvArgs w{}; w.W = Lw.w2; w.x = s->gate; w.ldx = FF; w.resid = s->ffin; w.ldr = E; w.y = nxt; w.ldy = E;
+            w.N = N; w.out_rows = E; w.tsilu = s->tsilu;
+            if ((rc = quant_kq(s, w, false))) return rc;
+            if (s->fold_send && il == s->L - 1) {
+                w.mb_mine = (MailboxHdr *) s->mb_block;
+                w.mb_peer_inbox = (uint2 *)(s->mb_next + sizeof(MailboxHdr)); w.mb_slot_elems = s->mb_slot_floats;
+                rc = Lw.w2.wtype == kWT_Q4_K ? launch_gemv_t<kWT_Q4_K, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w)
+                                             : launch_gemv_t<kWT_Q6_K, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
+                if (rc) return rc;
+            } else if ((rc = launch_gemv_kq<1, PRO_PREQ, EPI_RESID>(s, w))) return rc;
         } else if (fast) {
             s->cur_class = 3;
             if ((rc = launch_prep<false>(s, s->att, E, nullptr, E, N))) return rc;
@@ -606,11 +676,20 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
     return 0;
 }
 
+// kernel launches of one captured single-token step over the slice (k-quant slices: + one k_quant_q8k per matmul input,
+// + one launch per extra qkv run)
+static int step_launches(const b200_slice * s) {
+    int n = (s->D == 128 ? 5 : 6) * s->L + 1;
+    for (const LayerW & Lw : s->layers) n += (Lw.qkv_more[0].data ? 1 : 0) + (Lw.qkv_more[1].data ? 1 : 0);
+    if (wt_kquant(s->wtype)) n += 4 * s->L;
+    return n;
+}
+
 // N = 1: replay a captured graph (host variant adds the H2D / D2H copies as graph nodes)
 static int run_decode_graph(b200_slice * s, const float * in, float * out, bool host) {
     GraphKey key{in, out, (host ? 1 : 0) | (s->skip_attention ? 2 : 0) | (s->send_pending ? 4 : 0) | (s->cur << 3)};
     auto it = s->graphs.find(key);
-    const int per_step = (s->D == 128 ? 5 : 6) * s->L + 1;
+    const int per_step = step_launches(s);
     if (it == s->graphs.end()) {
         const int64_t before = s->launches;
         cudaGraph_t g = nullptr;
@@ -814,11 +893,13 @@ static int run_load_jobs(b200_slice * s, const GgjtFile & f, std::vector<LoadJob
         if (e != cudaSuccess) { rc = fail(B200_ECUDA, "weight upload failed: %s", cudaGetErrorString(e)); break; }
         if (job.kind == 0) {
             const int wt = (int) job.src[0]->type;
+            const bool kqt = wt_kquant(wt);             // k-quants: nb / nbq count 256-wide super-blocks
             const int K = (int) job.src[0]->ne[0], rows_per = (int) job.src[0]->ne[1];
-            const int nb = K / 32, nbq = ((nb + 3) / 4 + kQS - 1) / kQS * kQS, TR = kWPC * job.G;
+            const int nb = kqt ? K / 256 : K / 32, TR = kWPC * job.G;
+            const int nbq = kqt ? (nb + kKQS - 1) / kKQS * kKQS : ((nb + 3) / 4 + kQS - 1) / kQS * kQS;
             const int total_groups = (rows_per + 7) / 8 * job.nsrc;
             const int n_tiles = (total_groups + TR - 1) / TR;
-            const long long tile_bytes = (long long) nbq * TR * chunk_bytes(wt);
+            const long long tile_bytes = (long long) nbq * TR * (kqt ? kq_chunk_bytes(wt) : chunk_bytes(wt));
             uint8_t * dst = nullptr;
             if ((rc = dev_alloc(s, &dst, (size_t) n_tiles * tile_bytes))) break;
             RepackArgs ra{};
@@ -826,7 +907,8 @@ static int run_load_jobs(b200_slice * s, const GgjtFile & f, std::vector<LoadJob
             for (int i = 0; i < job.nsrc; i++) { ra.src[i] = lp.scratch[slot] + off; off += (job.src[i]->nbytes + 255) & ~(size_t) 255; }
             ra.mode = job.mode; ra.wtype = wt; ra.rows_per_src = rows_per; ra.nb = nb; ra.nbq = nbq; ra.TR = TR; ra.n_tiles = n_tiles;
             ra.dst = dst;
-            k_repack<<<s->n_sm * 8, 256, 0, s->stream>>>(ra);
+            if (kqt) k_repack_kq<<<s->n_sm * 8, 256, 0, s->stream>>>(ra);
+            else k_repack<<<s->n_sm * 8, 256, 0, s->stream>>>(ra);
             PackedW * out = job.out;
             out->data = dst; out->wtype = wt; out->rows = rows_per * job.nsrc; out->K = K; out->nb = nb; out->nbq = nbq; out->TR = TR;
             out->n_tiles = n_tiles; out->tile_bytes = tile_bytes;
@@ -924,8 +1006,12 @@ static int load_locked(b200_slice * s, const char * path) {
     try {
         const std::string p0 = "layers." + std::to_string(s->first_layer);
         s->wtype = (int) f.get(p0 + ".attention.wq.weight", {E, E}).type;
-        if (!wt_block_quant(s->wtype) && s->wtype != kWT_F16)
-            return fail(B200_EFILE, "weight type %d unsupported (Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, F16)", s->wtype);
+        const bool kq = wt_kquant(s->wtype);
+        if (!wt_block_quant(s->wtype) && s->wtype != kWT_F16 && !kq)
+            return fail(B200_EFILE, "weight type %d unsupported (Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, F16, Q4_K, Q6_K): %s", s->wtype,
+                        (p0 + ".attention.wq.weight").c_str());
+        if (kq && (E % 256 || FF % 256))
+            return fail(B200_EFILE, "k-quant slice needs n_embd and n_ff divisible by 256 (n_embd %u, n_ff %u)", E, FF);
         float * d_norms = nullptr;
         if ((rc = dev_alloc(s, &d_norms, (size_t) s->L * 2 * E))) return rc;
         norms.resize((size_t) s->L * 2 * E);
@@ -942,8 +1028,15 @@ static int load_locked(b200_slice * s, const char * path) {
             const GgjtTensor & w2 = f.get(p + ".feed_forward.w2.weight", {FF, E});
             const GgjtTensor & w3 = f.get(p + ".feed_forward.w3.weight", {E, FF});
             if (an.type != GT_F32 || fn.type != GT_F32) return fail(B200_EFILE, "norm weights must be F32");
-            for (const GgjtTensor * t : {&wq, &wk, &wv, &wo, &w1, &w2, &w3})
-                if ((int) t->type != s->wtype) return fail(B200_EFILE, "mixed weight types in slice (%s)", t->name.c_str());
+            for (const GgjtTensor * t : {&wq, &wk, &wv, &wo, &w1, &w2, &w3}) {
+                // a k-quant slice holds Q4_K and Q6_K matrices in any mix (Q4_K_S / Q4_K_M / Q6_K files)
+                if (kq && !wt_kquant((int) t->type))
+                    return fail(B200_EFILE, "%s has type %u: a k-quant slice takes Q4_K (12) and Q6_K (14) matrices only", t->name.c_str(), t->type);
+                if (!kq && (int) t->type != s->wtype) return fail(B200_EFILE, "mixed weight types in slice (%s)", t->name.c_str());
+            }
+            if (kq && w1.type != w3.type)
+                return fail(B200_EFILE, "%s (type %u) and %s (type %u) differ: w1 and w3 are packed together", w1.name.c_str(), w1.type,
+                            w3.name.c_str(), w3.type);
             Lw.attn_norm = d_norms + (size_t) i * 2 * E; Lw.ffn_norm = Lw.attn_norm + E;
             memcpy(norms.data() + (size_t) i * 2 * E, f.data(an), (size_t) E * 4);
             memcpy(norms.data() + (size_t) i * 2 * E + E, f.data(fn), (size_t) E * 4);
@@ -958,7 +1051,18 @@ static int load_locked(b200_slice * s, const char * path) {
                     jobs.push_back(j);
                 }
             } else {
-                LoadJob a; a.nsrc = 3; a.src[0] = &wq; a.src[1] = &wk; a.src[2] = &wv; a.mode = 1; a.G = 1; a.out = &Lw.qkv; jobs.push_back(a);
+                // wq | wk | wv back to back, cut into runs of one type (only k-quant slices mix types)
+                const GgjtTensor * qkv[3] = {&wq, &wk, &wv};
+                for (int t0 = 0, part = 0; t0 < 3; part++) {
+                    int t1 = t0 + 1;
+                    while (t1 < 3 && qkv[t1]->type == qkv[t0]->type) t1++;
+                    LoadJob a; a.nsrc = t1 - t0; a.mode = a.nsrc > 1 ? 1 : 0; a.G = 1;
+                    for (int k = t0; k < t1; k++) a.src[k - t0] = qkv[k];
+                    a.out = part == 0 ? &Lw.qkv : &Lw.qkv_more[part - 1];
+                    if (part > 0) Lw.qkv_row[part - 1] = t0 * (int) E;
+                    jobs.push_back(a);
+                    t0 = t1;
+                }
                 LoadJob o; o.nsrc = 1; o.src[0] = &wo; o.mode = 0; o.G = 1; o.out = &Lw.wo;
                 jobs.push_back(o);
                 LoadJob g; g.nsrc = 2; g.src[0] = &w1; g.src[1] = &w3; g.mode = 2; g.G = 2; g.out = &Lw.w13; jobs.push_back(g);
@@ -985,7 +1089,12 @@ static int load_locked(b200_slice * s, const char * path) {
         (rc = dev_alloc(s, &s->d_out, nE)) || (rc = dev_alloc(s, &s->d_npast, (size_t) s->n_sessions)))
         return rc;
     if ((rc = dev_alloc(s, &s->xh, (size_t) s->n_ctx * (FF > E ? FF : E) + 64))) return rc;
-    if (s->wtype != kWT_F16) {
+    if (wt_kquant(s->wtype)) {
+        const int nbq = std::max(s->layers[0].wo.nbq, s->layers[0].w2.nbq);   // K = n_embd and K = n_ff
+        if ((rc = dev_alloc(s, &s->kq_aq, (size_t) s->n_ctx * nbq * 72)) || (rc = dev_alloc(s, &s->kq_ad, (size_t) s->n_ctx * kq_nbd(nbq))))
+            return rc;
+    }
+    if (s->wtype != kWT_F16 && !wt_kquant(s->wtype)) {
         s->nbqE = s->layers[0].wo.nbq; s->nbqF = s->layers[0].w2.nbq;
         const size_t nq = (size_t) s->n_ctx;
         // Q4_1 / Q5_1: every scale array carries a second plane (Q8_1's block sums s) right behind the scales
@@ -1445,7 +1554,8 @@ static int pipeline_step_peer(b200_slice * s, const float * d_in, int n_rows, in
     const int xfer_ctas = (int) std::min<size_t>(32, (count + 8191) / 8192);      // one CTA per 8 K elements, at most 32
     if (!sessions) { s->cur = session; s->cols = nullptr; }
     // fold the send into the slice's last matmul for plain single-token steps of quantised, head-size-128 slices
-    const bool fold = s->use_fold && sends && !sessions && n_rows == 1 && s->D == 128 && s->wtype != kWT_F16 && s->use_ring && !s->use_nq &&
+    const bool fold = s->use_fold && sends && !sessions && n_rows == 1 && s->D == 128 && s->wtype != kWT_F16 && s->use_ring &&
+                      (!s->use_nq || wt_kquant(s->wtype)) &&
                       !s->skip_attention;
     const float * in = recv_in ? s->d_in : d_in;
     int rc = 0;
@@ -1492,7 +1602,7 @@ static int pipeline_step_peer(b200_slice * s, const float * d_in, int n_rows, in
             it = s->pp_graphs.emplace(key, ge).first;
         }
         B200_CUDA(cudaGraphLaunch(it->second, s->stream));
-        s->launches += (s->D == 128 ? 5 : 6) * s->L + 1 + (recv_in ? 1 : 0) + (sends ? 1 : 0) + (recv_final ? 1 : 0);
+        s->launches += step_launches(s) + (recv_in ? 1 : 0) + (sends ? 1 : 0) + (recv_final ? 1 : 0);
         s->past[session] += 1;
     } else {
         s->cur = session; s->cols = nullptr;
@@ -1783,6 +1893,8 @@ __global__ void k_embed_rows(const uint8_t * emb, int type, int E, const int32_t
             const int x = (j < 16 ? (q & 0x0F) : (q >> 4)) | (((qh[j >> 3] >> (j & 7)) & 1) << 4);
             if (q51) v = fadd(fmul((float) x, d), h2f(*(const uint16_t *)(blk + 2)));   // x * d, then + m (two roundings)
             else     v = fmul((float)(x - 16), d);
+        } else if (type == kWT_Q4_K) {
+            v = dequant_q4k(emb + ((size_t) t * (E / 256) + i / 256) * 144, i & 255);
         } else if (type == kWT_Q8_0) {
             const uint8_t * blk = emb + ((size_t) t * (E / 32) + i / 32) * 34;
             v = fmul((float)((const int8_t *)(blk + 2))[i & 31], h2f(*(const uint16_t *) blk));
@@ -1921,8 +2033,9 @@ int b200_extra_load(const char * path, int device, b200_extra_t ** out) {
         const GgjtTensor & tn = f.get("norm.weight", {E});
         const GgjtTensor & to = f.get("output.weight", {E, V});
         e->emb_type = (int) te.type; e->out_type = (int) to.type;
-        if (!wt_block_quant((int) te.type) && te.type != GT_F16 && te.type != GT_F32)
+        if (!wt_block_quant((int) te.type) && te.type != GT_F16 && te.type != GT_F32 && te.type != GT_Q4_K)
             return fail(B200_EFILE, "tok_embeddings type %u unsupported", te.type);
+        if (te.type == GT_Q4_K && E % 256) return fail(B200_EFILE, "Q4_K tok_embeddings needs n_embd %% 256 == 0");
         if (!wt_block_quant((int) to.type) && to.type != GT_F16 && to.type != GT_Q6_K)
             return fail(B200_EFILE, "output.weight type %u unsupported (Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, F16, Q6_K)", to.type);
         if (to.type == GT_Q6_K && E % 256) return fail(B200_EFILE, "Q6_K output.weight needs n_embd %% 256 == 0");

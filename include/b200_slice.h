@@ -29,7 +29,8 @@ typedef struct b200_extra b200_extra_t;
 enum {
     B200_OK       = 0,
     B200_EINVAL   = 1,   /* bad argument (null handle, n_tokens <= 0, ...) */
-    B200_EFILE    = 2,   /* slice file missing / malformed / unsupported tensor type (layers: Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, F16) */
+    B200_EFILE    = 2,   /* slice file missing / malformed / unsupported tensor type (layers: Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, F16,
+                            or Q4_K / Q6_K matrices in any mix; weight_type is then the first layer's wq type) */
     B200_ENODEV   = 3,   /* no CUDA device, or device is not sm_90 */
     B200_ECUDA    = 4,   /* a CUDA call or kernel failed */
     B200_ECONTEXT = 5,   /* n_past + n_tokens would exceed n_ctx */
@@ -102,7 +103,7 @@ int b200_batch_forward(b200_slice_t * s, const int * sessions, int n_seq, const 
 int b200_batch_forward_device(b200_slice_t * s, const int * sessions, int n_seq, const float * d_in, float * d_out, int sync);
 
 /* Fast mode for prefill calls (n_tokens >= min_tokens): the Q4_0 / Q8_0 weight matmuls run on the wgmma tensor cores with
- * the dequantisation fused in (csrc/fastgemm2.cuh; Q4_1, Q5_0, Q5_1 and F16 slices ignore the switch and stay exact).
+ * the dequantisation fused in (csrc/fastgemm2.cuh; Q4_1, Q5_0, Q5_1, Q4_K / Q6_K and F16 slices ignore the switch and stay exact).
  * NOT bit-exact: operands are rounded to fp16 after the reference's Q8_0 activation quantisation and summed in fp32.
  * Each matmul output is within TAU * sum_k |w16 * x16| of the float64 sum of the same fp16 operands (TAU <= 2^-16, see
  * tests/test_gpu_fast_prefill.py, which also bounds the deviation from exact mode).  Off by default (or
