@@ -16,7 +16,7 @@ LIB = os.path.join(HERE, "libb200slice.so")
 LLM = os.path.join(HERE, "llm" + sysconfig.get_config_var("EXT_SUFFIX"))
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
-CU_SOURCES = ["runtime.cu"]          # one translation unit: kernels.cuh / fastgemm.cuh are headers of it
+CU_SOURCES = ["runtime.cu"]          # one translation unit: kernels.cuh / fastgemm2.cuh are headers of it
 
 
 def _newer(target: str, deps) -> bool:

@@ -6,7 +6,6 @@
 // the position kept in device memory.
 #include "kernels.cuh"
 #include "kquant.cuh"
-#include "fastgemm.cuh"
 #include "fastgemm2.cuh"
 #include "ggjt_file.hpp"
 
@@ -21,6 +20,7 @@
 #include <memory>
 #include <mutex>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 namespace b200 {
@@ -72,7 +72,6 @@ struct b200_slice {
     bool skip_attention = false;   // measurement aid: replay only the weight matmuls of a step (bench.py roofline)
     bool attn_lut_smem = true;     // single-token attention stages the exp table in shared memory (decided at load)
     bool fast_prefill = false; int fast_min_tokens = 32; uint16_t * xh = nullptr;   // tensor-core prefill (fast mode)
-    int fast_version = 2;                                                               // 2: fastgemm2.cuh (TMA tensor map, N = 256), 1: fastgemm.cuh
     int opt_ns = 0, opt_cta_per_sm = 0, opt_nc = 0, opt_pre = 3, opt_nomath = 0;   // read once at load (environment)
     float ema_token_ms = 0.f;              // host-buffer decode calls: smoothed device time of one token (sleep-then-poll wait)
     std::mutex mu;
@@ -122,7 +121,61 @@ static void prof_end(b200_slice * s) {
     s->prof_used += 2;
 }
 
-// ---------------------------------------------------------------- kernel dispatch
+// ---------------------------------------------------------------- kernel launch
+// Every kernel of a forward goes through here: programmatic dependent launch when enabled, the per-launch profile
+// events and the launch count.
+template <typename K, typename... A>
+static int launch(b200_slice * s, K kern, dim3 grid, dim3 block, size_t smem, const A &... args) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s->stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = s->use_pdl ? 1 : 0;
+    prof_begin(s);
+    B200_CUDA(cudaLaunchKernelEx(&cfg, kern, args...));
+    prof_end(s);
+    s->launches++;
+    return 0;
+}
+
+// A kernel's opt-in dynamic shared memory limit (with `carveout`, also the largest shared-memory carve-out), set once per
+// device.  The flags are per kernel because every kernel is its own template argument (the k_gemv instantiations share
+// one function type).
+template <auto Kern>
+static int smem_attr(const b200_slice * s, int bytes, bool carveout = false) {
+    static bool done[16] = {false};
+    if (done[s->device & 15]) return 0;
+    B200_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    if (carveout) B200_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    done[s->device & 15] = true;
+    return 0;
+}
+
+// Calls f(std::integral_constant<int, WT>{}) for weight type wt: one of the block-quantised types (Q4_0, Q4_1, Q5_0, Q5_1,
+// Q8_0), or with KQ one of the k-quants (Q4_K, Q6_K).  Only the kernels of that family are instantiated (k_gemv_kq has no
+// PRO_NORM prologue).  `what` names the missing kernel in the error.
+template <bool KQ, class F>
+static int with_wtype(int wt, const char * what, F && f) {
+    using std::integral_constant;
+    if constexpr (KQ) {
+        switch (wt) {
+        case kWT_Q4_K: return f(integral_constant<int, kWT_Q4_K>{});
+        case kWT_Q6_K: return f(integral_constant<int, kWT_Q6_K>{});
+        }
+    } else {
+        switch (wt) {
+        case kWT_Q4_0: return f(integral_constant<int, kWT_Q4_0>{});
+        case kWT_Q4_1: return f(integral_constant<int, kWT_Q4_1>{});
+        case kWT_Q5_0: return f(integral_constant<int, kWT_Q5_0>{});
+        case kWT_Q5_1: return f(integral_constant<int, kWT_Q5_1>{});
+        case kWT_Q8_0: return f(integral_constant<int, kWT_Q8_0>{});
+        }
+    }
+    return fail(B200_EINVAL, "no %s for weight type %d", what, wt);
+}
+
+// ---------------------------------------------------------------- weight matmuls
 // Dynamic shared memory of a k_gemv launch: `act` bytes for the NC columns' activations (plus the f32 input row of a
 // one-column PRO_NORM launch) and barriers, and `stage` bytes per ring stage; a launch with NS stages needs bytes(NS).
 struct GemvSmem {
@@ -152,8 +205,7 @@ static constexpr auto gemv_kernel() {
 
 template <int WT, int G, int NC, int PRO, int EPI, bool RING>
 static int launch_gemv_t(b200_slice * s, GemvArgs a) {
-    auto kern = gemv_kernel<WT, G, NC, PRO, EPI, RING>();
-    static bool attr_set[16] = {false};
+    constexpr auto kern = gemv_kernel<WT, G, NC, PRO, EPI, RING>();
     const GemvSmem sm = gemv_smem<WT, G, NC, PRO>(a.W);
     const size_t stage = sm.stage, act = sm.act;
     // Ring depth: as deep as possible while EVERY tile of the matrix still gets a co-resident CTA (no second wave):
@@ -172,12 +224,8 @@ static int launch_gemv_t(b200_slice * s, GemvArgs a) {
     }
     const size_t smem = sm.bytes(NS);
     if (smem > (size_t) kSmemLimit) return fail(B200_EINVAL, "gemv needs %zu B of shared memory (K=%d, NC=%d)", smem, a.W.K, NC);
-    if (!attr_set[s->device & 15]) {
-        B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-        // without this the driver's carve-out heuristic leaves room for only 2 CTAs/SM however small the ring is
-        B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-        attr_set[s->device & 15] = true;
-    }
+    // without the carve-out the driver's heuristic leaves room for only 2 CTAs/SM however small the ring is
+    if (int rc = smem_attr<kern>(s, kSmemLimit, true)) return rc;
     a.NS = NS; a.dbg_nomath = s->opt_nomath; a.pre_stages = s->opt_pre;
     a.trace = nullptr;
     if (s->trace && s->trace_next < 512) { a.trace = s->trace + (size_t) s->trace_next * 1024 * 8; s->trace_next++; s->trace_cls.push_back(s->cur_class); }
@@ -188,21 +236,8 @@ static int launch_gemv_t(b200_slice * s, GemvArgs a) {
     int gx = a.W.n_tiles;
     const int cap = s->n_sm * per_sm;
     if (gx > cap) gx = cap;
-    cudaLaunchConfig_t cfg{};
     if (a.trace) s->trace_ctas.push_back(gx * ncol);
-    cfg.gridDim = dim3(gx, ncol, 1);
-    cfg.blockDim = dim3(RING ? kConsumers + 32 : kConsumers, 1, 1);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = s->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = s->use_pdl ? 1 : 0;
-    prof_begin(s);
-    B200_CUDA(cudaLaunchKernelEx(&cfg, kern, a));
-    prof_end(s);
-    s->launches++;
-    return 0;
+    return launch(s, kern, dim3(gx, ncol, 1), dim3(RING ? kConsumers + 32 : kConsumers, 1, 1), smem, a);
 }
 
 template <int WT, int G, int PRO, int EPI>
@@ -228,28 +263,26 @@ static int launch_gemv_nc(b200_slice * s, const GemvArgs & a) {
 
 template <int G, int PRO, int EPI>
 static int launch_gemv(b200_slice * s, const GemvArgs & a) {
-    switch (a.W.wtype) {
-    case kWT_Q4_0: return launch_gemv_nc<kWT_Q4_0, G, PRO, EPI>(s, a);
-    case kWT_Q4_1: return launch_gemv_nc<kWT_Q4_1, G, PRO, EPI>(s, a);
-    case kWT_Q5_0: return launch_gemv_nc<kWT_Q5_0, G, PRO, EPI>(s, a);
-    case kWT_Q5_1: return launch_gemv_nc<kWT_Q5_1, G, PRO, EPI>(s, a);
-    case kWT_Q8_0: return launch_gemv_nc<kWT_Q8_0, G, PRO, EPI>(s, a);
-    default: return fail(B200_EINVAL, "no block-quantised matmul for weight type %d", a.W.wtype);
-    }
+    return with_wtype<false>(a.W.wtype, "block-quantised matmul",
+                             [&](auto wt) { return launch_gemv_nc<decltype(wt)::value, G, PRO, EPI>(s, a); });
 }
 
 // Q4_K / Q6_K matrices (kquant.cuh): the type is per matrix, the activations are always Q8_K, quantised in the prologue
 template <int G, int PRO, int EPI>
 static int launch_gemv_kq(b200_slice * s, const GemvArgs & a) {
-    switch (a.W.wtype) {
-    case kWT_Q4_K: return launch_gemv_nc<kWT_Q4_K, G, PRO, EPI>(s, a);
-    case kWT_Q6_K: return launch_gemv_nc<kWT_Q6_K, G, PRO, EPI>(s, a);
-    default: return fail(B200_EINVAL, "no k-quant matmul for weight type %d", a.W.wtype);
-    }
+    return with_wtype<true>(a.W.wtype, "k-quant matmul",
+                            [&](auto wt) { return launch_gemv_nc<decltype(wt)::value, G, PRO, EPI>(s, a); });
 }
 
-template <typename K, typename A>
-static int launch_simple(b200_slice * s, K kern, dim3 grid, dim3 block, size_t smem, const A & args);
+// The slice's last w2 of a single-token step with the pipeline send folded in (EPI_RESID_SEND): its rows leave for the
+// next rank's inbox as they are computed.  One column, ring kernel.
+template <bool KQ>
+static int launch_w2_send(b200_slice * s, GemvArgs w) {
+    w.mb_mine = (MailboxHdr *) s->mb_block;
+    w.mb_peer_inbox = (uint2 *)(s->mb_next + sizeof(MailboxHdr)); w.mb_slot_elems = s->mb_slot_floats;
+    return with_wtype<KQ>(w.W.wtype, "pipelined matmul",
+                          [&](auto wt) { return launch_gemv_t<decltype(wt)::value, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w); });
+}
 
 // The input of a k-quant matmul: [RMSNorm * norm_w ->] Q8_K of its N columns, once per column (k_quant_q8k), into the
 // slice's Q8_K buffer, from which the matmul's CTAs fetch it (PRO_PREQ).
@@ -257,43 +290,16 @@ static int quant_kq(b200_slice * s, GemvArgs & a, bool norm) {
     const int nbq = a.W.nbq;
     QuantKArgs q{a.x, a.ldx, a.norm_w, a.W.K, s->kq_aq, s->n_ctx * nbq * 64, s->kq_ad, nbq};
     a.aq_in = s->kq_aq; a.in_soff = q.soff; a.da_in = s->kq_ad;
-    return norm ? launch_simple(s, k_quant_q8k<true>, dim3(a.N, 1, 1), dim3(256, 1, 1), 0, q)
-                : launch_simple(s, k_quant_q8k<false>, dim3(a.N, 1, 1), dim3(256, 1, 1), 0, q);
-}
-
-template <typename K, typename A>
-static int launch_simple(b200_slice * s, K kern, dim3 grid, dim3 block, size_t smem, const A & args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = s->use_pdl ? 1 : 0;
-    prof_begin(s);
-    B200_CUDA(cudaLaunchKernelEx(&cfg, kern, args));
-    prof_end(s);
-    s->launches++;
-    return 0;
+    return norm ? launch(s, k_quant_q8k<true>, dim3(a.N, 1, 1), dim3(256, 1, 1), 0, q)
+                : launch(s, k_quant_q8k<false>, dim3(a.N, 1, 1), dim3(256, 1, 1), 0, q);
 }
 
 template <int PRO, int EPI>
 static int launch_f16(b200_slice * s, GemvF16Args a) {
-    auto kern = k_gemv_f16<PRO, EPI>;
-    static bool attr_set[16] = {false};
-    const size_t smem = (size_t) a.K * 2 + 16;
-    if (!attr_set[s->device & 15]) {
-        B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-        attr_set[s->device & 15] = true;
-    }
+    int rc;
     if (a.N == 1 && s->use_ring && s->f16_ring && (a.K & 255) == 0) {
         // single-token steps: TMA-ring variant (weights stream from before the dependency wait, two CTAs per SM)
-        auto rk = k_gemv_f16_ring<PRO, EPI>;
-        static bool rattr[16] = {false};
-        if (!rattr[s->device & 15]) {
-            B200_CUDA(cudaFuncSetAttribute(rk, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-            B200_CUDA(cudaFuncSetAttribute(rk, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-            rattr[s->device & 15] = true;
-        }
+        if ((rc = smem_attr<k_gemv_f16_ring<PRO, EPI>>(s, kSmemLimit, true))) return rc;
         const int nc8 = (a.K / 32 + 7) / 8;
         const size_t fixed = (size_t) nc8 * 1024 + 64 + 64;
         int NS = s->opt_ns > 0 ? s->opt_ns : (int)(((size_t) 112 * 1024 - fixed) / ((size_t) kF16Warps * (kF16Stage + 16)));
@@ -303,80 +309,50 @@ static int launch_f16(b200_slice * s, GemvF16Args a) {
         const int n_tiles = (a.rows + kF16Warps - 1) / kF16Warps;
         int per_sm = (int)(kSmemLimit / (rsmem + 1024)); if (per_sm < 1) per_sm = 1; if (per_sm > 4) per_sm = 4;
         int rgx = n_tiles < s->n_sm * per_sm ? n_tiles : s->n_sm * per_sm;
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(rgx, 1, 1); cfg.blockDim = dim3(kF16Warps * 32 + 32, 1, 1); cfg.dynamicSmemBytes = rsmem; cfg.stream = s->stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = at; cfg.numAttrs = s->use_pdl ? 1 : 0;
-        prof_begin(s);
-        B200_CUDA(cudaLaunchKernelEx(&cfg, rk, a, NS));
-        prof_end(s);
-        s->launches++;
-        return 0;
+        return launch(s, k_gemv_f16_ring<PRO, EPI>, dim3(rgx, 1, 1), dim3(kF16Warps * 32 + 32, 1, 1), rsmem, a, NS);
     }
-    int gx = (a.rows + 7) / 8;
     if (a.N >= 2 && s->f16_mc) {
-        gx = (a.rows + 15) / 16;                         // 8 warps x 2 rows per CTA
         // multi-token call: 8 (or 4) columns per CTA share every weight load (k_gemv_f16_mc)
         // 4 columns per CTA keep the activation block at 64 KB for K = 4096: three CTAs (24 warps) per SM; B200_F16_MC=8 forces 8
         const bool c8 = s->f16_mc_cols == 8 && a.N > 4 && (size_t) a.K * 4 * 8 + 64 <= (size_t) 200 * 1024;
         const int nc = c8 ? 8 : 4;
         const size_t msmem = (size_t) a.K * 4 * nc + 64;
         if (msmem <= (size_t) 72 * 1024 || (c8 && msmem <= (size_t) kSmemLimit)) {
-            static bool mattr[16] = {false};
-            if (!mattr[s->device & 15]) {
-                B200_CUDA(cudaFuncSetAttribute(k_gemv_f16_mc<PRO, EPI, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-                B200_CUDA(cudaFuncSetAttribute(k_gemv_f16_mc<PRO, EPI, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-                mattr[s->device & 15] = true;
-            }
             const int ncolg = (a.N + nc - 1) / nc;
             int per_sm = (int)(kSmemLimit / (msmem + 1024)); if (per_sm < 1) per_sm = 1;
-            int mgx = gx; const int mcap = (s->n_sm * per_sm + ncolg - 1) / ncolg;
+            int mgx = (a.rows + 15) / 16;                    // 8 warps x 2 rows per CTA
+            const int mcap = (s->n_sm * per_sm + ncolg - 1) / ncolg;
             if (mgx > mcap) mgx = mcap < 1 ? 1 : mcap;
-            if (c8) return launch_simple(s, k_gemv_f16_mc<PRO, EPI, 8>, dim3(mgx, ncolg, 1), dim3(256, 1, 1), msmem, a);
-            return launch_simple(s, k_gemv_f16_mc<PRO, EPI, 4>, dim3(mgx, ncolg, 1), dim3(256, 1, 1), msmem, a);
+            if (c8) {
+                if ((rc = smem_attr<k_gemv_f16_mc<PRO, EPI, 8>>(s, kSmemLimit))) return rc;
+                return launch(s, k_gemv_f16_mc<PRO, EPI, 8>, dim3(mgx, ncolg, 1), dim3(256, 1, 1), msmem, a);
+            }
+            if ((rc = smem_attr<k_gemv_f16_mc<PRO, EPI, 4>>(s, kSmemLimit))) return rc;
+            return launch(s, k_gemv_f16_mc<PRO, EPI, 4>, dim3(mgx, ncolg, 1), dim3(256, 1, 1), msmem, a);
         }
     }
-    gx = (a.rows + 7) / 8;
+    int gx = (a.rows + 7) / 8;
     const int cap = s->n_sm * 8;
     if (gx > cap) gx = cap;
-    return launch_simple(s, kern, dim3(gx, a.N, 1), dim3(256, 1, 1), smem, a);
+    if ((rc = smem_attr<k_gemv_f16<PRO, EPI>>(s, kSmemLimit))) return rc;
+    return launch(s, k_gemv_f16<PRO, EPI>, dim3(gx, a.N, 1), dim3(256, 1, 1), (size_t) a.K * 2 + 16, a);
 }
 
 static int launch_norm_quant(b200_slice * s, const float * x, int ldx, const float * norm_w, int N) {
     NormQuantArgs q{x, ldx, norm_w, s->E, s->aq_x, s->da_x, s->nbqE, s->soffE};
-    switch (s->wtype) {
-    case kWT_Q4_0: return launch_simple(s, k_norm_quant<kWT_Q4_0>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
-    case kWT_Q4_1: return launch_simple(s, k_norm_quant<kWT_Q4_1>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
-    case kWT_Q5_0: return launch_simple(s, k_norm_quant<kWT_Q5_0>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
-    case kWT_Q5_1: return launch_simple(s, k_norm_quant<kWT_Q5_1>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
-    case kWT_Q8_0: return launch_simple(s, k_norm_quant<kWT_Q8_0>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
-    default: return fail(B200_EINVAL, "no activation quantiser for weight type %d", s->wtype);
-    }
+    return with_wtype<false>(s->wtype, "activation quantiser", [&](auto wt) {
+        return launch(s, k_norm_quant<decltype(wt)::value>, dim3(N, 1, 1), dim3(256, 1, 1), 0, q);
+    });
 }
 
-// ---------------------------------------------------------------- fast-mode prefill (wgmma), see fastgemm.cuh
+// ---------------------------------------------------------------- fast-mode prefill (wgmma), see fastgemm2.cuh
 template <bool NORM>
 static int launch_prep(b200_slice * s, const float * x, int ldx, const float * norm_w, int K, int N) {
     PrepArgs p{x, ldx, norm_w, s->xh, K, N};
-    return launch_simple(s, k_prep_q8_f16<NORM>, dim3(N, 1, 1), dim3(256, 1, 1), 0, p);
-}
-template <int EPI>
-static int launch_fast_gemm(b200_slice * s, const PackedW & W, const float * resid, int ldr, float * y, int ldy, int N, int out_rows) {
-    static bool attr_set[16] = {false};
-    auto kern = k_gemm_q4_tc<EPI>;
-    if (!attr_set[s->device & 15]) {
-        B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kFgSmem));
-        attr_set[s->device & 15] = true;
-    }
-    FastGemmArgs a{}; a.W = W; a.xh = s->xh; a.resid = resid; a.ldr = ldr; a.y = y; a.ldy = ldy; a.N = N; a.out_rows = out_rows;
-    a.tsilu = s->tsilu;
-    const int groups = W.n_tiles * W.TR;                     // 8-row groups in packed order
-    return launch_simple(s, kern, dim3((groups + 15) / 16, (N + kFgN - 1) / kFgN, 1), dim3(160, 1, 1), kFgSmem, a);
+    return launch(s, k_prep_q8_f16<NORM>, dim3(N, 1, 1), dim3(256, 1, 1), 0, p);
 }
 
-// second-generation wgmma prefill matmul (fastgemm2.cuh): 128 x 256 tiles, activations through a tensor-map TMA
+// 128 x 256 (or 128 x 128) tiles, activations through a tensor-map TMA
 typedef CUresult (*TensorMapEncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                       const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
                                       CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -393,7 +369,7 @@ static TensorMapEncodeFn tensor_map_encode() {
 }
 
 template <int WT, int EPI, int NT>
-static int launch_fast_gemm2_t(b200_slice * s, const PackedW & W, const float * resid, int ldr, float * y, int ldy, int N, int out_rows) {
+static int launch_fast_gemm_t(b200_slice * s, const PackedW & W, const float * resid, int ldr, float * y, int ldy, int N, int out_rows) {
     TensorMapEncodeFn enc = tensor_map_encode();
     if (!enc) return fail(B200_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
     // activations xh [N][K] fp16, K innermost; box = 64 halfs (128 B, the swizzle span) x 256 token rows; rows >= N read as zeros
@@ -405,275 +381,260 @@ static int launch_fast_gemm2_t(b200_slice * s, const PackedW & W, const float * 
     CUresult cr = enc(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void *) s->xh, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) return fail(B200_ECUDA, "cuTensorMapEncodeTiled failed (%d) for K=%d N=%d", (int) cr, W.K, N);
-    auto kern = k_gemm_tc2<WT, EPI, NT>;
-    static bool attr_set[16] = {false};
-    if (!attr_set[s->device & 15]) {
-        B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, f2_smem(WT, NT)));
-        attr_set[s->device & 15] = true;
-    }
+    if (int rc = smem_attr<k_gemm_tc2<WT, EPI, NT>>(s, f2_smem(WT, NT))) return rc;
     FastGemm2Args a{}; a.W = W; a.resid = resid; a.ldr = ldr; a.y = y; a.ldy = ldy; a.N = N; a.out_rows = out_rows; a.tsilu = s->tsilu;
     const int groups = W.n_tiles * W.TR;                     // 8-row groups in packed order
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((groups + 15) / 16, (N + NT - 1) / NT, 1); cfg.blockDim = dim3(kF2Threads, 1, 1);
-    cfg.dynamicSmemBytes = f2_smem(WT, NT); cfg.stream = s->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = s->use_pdl ? 1 : 0;
-    prof_begin(s);
-    B200_CUDA(cudaLaunchKernelEx(&cfg, kern, a, map));
-    prof_end(s);
-    s->launches++;
+    return launch(s, k_gemm_tc2<WT, EPI, NT>, dim3((groups + 15) / 16, (N + NT - 1) / NT, 1), dim3(kF2Threads, 1, 1), f2_smem(WT, NT), a, map);
+}
+
+template <int EPI>
+static int launch_fast_gemm(b200_slice * s, const PackedW & W, const float * resid, int ldr, float * y, int ldy, int N, int out_rows) {
+    // 256-token tiles halve the dequantisation per flop; a matrix whose 128-row tiles x 256-token tiles would leave SMs idle
+    // (wo, w2: 32 row tiles) takes 128-token tiles and three stages instead
+    const int mtiles = (W.n_tiles * W.TR + 15) / 16;
+    const bool wide = (long long) mtiles * ((N + 255) / 256) >= s->n_sm || N <= 128;
+    if (W.wtype == kWT_Q4_0) return wide ? launch_fast_gemm_t<kWT_Q4_0, EPI, 256>(s, W, resid, ldr, y, ldy, N, out_rows)
+                                         : launch_fast_gemm_t<kWT_Q4_0, EPI, 128>(s, W, resid, ldr, y, ldy, N, out_rows);
+    return wide ? launch_fast_gemm_t<kWT_Q8_0, EPI, 256>(s, W, resid, ldr, y, ldy, N, out_rows)
+                : launch_fast_gemm_t<kWT_Q8_0, EPI, 128>(s, W, resid, ldr, y, ldy, N, out_rows);
+}
+
+// ---------------------------------------------------------------- attention
+// Dynamic shared memory of the attention kernels at this n_ctx: scores (f32) and probabilities (f16) of every position,
+// then for head size 128 the staged K / V rows of the cluster kernel (up to 128 local rows = 512 positions) and in
+// single-token steps the exp table's negative half, for other head sizes the partial sums of k_attention.
+struct AttnSmem { int pf_rows; size_t plain, staged, lut, generic; };
+
+static AttnSmem attn_smem(int n_ctx, int D) {
+    AttnSmem m;
+    const size_t sc = (size_t)((n_ctx + 3) & ~3) * 4 + (size_t)((n_ctx + 7) & ~7) * 2, sc16 = (sc + 15) & ~(size_t) 15;
+    m.pf_rows = std::min(8 * ((n_ctx + 31) / 32), 128);
+    m.plain = sc16 + 64;                                                   // k_attn128<false>
+    m.staged = sc16 + (size_t) 2 * m.pf_rows * kAttnRow + 32 * 64 + 64;    // k_attn128<true>
+    m.lut = m.staged + 65536;                                              // k_attn128<true>, exp table staged
+    m.generic = sc + (size_t) 4 * D * 8 * 4 + 64;                          // k_attention
+    return m;
+}
+
+// RoPE, KV-cache append and attention of layer il over s->qkv, into s->att.  With `preq` the head-size-128 kernels also
+// write their output quantised for the wo matmul (aq_att / da_att).
+static int attention(b200_slice * s, int il, int N, bool preq) {
+    if (s->skip_attention) return 0;      // measurement aid: the matmul kernels of the step back to back
+    const int E = s->E, H = s->H, D = s->D;
+    // cols mode (batched independent sequences): the kernels add session * sess_stride themselves
+    const size_t sess_off = s->cols ? 0 : (size_t) s->cur * s->sess_stride;
+    uint16_t * kc = s->kc + sess_off + (size_t) il * s->n_ctx * E, * vc = s->vc + sess_off + (size_t) il * s->n_ctx * E;
+    int * d_npast = s->d_npast + s->cur;
+    const AttnSmem am = attn_smem(s->n_ctx, D);
+    const float kq_scale = 1.0f / sqrtf((float) E / (float) H);
+    int rc;
+    if (D != 128) {
+        s->cur_class = 1;
+        RopeArgs ra{s->qkv, E, H, D, N, d_npast, s->cs, s->q16, kc, vc, s->cols, s->sess_stride};
+        if ((rc = launch(s, k_rope_append, dim3((E / 2 + 255) / 256, N, 1), dim3(256, 1, 1), 0, ra))) return rc;
+        s->cur_class = 2;
+        AttnArgs aa{s->q16, kc, vc, d_npast, E, H, D, N, s->texp, s->att, kq_scale, s->cols, s->sess_stride};
+        return launch(s, k_attention, dim3(H, N, 1), dim3(512, 1, 1), am.generic, aa);
+    }
+    // head size 128: cluster kernel; for single-token and batched steps RoPE + KV append are fused into its prologue
+    constexpr int kChunk = 1024;     // query tokens per launch (grid.y)
+    Attn128Args aa{};
+    aa.pf_rows = am.pf_rows;
+    aa.qkv = s->qkv; aa.q16 = s->q16; aa.kc = kc; aa.vc = vc; aa.n_past = d_npast; aa.E = E; aa.H = H; aa.N = N;
+    aa.cols = s->cols; aa.sess_stride = s->sess_stride;
+    aa.cs = s->cs; aa.texp = s->texp; aa.out = s->att;
+    aa.n_ctx = s->n_ctx; aa.kq_scale = kq_scale;
+    const float dsc = preq ? wt_act_scale(s->wtype) : 0.f;
+    if (preq) { aa.aq_out = s->aq_att; aa.da_out = s->da_att; aa.out_nbq = s->nbqE; aa.out_dscale = dsc; aa.out_soff = s->soffE; }
+    if (s->cols) {
+        // every column is an independent N = 1 step: the fused (RoPE + append) kernel, one cluster row per column
+        s->cur_class = 2;
+        for (int n0 = 0; n0 < N; n0 += kChunk) {
+            aa.n0 = n0;
+            const int cnt = N - n0 < kChunk ? N - n0 : kChunk;
+            if ((rc = launch(s, k_attn128<true>, dim3(4 * H, cnt, 1), dim3(256, 1, 1), am.staged, aa))) return rc;
+        }
+        return 0;
+    }
+    if (N == 1) {
+        s->cur_class = 2;
+        aa.n0 = 0;
+        if (s->trace && s->trace_next < 512) { aa.trace = s->trace + (size_t) s->trace_next * 1024 * 8; s->trace_next++; s->trace_cls.push_back(2); s->trace_ctas.push_back(4 * H); }
+        aa.lut_smem = s->attn_lut_smem;
+        return launch(s, k_attn128<true>, dim3(4 * H, 1, 1), dim3(256, 1, 1), aa.lut_smem ? am.lut : am.staged, aa);
+    }
+    s->cur_class = 1;
+    RopeArgs ra{s->qkv, E, H, D, N, d_npast, s->cs, s->q16, kc, vc, nullptr, 0};
+    if ((rc = launch(s, k_rope_append, dim3((E / 2 + 255) / 256, N, 1), dim3(256, 1, 1), 0, ra))) return rc;
+    s->cur_class = 2;
+    if (s->use_tiled_attn && s->past[s->cur] + N <= kAttnTMax) {
+        // prompt chunk whose whole context fits the staged window: query-tiled kernel, K / V read once per 16 queries
+        const int Tn = s->past[s->cur] + N;
+        AttnTiledArgs ta{};
+        ta.q16 = s->q16; ta.kc = kc; ta.vc = vc; ta.n_past = d_npast; ta.E = E; ta.H = H; ta.N = N; ta.texp = s->texp; ta.out = s->att;
+        if (preq) { ta.aq_out = s->aq_att; ta.da_out = s->da_att; ta.out_nbq = s->nbqE; ta.out_dscale = dsc; ta.out_soff = s->soffE; }
+        ta.kq_scale = kq_scale; ta.t_rows = Tn; ta.t_pad = (Tn + 31) & ~31;
+        const size_t tsm = (size_t) ta.t_rows * kAttnRow + (size_t) kAttnQB * ta.t_pad * 6 + 4 * 8 * 128 * 4 + kAttnQB * 256 + 64;
+        if ((rc = smem_attr<k_attn128_tiled>(s, kSmemLimit))) return rc;
+        return launch(s, k_attn128_tiled, dim3(H, (N + kAttnQB - 1) / kAttnQB, 1), dim3(512, 1, 1), tsm, ta);
+    }
+    for (int n0 = 0; n0 < N; n0 += kChunk) {
+        aa.n0 = n0;
+        const int cnt = N - n0 < kChunk ? N - n0 : kChunk;
+        if ((rc = launch(s, k_attn128<false>, dim3(4 * H, cnt, 1), dim3(256, 1, 1), am.plain, aa))) return rc;
+    }
     return 0;
 }
-template <int EPI>
-static int launch_fast_any(b200_slice * s, const PackedW & W, const float * resid, int ldr, float * y, int ldy, int N, int out_rows) {
-    if (s->fast_version >= 2) {
-        // 256-token tiles halve the dequantisation per flop; a matrix whose 128-row tiles x 256-token tiles would leave SMs idle
-        // (wo, w2: 32 row tiles) takes 128-token tiles and three stages instead
-        const int mtiles = (W.n_tiles * W.TR + 15) / 16;
-        const bool wide = (long long) mtiles * ((N + 255) / 256) >= s->n_sm || N <= 128;
-        if (W.wtype == kWT_Q4_0) return wide ? launch_fast_gemm2_t<kWT_Q4_0, EPI, 256>(s, W, resid, ldr, y, ldy, N, out_rows)
-                                             : launch_fast_gemm2_t<kWT_Q4_0, EPI, 128>(s, W, resid, ldr, y, ldy, N, out_rows);
-        return wide ? launch_fast_gemm2_t<kWT_Q8_0, EPI, 256>(s, W, resid, ldr, y, ldy, N, out_rows)
-                    : launch_fast_gemm2_t<kWT_Q8_0, EPI, 128>(s, W, resid, ldr, y, ldy, N, out_rows);
+
+// ---------------------------------------------------------------- one layer per weight family
+// Each enqueues layer il for N tokens: qkv -> attention -> wo -> w1|w3 -> w2, reading `cur` and writing `nxt`.
+// Profile classes (cur_class): qkv 0, RoPE 1, attention 2, wo 3, w1|w3 4, w2 5; an input quantiser takes the class of
+// the matmul it feeds.
+
+// F16 weights: f32 activations, RMSNorm fused into the qkv and w1|w3 prologues
+static int layer_f16(b200_slice * s, int il, int N, const float * cur, float * nxt) {
+    const int E = s->E, FF = s->FF;
+    const LayerW & Lw = s->layers[il];
+    int rc;
+    GemvF16Args q{}; q.K = E; q.x = cur; q.ldx = E; q.norm_w = Lw.attn_norm; q.N = N; q.tsilu = s->tsilu;
+    q.rows = 3 * E; q.ldy = 3 * E;       // wq | wk | wv are packed back to back: one launch, one RMSNorm prologue
+    q.W = Lw.f_q; q.y = s->qkv;
+    if ((rc = launch_f16<PRO_NORM, EPI_STORE>(s, q))) return rc;
+    if ((rc = attention(s, il, N, false))) return rc;
+    s->cur_class = 3;
+    GemvF16Args o{}; o.K = E; o.x = s->att; o.ldx = E; o.N = N; o.tsilu = s->tsilu;
+    o.rows = E; o.W = Lw.f_o; o.resid = cur; o.ldr = E; o.y = s->ffin; o.ldy = E;
+    if ((rc = launch_f16<PRO_PLAIN, EPI_RESID>(s, o))) return rc;
+    s->cur_class = 4;
+    GemvF16Args g{}; g.K = E; g.x = s->ffin; g.ldx = E; g.norm_w = Lw.ffn_norm; g.N = N; g.tsilu = s->tsilu;
+    g.rows = FF; g.W = Lw.f_1; g.W2 = Lw.f_3; g.y = s->gate; g.ldy = FF;
+    if ((rc = launch_f16<PRO_NORM, EPI_GATE>(s, g))) return rc;
+    s->cur_class = 5;
+    GemvF16Args w{}; w.K = FF; w.x = s->gate; w.ldx = FF; w.N = N; w.tsilu = s->tsilu;
+    w.rows = E; w.W = Lw.f_2; w.resid = s->ffin; w.ldr = E; w.y = nxt; w.ldy = E;
+    return launch_f16<PRO_PLAIN, EPI_RESID>(s, w);
+}
+
+// Block-quantised weights (Q4_0, Q4_1, Q5_0, Q5_1, Q8_0), bit-exact: every matmul input is quantised like the
+// reference's, and where it can be, by the kernel that produces it (attention, the w1|w3 gate, the NQ epilogues)
+static int layer_exact(b200_slice * s, int il, int N, const float * cur, float * nxt) {
+    const int E = s->E, FF = s->FF;
+    const LayerW & Lw = s->layers[il];
+    // grid-barrier norm+quant epilogue: decode only (every CTA of wo / w2 must be co-resident: 1 tile per CTA)
+    const bool nq = s->use_nq && N == 1 && !s->cols && Lw.wo.n_tiles <= 256 && Lw.wo.n_tiles <= s->n_sm * 2;
+    const float dsc = wt_act_scale(s->wtype);
+    int rc;
+    GemvArgs q{}; q.W = Lw.qkv; q.x = cur; q.ldx = E; q.norm_w = Lw.attn_norm; q.y = s->qkv; q.ldy = 3 * E;
+    q.N = N; q.out_rows = 3 * E; q.tsilu = s->tsilu; q.aq_in = s->aq_x; q.da_in = s->da_x; q.in_soff = s->soffE;
+    // a multi-token call normalises + quantises every row ONCE instead of once per 32-row tile (k_norm_quant); with nq
+    // the layers after the first get their input already normalised + quantised by the previous w2's last CTA
+    if (N > 1 && (rc = launch_norm_quant(s, cur, E, Lw.attn_norm, N))) return rc;
+    if ((rc = N > 1 || (il > 0 && nq) ? launch_gemv<1, PRO_PREQ, EPI_STORE>(s, q) : launch_gemv<1, PRO_NORM, EPI_STORE>(s, q))) return rc;
+    if ((rc = attention(s, il, N, true))) return rc;
+    s->cur_class = 3;
+    GemvArgs o{}; o.W = Lw.wo; o.x = s->att; o.ldx = E; o.resid = cur; o.ldr = E; o.y = s->ffin; o.ldy = E;
+    o.N = N; o.out_rows = E; o.tsilu = s->tsilu; o.aq_in = s->aq_att; o.da_in = s->da_att; o.in_soff = s->soffE; o.out_soff = s->soffE;
+    o.nq_norm_w = Lw.ffn_norm; o.nq_counter = s->nq_counter; o.nq_partial = s->nq_partial; o.aq_out = s->aq_x; o.da_out = s->da_x; o.out_nbq = s->nbqE; o.out_dscale = dsc;
+    if (s->D == 128) rc = nq ? launch_gemv<1, PRO_PREQ, EPI_RESID_NQ>(s, o) : launch_gemv<1, PRO_PREQ, EPI_RESID>(s, o);    // quantised by the attention
+    else             rc = nq ? launch_gemv<1, PRO_PLAIN, EPI_RESID_NQ>(s, o) : launch_gemv<1, PRO_PLAIN, EPI_RESID>(s, o);
+    if (rc) return rc;
+    s->cur_class = 4;
+    GemvArgs g{}; g.W = Lw.w13; g.x = s->ffin; g.ldx = E; g.norm_w = Lw.ffn_norm; g.y = s->gate; g.ldy = FF;
+    g.N = N; g.out_rows = FF; g.tsilu = s->tsilu; g.aq_in = s->aq_x; g.da_in = s->da_x; g.in_soff = s->soffE; g.out_soff = s->soffF;
+    g.aq_out = s->aq_gate; g.da_out = s->da_gate; g.out_nbq = s->nbqF; g.out_dscale = dsc;
+    if (N > 1 && (rc = launch_norm_quant(s, s->ffin, E, Lw.ffn_norm, N))) return rc;
+    if ((rc = N > 1 || nq ? launch_gemv<2, PRO_PREQ, EPI_GATEQ>(s, g) : launch_gemv<2, PRO_NORM, EPI_GATEQ>(s, g))) return rc;
+    s->cur_class = 5;
+    GemvArgs w{}; w.W = Lw.w2; w.resid = s->ffin; w.ldr = E; w.y = nxt; w.ldy = E;
+    w.N = N; w.out_rows = E; w.tsilu = s->tsilu; w.aq_in = s->aq_gate; w.da_in = s->da_gate; w.in_soff = s->soffF; w.out_soff = s->soffE;
+    if (il + 1 < s->L && nq) {
+        w.nq_norm_w = s->layers[il + 1].attn_norm; w.nq_counter = s->nq_counter; w.nq_partial = s->nq_partial; w.aq_out = s->aq_x; w.da_out = s->da_x;
+        w.out_nbq = s->nbqE; w.out_dscale = dsc;
+        return launch_gemv<1, PRO_PREQ, EPI_RESID_NQ>(s, w);
     }
-    return launch_fast_gemm<EPI>(s, W, resid, ldr, y, ldy, N, out_rows);
+    if (s->fold_send && il == s->L - 1) return launch_w2_send<false>(s, w);
+    return launch_gemv<1, PRO_PREQ, EPI_RESID>(s, w);
+}
+
+// Fast mode (Q4_0 / Q8_0 prompt chunks): each matmul's input goes through k_prep_q8_f16, the matmul through k_gemm_tc2
+static int layer_fast(b200_slice * s, int il, int N, const float * cur, float * nxt) {
+    const int E = s->E, FF = s->FF;
+    const LayerW & Lw = s->layers[il];
+    int rc;
+    if ((rc = launch_prep<true>(s, cur, E, Lw.attn_norm, E, N))) return rc;
+    if ((rc = launch_fast_gemm<FG_STORE>(s, Lw.qkv, nullptr, 0, s->qkv, 3 * E, N, 3 * E))) return rc;
+    if ((rc = attention(s, il, N, true))) return rc;         // the quantised copy is written as in exact mode; wo reads s->att
+    s->cur_class = 3;
+    if ((rc = launch_prep<false>(s, s->att, E, nullptr, E, N))) return rc;
+    if ((rc = launch_fast_gemm<FG_RESID>(s, Lw.wo, cur, E, s->ffin, E, N, E))) return rc;
+    s->cur_class = 4;
+    if ((rc = launch_prep<true>(s, s->ffin, E, Lw.ffn_norm, E, N))) return rc;
+    if ((rc = launch_fast_gemm<FG_GATE>(s, Lw.w13, nullptr, 0, s->gate, FF, N, FF))) return rc;
+    s->cur_class = 5;
+    if ((rc = launch_prep<false>(s, s->gate, FF, nullptr, FF, N))) return rc;
+    return launch_fast_gemm<FG_RESID>(s, Lw.w2, s->ffin, E, nxt, E, N, E);
+}
+
+// k-quant weights (Q4_K / Q6_K in any mix, kquant.cuh): every matmul input is quantised to Q8_K by quant_kq
+static int layer_kquant(b200_slice * s, int il, int N, const float * cur, float * nxt) {
+    const int E = s->E, FF = s->FF;
+    const LayerW & Lw = s->layers[il];
+    int rc;
+    GemvArgs q{}; q.W = Lw.qkv; q.x = cur; q.ldx = E; q.norm_w = Lw.attn_norm; q.y = s->qkv; q.ldy = 3 * E;
+    q.N = N; q.out_rows = Lw.qkv.rows; q.tsilu = s->tsilu;
+    if ((rc = quant_kq(s, q, true)) || (rc = launch_gemv_kq<1, PRO_PREQ, EPI_STORE>(s, q))) return rc;
+    for (int i = 0; i < 2 && Lw.qkv_more[i].data; i++) {       // wq | wk and wv of different types: same input and rows, exact
+        q.W = Lw.qkv_more[i]; q.y = s->qkv + Lw.qkv_row[i]; q.out_rows = Lw.qkv_more[i].rows;
+        if ((rc = launch_gemv_kq<1, PRO_PREQ, EPI_STORE>(s, q))) return rc;
+    }
+    if ((rc = attention(s, il, N, false))) return rc;        // wo quantises the f32 s->att itself
+    s->cur_class = 3;
+    GemvArgs o{}; o.W = Lw.wo; o.x = s->att; o.ldx = E; o.resid = cur; o.ldr = E; o.y = s->ffin; o.ldy = E;
+    o.N = N; o.out_rows = E; o.tsilu = s->tsilu;
+    if ((rc = quant_kq(s, o, false)) || (rc = launch_gemv_kq<1, PRO_PREQ, EPI_RESID>(s, o))) return rc;
+    s->cur_class = 4;
+    GemvArgs g{}; g.W = Lw.w13; g.x = s->ffin; g.ldx = E; g.norm_w = Lw.ffn_norm; g.y = s->gate; g.ldy = FF;
+    g.N = N; g.out_rows = FF; g.tsilu = s->tsilu;
+    if ((rc = quant_kq(s, g, true)) || (rc = launch_gemv_kq<2, PRO_PREQ, EPI_GATE>(s, g))) return rc;
+    s->cur_class = 5;
+    GemvArgs w{}; w.W = Lw.w2; w.x = s->gate; w.ldx = FF; w.resid = s->ffin; w.ldr = E; w.y = nxt; w.ldy = E;
+    w.N = N; w.out_rows = E; w.tsilu = s->tsilu;
+    if ((rc = quant_kq(s, w, false))) return rc;
+    if (s->fold_send && il == s->L - 1) return launch_w2_send<true>(s, w);
+    return launch_gemv_kq<1, PRO_PREQ, EPI_RESID>(s, w);
 }
 
 // ---------------------------------------------------------------- one forward over the slice
 // Enqueue every layer for N tokens at device-side position *d_npast (tensor_processor.cpp:537-766).
 static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) {
-    const int E = s->E, FF = s->FF, H = s->H, D = s->D;
     const float * cur = in;
+    int rc;
     for (int il = 0; il < s->L; il++) {
-        LayerW & Lw = s->layers[il];
+        const LayerW & Lw = s->layers[il];
+        float * nxt = (il == s->L - 1) ? out : ((il & 1) ? s->xb : s->xa);
         // fast mode is for prefill calls only: a single-token step or a batched step (cols: one token of each of N sessions)
         // stays exact, so decode and batch_forward keep the reference's bits whatever min_tokens is
         const bool fast = s->fast_prefill && N > 1 && !s->cols && N >= s->fast_min_tokens &&
-                          (s->wtype == kWT_Q4_0 || (s->wtype == kWT_Q8_0 && s->fast_version >= 2)) &&
+                          (s->wtype == kWT_Q4_0 || s->wtype == kWT_Q8_0) &&
                           (Lw.qkv.n_tiles * Lw.qkv.TR) % 16 == 0 &&
                           (Lw.wo.n_tiles * Lw.wo.TR) % 16 == 0 && (Lw.w13.n_tiles * Lw.w13.TR) % 16 == 0;
-        // grid-barrier norm+quant epilogue: decode only (every CTA of wo / w2 must be co-resident: 1 tile per CTA)
-        // k-quant slices (Q4_K / Q6_K in any mix) take the exact kernels of kquant.cuh: no fast mode, no NQ epilogue
-        const bool kq = wt_kquant(s->wtype);
-        const bool nq = s->use_nq && N == 1 && !s->cols && s->wtype != kWT_F16 && !kq && Lw.wo.n_tiles <= 256 && Lw.wo.n_tiles <= s->n_sm * 2;
-        float * nxt = (il == s->L - 1) ? out : ((il & 1) ? s->xb : s->xa);
-        // cols mode (batched independent sequences): the kernels add session * sess_stride themselves
-        const size_t sess_off = s->cols ? 0 : (size_t) s->cur * s->sess_stride;
-        uint16_t * kc = s->kc + sess_off + (size_t) il * s->n_ctx * E, * vc = s->vc + sess_off + (size_t) il * s->n_ctx * E;
-        int * d_npast = s->d_npast + s->cur;
-        int rc;
         s->cur_class = 0;
-        if (s->wtype == kWT_F16) {
-            GemvF16Args f{}; f.K = E; f.x = cur; f.ldx = E; f.norm_w = Lw.attn_norm; f.N = N; f.tsilu = s->tsilu;
-            f.rows = 3 * E; f.ldy = 3 * E;       // wq | wk | wv are packed back to back: one launch, one RMSNorm prologue
-            f.W = Lw.f_q; f.y = s->qkv;         if ((rc = launch_f16<PRO_NORM, EPI_STORE>(s, f))) return rc;
-        } else if (kq) {
-            GemvArgs g{}; g.W = Lw.qkv; g.x = cur; g.ldx = E; g.norm_w = Lw.attn_norm; g.y = s->qkv; g.ldy = 3 * E;
-            g.N = N; g.out_rows = Lw.qkv.rows; g.tsilu = s->tsilu;
-            if ((rc = quant_kq(s, g, true)) || (rc = launch_gemv_kq<1, PRO_PREQ, EPI_STORE>(s, g))) return rc;
-            for (int i = 0; i < 2 && Lw.qkv_more[i].data; i++) {       // wq | wk and wv of different types: same input and rows, exact
-                g.W = Lw.qkv_more[i]; g.y = s->qkv + Lw.qkv_row[i]; g.out_rows = Lw.qkv_more[i].rows;
-                if ((rc = launch_gemv_kq<1, PRO_PREQ, EPI_STORE>(s, g))) return rc;
-            }
-        } else if (fast) {
-            if ((rc = launch_prep<true>(s, cur, E, Lw.attn_norm, E, N))) return rc;
-            if ((rc = launch_fast_any<FG_STORE>(s, Lw.qkv, nullptr, 0, s->qkv, 3 * E, N, 3 * E))) return rc;
-        } else {
-            GemvArgs g{}; g.W = Lw.qkv; g.x = cur; g.ldx = E; g.norm_w = Lw.attn_norm; g.y = s->qkv; g.ldy = 3 * E;
-            g.N = N; g.out_rows = 3 * E; g.tsilu = s->tsilu; g.aq_in = s->aq_x; g.da_in = s->da_x; g.in_soff = s->soffE;
-            // layers after the first get their input already normalised + quantised by the previous w2's last CTA
-            if (il > 0 && nq) { if ((rc = launch_gemv<1, PRO_PREQ, EPI_STORE>(s, g))) return rc; }
-            else if (N > 1) {
-                // multi-token call: normalise + quantise every row ONCE instead of once per 32-row tile (k_norm_quant)
-                if ((rc = launch_norm_quant(s, cur, E, Lw.attn_norm, N))) return rc;
-                if ((rc = launch_gemv<1, PRO_PREQ, EPI_STORE>(s, g))) return rc;
-            }
-            else                     { if ((rc = launch_gemv<1, PRO_NORM, EPI_STORE>(s, g))) return rc; }
-        }
-        if (s->skip_attention) {
-            // measurement aid: the matmul kernels of the step back to back, attention left out
-        } else if (D == 128) {
-            // head size 128: cluster kernel; for N = 1 RoPE + KV append are fused into its prologue
-            constexpr int kChunk = 1024;     // query tokens per launch (grid.y)
-            // scores + probabilities, then (single-token kernels) the staged K / V rows: up to 128 local rows = 512 positions
-            const size_t sc_bytes = (((size_t)((s->n_ctx + 3) & ~3) * 4 + (size_t)((s->n_ctx + 7) & ~7) * 2) + 15) & ~(size_t) 15;
-            int pf_rows = 8 * ((s->n_ctx + 31) / 32);
-            if (pf_rows > 128) pf_rows = 128;
-            const size_t asm_plain = sc_bytes + 64, asm_bytes = sc_bytes + (size_t) 2 * pf_rows * kAttnRow + 32 * 64 + 64;
-            const size_t asm_lut = asm_bytes + 65536;            // + the exp table's negative half (single-token steps only)
-            Attn128Args aa{};
-            aa.pf_rows = pf_rows;
-            aa.qkv = s->qkv; aa.q16 = s->q16; aa.kc = kc; aa.vc = vc; aa.n_past = d_npast; aa.E = E; aa.H = H; aa.N = N;
-            aa.cols = s->cols; aa.sess_stride = s->sess_stride;
-            aa.cs = s->cs; aa.texp = s->texp; aa.out = s->att;
-            aa.n_ctx = s->n_ctx; aa.kq_scale = 1.0f / sqrtf((float) E / (float) H);
-            const bool preq = s->wtype != kWT_F16 && !kq;       // k-quant wo quantises the f32 s->att itself
-            const float dsc = preq ? wt_act_scale(s->wtype) : 0.f;
-            if (preq) { aa.aq_out = s->aq_att; aa.da_out = s->da_att; aa.out_nbq = s->nbqE; aa.out_dscale = dsc; aa.out_soff = s->soffE; }
-            if (s->cols) {
-                // every column is an independent N = 1 step: the fused (RoPE + append) kernel, one cluster row per column
-                s->cur_class = 2;
-                for (int n0 = 0; n0 < N; n0 += kChunk) {
-                    aa.n0 = n0;
-                    const int cnt = N - n0 < kChunk ? N - n0 : kChunk;
-                    if ((rc = launch_simple(s, k_attn128<true>, dim3(4 * H, cnt, 1), dim3(256, 1, 1), asm_bytes, aa))) return rc;
-                }
-            } else if (N == 1) {
-                s->cur_class = 2;
-                aa.n0 = 0;
-                if (s->trace && s->trace_next < 512) { aa.trace = s->trace + (size_t) s->trace_next * 1024 * 8; s->trace_next++; s->trace_cls.push_back(2); s->trace_ctas.push_back(4 * H); }
-                aa.lut_smem = s->attn_lut_smem;
-                if ((rc = launch_simple(s, k_attn128<true>, dim3(4 * H, 1, 1), dim3(256, 1, 1), aa.lut_smem ? asm_lut : asm_bytes, aa))) return rc;
-            } else if (s->use_tiled_attn && s->past[s->cur] + N <= kAttnTMax) {
-                // prompt chunk whose whole context fits the staged window: query-tiled kernel, K / V read once per 16 queries
-                s->cur_class = 1;
-                RopeArgs ra{s->qkv, E, H, D, N, d_npast, s->cs, s->q16, kc, vc, nullptr, 0};
-                if ((rc = launch_simple(s, k_rope_append, dim3((E / 2 + 255) / 256, N, 1), dim3(256, 1, 1), 0, ra))) return rc;
-                s->cur_class = 2;
-                const int Tn = s->past[s->cur] + N;
-                AttnTiledArgs ta{};
-                ta.q16 = s->q16; ta.kc = kc; ta.vc = vc; ta.n_past = d_npast; ta.E = E; ta.H = H; ta.N = N; ta.texp = s->texp; ta.out = s->att;
-                if (preq) { ta.aq_out = s->aq_att; ta.da_out = s->da_att; ta.out_nbq = s->nbqE; ta.out_dscale = dsc; ta.out_soff = s->soffE; }
-                ta.kq_scale = aa.kq_scale; ta.t_rows = Tn; ta.t_pad = (Tn + 31) & ~31;
-                const size_t tsm = (size_t) ta.t_rows * kAttnRow + (size_t) kAttnQB * ta.t_pad * 6 + 4 * 8 * 128 * 4 + kAttnQB * 256 + 64;
-                static bool tattr[16] = {false};
-                if (!tattr[s->device & 15]) {
-                    B200_CUDA(cudaFuncSetAttribute(k_attn128_tiled, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-                    tattr[s->device & 15] = true;
-                }
-                if ((rc = launch_simple(s, k_attn128_tiled, dim3(H, (N + kAttnQB - 1) / kAttnQB, 1), dim3(512, 1, 1), tsm, ta))) return rc;
-            } else {
-                s->cur_class = 1;
-                RopeArgs ra{s->qkv, E, H, D, N, d_npast, s->cs, s->q16, kc, vc, nullptr, 0};
-                if ((rc = launch_simple(s, k_rope_append, dim3((E / 2 + 255) / 256, N, 1), dim3(256, 1, 1), 0, ra))) return rc;
-                s->cur_class = 2;
-                for (int n0 = 0; n0 < N; n0 += kChunk) {
-                    aa.n0 = n0;
-                    const int cnt = N - n0 < kChunk ? N - n0 : kChunk;
-                    if ((rc = launch_simple(s, k_attn128<false>, dim3(4 * H, cnt, 1), dim3(256, 1, 1), asm_plain, aa))) return rc;
-                }
-            }
-        } else {
-            s->cur_class = 1;
-            RopeArgs ra{s->qkv, E, H, D, N, d_npast, s->cs, s->q16, kc, vc, s->cols, s->sess_stride};
-            if ((rc = launch_simple(s, k_rope_append, dim3((E / 2 + 255) / 256, N, 1), dim3(256, 1, 1), 0, ra))) return rc;
-            s->cur_class = 2;
-            AttnArgs aa{s->q16, kc, vc, d_npast, E, H, D, N, s->texp, s->att, 1.0f / sqrtf((float) E / (float) H), s->cols, s->sess_stride};
-            const size_t asm_bytes = (size_t)((s->n_ctx + 3) & ~3) * 4 + (size_t)((s->n_ctx + 7) & ~7) * 2 + (size_t) 4 * D * 8 * 4 + 64;
-            if ((rc = launch_simple(s, k_attention, dim3(H, N, 1), dim3(512, 1, 1), asm_bytes, aa))) return rc;
-        }
-        if (s->wtype == kWT_F16) {
-            GemvF16Args f{}; f.K = E; f.x = s->att; f.ldx = E; f.N = N; f.tsilu = s->tsilu;
-            s->cur_class = 3;
-            f.rows = E; f.W = Lw.f_o; f.resid = cur; f.ldr = E; f.y = s->ffin; f.ldy = E;
-            if ((rc = launch_f16<PRO_PLAIN, EPI_RESID>(s, f))) return rc;
-            s->cur_class = 4;
-            GemvF16Args g{}; g.K = E; g.x = s->ffin; g.ldx = E; g.norm_w = Lw.ffn_norm; g.N = N; g.tsilu = s->tsilu;
-            g.rows = FF; g.W = Lw.f_1; g.W2 = Lw.f_3; g.y = s->gate; g.ldy = FF;
-            if ((rc = launch_f16<PRO_NORM, EPI_GATE>(s, g))) return rc;
-            s->cur_class = 5;
-            GemvF16Args w{}; w.K = FF; w.x = s->gate; w.ldx = FF; w.N = N; w.tsilu = s->tsilu;
-            w.rows = E; w.W = Lw.f_2; w.resid = s->ffin; w.ldr = E; w.y = nxt; w.ldy = E;
-            if ((rc = launch_f16<PRO_PLAIN, EPI_RESID>(s, w))) return rc;
-        } else if (kq) {
-            s->cur_class = 3;
-            GemvArgs o{}; o.W = Lw.wo; o.x = s->att; o.ldx = E; o.resid = cur; o.ldr = E; o.y = s->ffin; o.ldy = E;
-            o.N = N; o.out_rows = E; o.tsilu = s->tsilu;
-            if ((rc = quant_kq(s, o, false)) || (rc = launch_gemv_kq<1, PRO_PREQ, EPI_RESID>(s, o))) return rc;
-            s->cur_class = 4;
-            GemvArgs g{}; g.W = Lw.w13; g.x = s->ffin; g.ldx = E; g.norm_w = Lw.ffn_norm; g.y = s->gate; g.ldy = FF;
-            g.N = N; g.out_rows = FF; g.tsilu = s->tsilu;
-            if ((rc = quant_kq(s, g, true)) || (rc = launch_gemv_kq<2, PRO_PREQ, EPI_GATE>(s, g))) return rc;
-            s->cur_class = 5;
-            GemvArgs w{}; w.W = Lw.w2; w.x = s->gate; w.ldx = FF; w.resid = s->ffin; w.ldr = E; w.y = nxt; w.ldy = E;
-            w.N = N; w.out_rows = E; w.tsilu = s->tsilu;
-            if ((rc = quant_kq(s, w, false))) return rc;
-            if (s->fold_send && il == s->L - 1) {
-                w.mb_mine = (MailboxHdr *) s->mb_block;
-                w.mb_peer_inbox = (uint2 *)(s->mb_next + sizeof(MailboxHdr)); w.mb_slot_elems = s->mb_slot_floats;
-                rc = Lw.w2.wtype == kWT_Q4_K ? launch_gemv_t<kWT_Q4_K, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w)
-                                             : launch_gemv_t<kWT_Q6_K, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
-                if (rc) return rc;
-            } else if ((rc = launch_gemv_kq<1, PRO_PREQ, EPI_RESID>(s, w))) return rc;
-        } else if (fast) {
-            s->cur_class = 3;
-            if ((rc = launch_prep<false>(s, s->att, E, nullptr, E, N))) return rc;
-            if ((rc = launch_fast_any<FG_RESID>(s, Lw.wo, cur, E, s->ffin, E, N, E))) return rc;
-            s->cur_class = 4;
-            if ((rc = launch_prep<true>(s, s->ffin, E, Lw.ffn_norm, E, N))) return rc;
-            if ((rc = launch_fast_any<FG_GATE>(s, Lw.w13, nullptr, 0, s->gate, FF, N, FF))) return rc;
-            s->cur_class = 5;
-            if ((rc = launch_prep<false>(s, s->gate, FF, nullptr, FF, N))) return rc;
-            if ((rc = launch_fast_any<FG_RESID>(s, Lw.w2, s->ffin, E, nxt, E, N, E))) return rc;
-        } else {
-            const float dsc = wt_act_scale(s->wtype);
-            s->cur_class = 3;
-            GemvArgs o{}; o.W = Lw.wo; o.x = s->att; o.ldx = E; o.resid = cur; o.ldr = E; o.y = s->ffin; o.ldy = E;
-            o.N = N; o.out_rows = E; o.tsilu = s->tsilu; o.aq_in = s->aq_att; o.da_in = s->da_att; o.in_soff = s->soffE; o.out_soff = s->soffE;
-            o.nq_norm_w = Lw.ffn_norm; o.nq_counter = s->nq_counter; o.nq_partial = s->nq_partial; o.aq_out = s->aq_x; o.da_out = s->da_x; o.out_nbq = s->nbqE; o.out_dscale = dsc;
-            if (D == 128) {
-                if (nq) { if ((rc = launch_gemv<1, PRO_PREQ, EPI_RESID_NQ>(s, o))) return rc; }
-                else    { if ((rc = launch_gemv<1, PRO_PREQ, EPI_RESID>(s, o))) return rc; }
-            } else {
-                if (nq) { if ((rc = launch_gemv<1, PRO_PLAIN, EPI_RESID_NQ>(s, o))) return rc; }
-                else    { if ((rc = launch_gemv<1, PRO_PLAIN, EPI_RESID>(s, o))) return rc; }
-            }
-            s->cur_class = 4;
-            GemvArgs g{}; g.W = Lw.w13; g.x = s->ffin; g.ldx = E; g.norm_w = Lw.ffn_norm; g.y = s->gate; g.ldy = FF;
-            g.N = N; g.out_rows = FF; g.tsilu = s->tsilu; g.aq_in = s->aq_x; g.da_in = s->da_x; g.in_soff = s->soffE; g.out_soff = s->soffF;
-            g.aq_out = s->aq_gate; g.da_out = s->da_gate; g.out_nbq = s->nbqF; g.out_dscale = dsc;
-            if (nq) { if ((rc = launch_gemv<2, PRO_PREQ, EPI_GATEQ>(s, g))) return rc; }
-            else if (N > 1) {
-                if ((rc = launch_norm_quant(s, s->ffin, E, Lw.ffn_norm, N))) return rc;
-                if ((rc = launch_gemv<2, PRO_PREQ, EPI_GATEQ>(s, g))) return rc;
-            }
-            else    { if ((rc = launch_gemv<2, PRO_NORM, EPI_GATEQ>(s, g))) return rc; }
-            s->cur_class = 5;
-            GemvArgs w{}; w.W = Lw.w2; w.resid = s->ffin; w.ldr = E; w.y = nxt; w.ldy = E;
-            w.N = N; w.out_rows = E; w.tsilu = s->tsilu; w.aq_in = s->aq_gate; w.da_in = s->da_gate; w.in_soff = s->soffF; w.out_soff = s->soffE;
-            if (il + 1 < s->L && nq) {
-                w.nq_norm_w = s->layers[il + 1].attn_norm; w.nq_counter = s->nq_counter; w.nq_partial = s->nq_partial; w.aq_out = s->aq_x; w.da_out = s->da_x;
-                w.out_nbq = s->nbqE; w.out_dscale = dsc;
-                if ((rc = launch_gemv<1, PRO_PREQ, EPI_RESID_NQ>(s, w))) return rc;
-            } else if (s->fold_send && il == s->L - 1) {
-                w.mb_mine = (MailboxHdr *) s->mb_block;
-                w.mb_peer_inbox = (uint2 *)(s->mb_next + sizeof(MailboxHdr)); w.mb_slot_elems = s->mb_slot_floats;
-                if (s->wtype == kWT_Q4_0) rc = launch_gemv_t<kWT_Q4_0, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
-                else if (s->wtype == kWT_Q4_1) rc = launch_gemv_t<kWT_Q4_1, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
-                else if (s->wtype == kWT_Q5_0) rc = launch_gemv_t<kWT_Q5_0, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
-                else if (s->wtype == kWT_Q5_1) rc = launch_gemv_t<kWT_Q5_1, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
-                else if (s->wtype == kWT_Q8_0) rc = launch_gemv_t<kWT_Q8_0, 1, 1, PRO_PREQ, EPI_RESID_SEND, true>(s, w);
-                else rc = fail(B200_EINVAL, "no pipelined matmul for weight type %d", s->wtype);
-                if (rc) return rc;
-            } else if ((rc = launch_gemv<1, PRO_PREQ, EPI_RESID>(s, w))) return rc;
-        }
+        if (s->wtype == kWT_F16)        rc = layer_f16(s, il, N, cur, nxt);
+        else if (wt_kquant(s->wtype))   rc = layer_kquant(s, il, N, cur, nxt);
+        else if (fast)                  rc = layer_fast(s, il, N, cur, nxt);
+        else                            rc = layer_exact(s, il, N, cur, nxt);
+        if (rc) return rc;
         cur = nxt;
     }
+    s->cur_class = 6;
     if (s->send_pending) {
         // pipeline hand-off: the activation leaves for the next slice's GPU right behind the last matmul
         s->send_pending = false;
-        s->cur_class = 6;
-        int rc = launch_simple(s, k_peer_send, dim3(s->send_ctas, 1, 1), dim3(1024, 1, 1), 0, s->send_args);
-        if (rc) return rc;
+        if ((rc = launch(s, k_peer_send, dim3(s->send_ctas, 1, 1), dim3(1024, 1, 1), 0, s->send_args))) return rc;
     }
-    {
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(1); cfg.blockDim = dim3(32); cfg.stream = s->stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = at; cfg.numAttrs = s->use_pdl ? 1 : 0;
-        s->cur_class = 6;
-        prof_begin(s);
-        if (s->cols) B200_CUDA(cudaLaunchKernelEx(&cfg, k_advance_cols, s->d_npast, s->cols, N));
-        else if (s->fold_send) B200_CUDA(cudaLaunchKernelEx(&cfg, k_advance_sent, s->d_npast + s->cur, N, (MailboxHdr *) s->mb_block));
-        else         B200_CUDA(cudaLaunchKernelEx(&cfg, k_advance, s->d_npast + s->cur, N));
-        prof_end(s);
-        s->launches++;
-    }
-    return 0;
+    if (s->cols) return launch(s, k_advance_cols, dim3(1), dim3(32), 0, s->d_npast, s->cols, N);
+    if (s->fold_send) return launch(s, k_advance_sent, dim3(1), dim3(32), 0, s->d_npast + s->cur, N, (MailboxHdr *) s->mb_block);
+    return launch(s, k_advance, dim3(1), dim3(32), 0, s->d_npast + s->cur, N);
 }
 
 // kernel launches of one captured single-token step over the slice (k-quant slices: + one k_quant_q8k per matmul input,
@@ -983,21 +944,14 @@ static int load_locked(b200_slice * s, const char * path) {
     s->E = (int) f.n_embd; s->H = (int) f.n_head; s->D = s->E / s->H; s->L = (int) f.n_layer; s->first_layer = (int) f.first_layer;
     s->FF = (int)(((2 * (4 * f.n_embd) / 3 + f.n_mult - 1) / f.n_mult) * f.n_mult);   // tensor_processor.cpp:1250
     if (s->D > 128 || (s->D & 1)) return fail(B200_EFILE, "head size %d unsupported (<=128, even)", s->D);
-    size_t attn_smem = 0;                           // dynamic shared memory of the single-token attention kernel
-    {
-        // worst-case dynamic shared memory of the attention kernels at this n_ctx (scores f32 + probabilities f16 per
-        // position, + staged rows / exp table / partials): reject the load instead of failing every forward later
-        const size_t sc_bytes = (((size_t)((s->n_ctx + 3) & ~3) * 4 + (size_t)((s->n_ctx + 7) & ~7) * 2) + 15) & ~(size_t) 15;
-        int pf_rows = 8 * ((s->n_ctx + 31) / 32); if (pf_rows > 128) pf_rows = 128;
-        const size_t need128 = sc_bytes + (size_t) 2 * pf_rows * kAttnRow + 32 * 64 + 64 + 65536;
-        const size_t need_gen = (size_t)((s->n_ctx + 3) & ~3) * 4 + (size_t)((s->n_ctx + 7) & ~7) * 2 + (size_t) 4 * s->D * 8 * 4 + 64;
-        const size_t need = s->D == 128 ? need128 : need_gen, limit = s->D == 128 ? (size_t) 200 * 1024 : (size_t) kSmemLimit;
-        if (need > limit)
-            return fail(B200_EINVAL, "n_ctx %d needs %zu B of attention shared memory (limit %zu B): largest supported n_ctx for head size %d is %d",
-                        s->n_ctx, need, limit, s->D, s->D == 128 ? (int)((limit - 2 * 128 * kAttnRow - 32 * 64 - 64 - 65536 - 16) / 6) & ~31
-                                                                 : (int)((limit - (size_t) 4 * s->D * 32 - 64) / 6) & ~31);
-        attn_smem = need;
-    }
+    // worst-case dynamic shared memory of the attention kernels at this n_ctx (the single-token kernel with the exp table
+    // staged, or k_attention): reject the load instead of failing every forward later
+    const AttnSmem am = attn_smem(s->n_ctx, s->D);
+    const size_t attn_need = s->D == 128 ? am.lut : am.generic, attn_limit = s->D == 128 ? (size_t) 200 * 1024 : (size_t) kSmemLimit;
+    if (attn_need > attn_limit)
+        return fail(B200_EINVAL, "n_ctx %d needs %zu B of attention shared memory (limit %zu B): largest supported n_ctx for head size %d is %d",
+                    s->n_ctx, attn_need, attn_limit, s->D, s->D == 128 ? (int)((attn_limit - 2 * 128 * kAttnRow - 32 * 64 - 64 - 65536 - 16) / 6) & ~31
+                                                                       : (int)((attn_limit - (size_t) 4 * s->D * 32 - 64) / 6) & ~31);
     const uint32_t E = f.n_embd, FF = (uint32_t) s->FF;
     s->layers.resize(s->L);
     int rc;
@@ -1130,7 +1084,7 @@ static int load_locked(b200_slice * s, const char * path) {
         // fewer clusters than there are heads (H100 SXM, 7B: 30 of 32): the rest wait for a whole second wave, every
         // layer.  Then the table is read through L2 instead (the same entries, so the same results).
         cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(4 * s->H, 1, 1); cfg.blockDim = dim3(256, 1, 1); cfg.dynamicSmemBytes = attn_smem;
+        cfg.gridDim = dim3(4 * s->H, 1, 1); cfg.blockDim = dim3(256, 1, 1); cfg.dynamicSmemBytes = attn_need;
         int clusters = 0;
         B200_CUDA(cudaOccupancyMaxActiveClusters(&clusters, k_attn128<true>, &cfg));
         s->attn_lut_smem = clusters >= s->H;
@@ -1195,7 +1149,6 @@ int b200_slice_load_ex(const char * path, int device, int n_ctx, int n_sessions,
     s->use_graph = env_int("B200_GRAPH", 1) != 0;
     s->use_pdl   = env_int("B200_PDL", 1) != 0;
     s->fast_prefill = env_int("B200_FAST_PREFILL", 0) != 0; s->fast_min_tokens = env_int("B200_FAST_MIN_TOKENS", 32);
-    s->fast_version = env_int("B200_FAST_V", 2);
     s->use_nq    = env_int("B200_NQ", 0) != 0;   // grid-barrier norm+quant epilogue in wo / w2 (decode): exact, opt-in (its barrier costs what it saves)
     s->opt_ns = env_int("B200_NS", 0); s->opt_cta_per_sm = env_int("B200_CTA_PER_SM", 0); s->opt_nc = env_int("B200_NC", 0);
     s->opt_pre = env_int("B200_PRE", 3); s->opt_nomath = env_int("B200_DBG_NOMATH", 0);
@@ -1562,14 +1515,14 @@ static int pipeline_step_peer(b200_slice * s, const float * d_in, int n_rows, in
     auto body = [&]() -> int {
         int e;
         s->cur_class = 6;
-        if (recv_in && (e = launch_simple(s, k_peer_recv, dim3(xfer_ctas, 1, 1), dim3(1024, 1, 1), 0, ra))) return e;
+        if (recv_in && (e = launch(s, k_peer_recv, dim3(xfer_ctas, 1, 1), dim3(1024, 1, 1), 0, ra))) return e;
         if (sends && !fold) { s->send_args = sa; s->send_pending = true; s->send_ctas = xfer_ctas; }
         s->fold_send = fold;
         e = enqueue_layers(s, in, n_rows, s->d_out);
         s->send_pending = false; s->fold_send = false;
         if (e) return e;
         s->cur_class = 6;
-        if (recv_final && (e = launch_simple(s, k_peer_recv, dim3(xfer_ctas, 1, 1), dim3(1024, 1, 1), 0, rf))) return e;
+        if (recv_final && (e = launch(s, k_peer_recv, dim3(xfer_ctas, 1, 1), dim3(1024, 1, 1), 0, rf))) return e;
         return 0;
     };
     B200_CUDA(cudaEventRecord(s->ev0, s->stream));
@@ -1744,7 +1697,7 @@ int b200_pipeline_pingpong(b200_slice_t * s, int n_rows, int iters, float * us_p
     auto send = [&]() -> int {
         if (s->mb_on) {
             PeerSendArgs sa{mine, (uint2 *)(s->mb_next + sizeof(MailboxHdr)), s->mb_slot_floats, s->d_out, (int) count};
-            return launch_simple(s, k_peer_send, dim3((unsigned) std::min<size_t>(32, (count + 8191) / 8192), 1, 1), dim3(1024, 1, 1), 0, sa);
+            return launch(s, k_peer_send, dim3((unsigned) std::min<size_t>(32, (count + 8191) / 8192), 1, 1), dim3(1024, 1, 1), 0, sa);
         }
         int rc = n.Send(s->d_out, count, kNcclFloat32, (r + 1) % W, s->nccl_comm, s->stream);
         return rc ? nccl_fail("ncclSend", rc) : 0;
@@ -1752,7 +1705,7 @@ int b200_pipeline_pingpong(b200_slice_t * s, int n_rows, int iters, float * us_p
     auto recv = [&]() -> int {
         if (s->mb_on) {
             PeerRecvArgs ra{mine, (const uint2 *)(s->mb_block + sizeof(MailboxHdr)), s->mb_slot_floats, &((MailboxHdr *) s->mb_prev)->ack, s->d_in, (int) count};
-            return launch_simple(s, k_peer_recv, dim3((unsigned) std::min<size_t>(32, (count + 8191) / 8192), 1, 1), dim3(1024, 1, 1), 0, ra);
+            return launch(s, k_peer_recv, dim3((unsigned) std::min<size_t>(32, (count + 8191) / 8192), 1, 1), dim3(1024, 1, 1), 0, ra);
         }
         int rc = n.Recv(s->d_in, count, kNcclFloat32, (r + W - 1) % W, s->nccl_comm, s->stream);
         return rc ? nccl_fail("ncclRecv", rc) : 0;
@@ -1813,7 +1766,7 @@ int b200_pipeline_collect(b200_slice_t * s, int n_rows, float * d_dst) {
         PeerRecvArgs rf{(MailboxHdr *) s->mb_block, (const uint2 *)(s->mb_block + sizeof(MailboxHdr)), s->mb_slot_floats,
                         &((MailboxHdr *) s->mb_prev)->ack, dst, (int) count};
         s->cur_class = 6;
-        int rc = launch_simple(s, k_peer_recv, dim3((unsigned) std::min<size_t>(32, (count + 8191) / 8192), 1, 1), dim3(1024, 1, 1), 0, rf);
+        int rc = launch(s, k_peer_recv, dim3((unsigned) std::min<size_t>(32, (count + 8191) / 8192), 1, 1), dim3(1024, 1, 1), 0, rf);
         if (rc) return rc;
     } else {
         NcclApi & n = nccl();
@@ -2108,12 +2061,8 @@ static int extra_logits_device(b200_extra * e, const float * emb, int n_tokens) 
     if (e->out_type == kWT_Q6_K) {
         LmHeadQ6Args q{e->out_q6k, e->n_vocab, e->E, e->d_x, e->E, e->norm_w, e->d_logits, e->n_vocab, n_tokens};
         const size_t smem = (size_t)(e->E / 256) * (64 * 4 + 4) + (size_t) e->E * 4 + 64;
-        static bool attr_set[16] = {false};
-        if (!attr_set[s->device & 15]) {
-            B200_CUDA(cudaFuncSetAttribute(k_lmhead_q6k, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-            attr_set[s->device & 15] = true;
-        }
-        return launch_simple(s, k_lmhead_q6k, dim3((e->n_vocab + 31) / 32, n_tokens, 1), dim3(256, 1, 1), smem, q);
+        if ((rc = smem_attr<k_lmhead_q6k>(s, 200 * 1024))) return rc;
+        return launch(s, k_lmhead_q6k, dim3((e->n_vocab + 31) / 32, n_tokens, 1), dim3(256, 1, 1), smem, q);
     }
     if (e->out_type == kWT_F16) {
         GemvF16Args f{}; f.K = e->E; f.x = e->d_x; f.ldx = e->E; f.norm_w = e->norm_w; f.N = n_tokens;

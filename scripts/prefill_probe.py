@@ -1,6 +1,5 @@
 """Prefill throughput probe (needs an H100): a 4-layer LLaMA-7B Q4_0 slice, one 512-token prompt in 64- / 512-token calls.
-    exact   the bit-exact multi-column k_gemv path
-    fast1   wgmma kernel of round 1 (fastgemm.cuh)            fast2   wgmma + tensor-map TMA, 128 x 256 tiles (fastgemm2.cuh)
+    exact   the bit-exact multi-column k_gemv path            fast2   wgmma + tensor-map TMA, 128 x 256 tiles (fastgemm2.cuh)
 Prints ms per call and the 32-layer-equivalent tokens/s; checks fast modes against exact (relative RMS)."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -14,8 +13,7 @@ wt = os.environ.get("PROBE_WT", "q4_0")
 path = bench.slice_file("7b", 0, L - 1)
 x = bench.synth_inputs(512, sh.n_embd, 1)
 ref = None
-for name, env, chunk in (("exact", {}, 64), ("fast1", {"B200_FAST_PREFILL": "1", "B200_FAST_V": "1"}, 512),
-                         ("fast2", {"B200_FAST_PREFILL": "1", "B200_FAST_V": "2"}, 512), ("fast2/256", {"B200_FAST_PREFILL": "1", "B200_FAST_V": "2"}, 256)):
+for name, env, chunk in (("exact", {}, 64), ("fast2", {"B200_FAST_PREFILL": "1"}, 512), ("fast2/256", {"B200_FAST_PREFILL": "1"}, 256)):
     os.environ.update(env)
     sl = capi.Slice(path, 0, 512)
     outs = []

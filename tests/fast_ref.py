@@ -1,4 +1,4 @@
-"""Float64 restatement of one fast-mode matmul (csrc/fastgemm.cuh, csrc/fastgemm2.cuh), in numpy.
+"""Float64 restatement of one fast-mode matmul (csrc/fastgemm2.cuh), in numpy.
 
 Both operands of the tensor-core matmul can be reproduced bit for bit on the host:
   * activations, as k_prep_q8_f16 makes them: [RMSNorm * w ->] Q8_0 quantise (fp16 scale, round half to even) ->

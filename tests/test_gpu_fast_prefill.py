@@ -1,4 +1,4 @@
-"""GPU: the wgmma "fast mode" prefill (csrc/fastgemm.cuh, csrc/fastgemm2.cuh) against exact mode and against a float64
+"""GPU: the wgmma "fast mode" prefill (csrc/fastgemm2.cuh) against exact mode and against a float64
 restatement of each matmul (tests/fast_ref.py).
 
 Fast mode is NOT bit-exact by design: the weight matmuls run as fp16 x fp16 -> fp32 tensor-core MMAs on operands
@@ -27,8 +27,8 @@ pytestmark = pytest.mark.gpu
 # Largest normalised error |y - y_ref| / sum_k |w16 * x16| of test_each_fast_matmul_is_within_the_float64_bound, measured
 # on an NVIDIA H100 80GB HBM3 (400 W power limit), per case over all its token counts and matmuls (w2, the longest K,
 # is the largest in every case):
-#   7b q4_0 v2 1.53e-6   7b q8_0 v2 1.55e-6   7b q4_0 v1 1.53e-6   13b q4_0 v2 1.73e-6   3b q4_0 v2 1.42e-6
-#   tiny128b q4_0 v2 5.54e-7   tiny128b q8_0 v2 5.74e-7   tiny128b q4_0 v1 5.54e-7
+#   7b q4_0 v2 1.53e-6   7b q8_0 v2 1.55e-6   13b q4_0 v2 1.73e-6   3b q4_0 v2 1.42e-6
+#   tiny128b q4_0 v2 5.54e-7   tiny128b q8_0 v2 5.74e-7
 # The error grows with K (2.5e-7 at K = 512, 7e-7 at 4096, 1.7e-6 at 13824): the tensor core adds each k16 product
 # group into the fp32 accumulator with less than round-to-nearest accuracy (the same fp16 products summed in fp32
 # by a CPU BLAS stay below 5e-8 at K = 11008).  TAU is 4x the largest, rounded up to a power of two.  At TAU, zeroing one 32-wide activation block puts >= 99.05 % of a token's outputs outside the bound.
@@ -73,17 +73,16 @@ def big_models(tmp_path_factory):
     return get
 
 
-_V = {(2, ggjt.T_Q4_0): "v2-tma-n256-q4_0", (2, ggjt.T_Q8_0): "v2-tma-n256-q8_0", (1, ggjt.T_Q4_0): "v1-q4_0"}
-_LAYER_CASES = [pytest.param("tiny128b", n, v, wt, id="%d-%s" % (n, _V[(v, wt)]))
-                for (v, wt) in _V for n in (128, 200, 33, 300)]
-_LAYER_CASES += [pytest.param(shape, 512, 2, wt, id="%s-512-%s" % (shape, _V[(2, wt)]))
+_V = {ggjt.T_Q4_0: "v2-tma-n256-q4_0", ggjt.T_Q8_0: "v2-tma-n256-q8_0"}
+_LAYER_CASES = [pytest.param("tiny128b", n, wt, id="%d-%s" % (n, _V[wt]))
+                for wt in _V for n in (128, 200, 33, 300)]
+_LAYER_CASES += [pytest.param(shape, 512, wt, id="%s-512-%s" % (shape, _V[wt]))
                  for shape in ("7b", "30b", "65b") for wt in (ggjt.T_Q4_0, ggjt.T_Q8_0)]
 
 
-@pytest.mark.parametrize("shape,n_tokens,version,wtype", _LAYER_CASES)
-def test_fast_prefill_close_to_exact(tmp_models, big_models, monkeypatch, shape, n_tokens, version, wtype):
+@pytest.mark.parametrize("shape,n_tokens,wtype", _LAYER_CASES)
+def test_fast_prefill_close_to_exact(tmp_models, big_models, shape, n_tokens, wtype):
     from distributedllm_b200 import capi
-    monkeypatch.setenv("B200_FAST_V", str(version))
     sh = ggjt.SHAPES[shape]
     path = tmp_models(shape, wtype, 0, 1) if shape.startswith("tiny") else big_models(shape, wtype)
     x = np.random.default_rng(4).standard_normal((n_tokens, sh.n_embd), dtype=np.float32)
@@ -107,10 +106,9 @@ def test_fast_prefill_close_to_exact(tmp_models, big_models, monkeypatch, shape,
     fast.close()
 
 
-@pytest.mark.parametrize("version,wtype", [(2, ggjt.T_Q4_0), (2, ggjt.T_Q8_0), (1, ggjt.T_Q4_0)])
-def test_tensor_core_matmul_alone_is_tight(tmp_models, monkeypatch, version, wtype):
+@pytest.mark.parametrize("wtype", [pytest.param(ggjt.T_Q4_0, id="2-2"), pytest.param(ggjt.T_Q8_0, id="2-8")])
+def test_tensor_core_matmul_alone_is_tight(tmp_models, wtype):
     from distributedllm_b200 import capi
-    monkeypatch.setenv("B200_FAST_V", str(version))
     sh = ggjt.SHAPES["tiny128b"]
     path = tmp_models("tiny128b", wtype, 0, 0)
     x = np.random.default_rng(4).standard_normal((128, sh.n_embd), dtype=np.float32)
@@ -173,22 +171,20 @@ def test_fast_prefill_keeps_greedy_ids_where_the_margin_allows(tmp_path):
 
 
 # ------------------------------------------------------------------------------------ each matmul against float64
-# (shape, wtype, version, token counts).  One layer each, so every matmul's input and output can be read back.
+# (shape, wtype, token counts).  One layer each, so every matmul's input and output can be read back.
 MATMUL_CASES = [
-    ("7b", ggjt.T_Q4_0, 2, (512, 300, 129, 33)),
-    ("7b", ggjt.T_Q8_0, 2, (512, 300)),
-    ("7b", ggjt.T_Q4_0, 1, (300,)),
-    ("13b", ggjt.T_Q4_0, 2, (300,)),
-    ("3b", ggjt.T_Q4_0, 2, (300,)),                # w2: K = 8640, 67.5 quads of 128
-    ("30b", ggjt.T_Q4_0, 2, (300,)),               # w2: K = 17920
-    ("30b", ggjt.T_Q8_0, 2, (300,)),
-    ("65b", ggjt.T_Q4_0, 2, (300,)),               # w2: K = 22016
-    ("65b", ggjt.T_Q8_0, 2, (300,)),
-    ("tiny128b", ggjt.T_Q4_0, 2, (128, 300)),
-    ("tiny128b", ggjt.T_Q8_0, 2, (128, 300)),
-    ("tiny128b", ggjt.T_Q4_0, 1, (128, 300)),
+    ("7b", ggjt.T_Q4_0, (512, 300, 129, 33)),
+    ("7b", ggjt.T_Q8_0, (512, 300)),
+    ("13b", ggjt.T_Q4_0, (300,)),
+    ("3b", ggjt.T_Q4_0, (300,)),                # w2: K = 8640, 67.5 quads of 128
+    ("30b", ggjt.T_Q4_0, (300,)),               # w2: K = 17920
+    ("30b", ggjt.T_Q8_0, (300,)),
+    ("65b", ggjt.T_Q4_0, (300,)),               # w2: K = 22016
+    ("65b", ggjt.T_Q8_0, (300,)),
+    ("tiny128b", ggjt.T_Q4_0, (128, 300)),
+    ("tiny128b", ggjt.T_Q8_0, (128, 300)),
 ]
-_CASE_IDS = ["%s-%s-v%d" % (c[0], ggjt.TYPE_NAME[c[1]], c[2]) for c in MATMUL_CASES]
+_CASE_IDS = ["%s-%s-v2" % (c[0], ggjt.TYPE_NAME[c[1]]) for c in MATMUL_CASES]
 
 
 def _n_sm() -> int:
@@ -196,18 +192,15 @@ def _n_sm() -> int:
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def tile_plan(shape: str, wtype: int, version: int, n: int, n_sm: int) -> dict:
-    """matmul -> (kernel instantiation, token tiles, last tile ragged), restating launch_fast_any: a matrix takes 256-token
-    tiles when (128-row tiles) x (256-token tiles) fills the SMs or when N <= 128, else 128-token tiles; v1 always 128."""
+def tile_plan(shape: str, wtype: int, n: int, n_sm: int) -> dict:
+    """matmul -> (kernel instantiation, token tiles, last tile ragged), restating launch_fast_gemm: a matrix takes 256-token
+    tiles when (128-row tiles) x (256-token tiles) fills the SMs or when N <= 128, else 128-token tiles."""
     sh = ggjt.SHAPES[shape]
     plan = {}
     for mat, rows in (("qkv", 3 * sh.n_embd), ("wo", sh.n_embd), ("w13", 2 * sh.n_ff), ("w2", sh.n_embd)):
-        if version == 1:
-            kern, nt = "v1", 128
-        else:
-            wide = (rows // 128) * -(-n // 256) >= n_sm or n <= 128
-            nt = 256 if wide else 128
-            kern = "v2-%s-nt%d" % (ggjt.TYPE_NAME[wtype], nt)
+        wide = (rows // 128) * -(-n // 256) >= n_sm or n <= 128
+        nt = 256 if wide else 128
+        kern = "v2-%s-nt%d" % (ggjt.TYPE_NAME[wtype], nt)
         plan[mat] = (kern, -(-n // nt), n % nt != 0)
     return plan
 
@@ -215,12 +208,12 @@ def tile_plan(shape: str, wtype: int, version: int, n: int, n_sm: int) -> dict:
 def test_cases_run_every_instantiation_over_several_ragged_token_tiles():
     n_sm = _n_sm()
     covered = set()
-    for shape, wtype, version, ns in MATMUL_CASES:
+    for shape, wtype, ns in MATMUL_CASES:
         for n in ns:
-            for kern, tiles, ragged in tile_plan(shape, wtype, version, n, n_sm).values():
+            for kern, tiles, ragged in tile_plan(shape, wtype, n, n_sm).values():
                 if tiles >= 2 and ragged:
                     covered.add(kern)
-    want = {"v1", "v2-q4_0-nt128", "v2-q4_0-nt256", "v2-q8_0-nt128", "v2-q8_0-nt256"}
+    want = {"v2-q4_0-nt128", "v2-q4_0-nt256", "v2-q8_0-nt128", "v2-q8_0-nt256"}
     assert want <= covered, (n_sm, sorted(want - covered))
 
 
@@ -238,15 +231,14 @@ def _outside_fraction(err_of_mutated, bound: float) -> float:
     return float(np.mean(err_of_mutated > bound))
 
 
-@pytest.mark.parametrize("shape,wtype,version,ns", MATMUL_CASES, ids=_CASE_IDS)
-def test_each_fast_matmul_is_within_the_float64_bound(tmp_models, big_models, monkeypatch, shape, wtype, version, ns):
+@pytest.mark.parametrize("shape,wtype,ns", MATMUL_CASES, ids=_CASE_IDS)
+def test_each_fast_matmul_is_within_the_float64_bound(tmp_models, big_models, shape, wtype, ns):
     """Every token and a row sample (every row of the first and last tile, 1/8 of the others, every 8-row position) of
     the four matmuls of one layer, against fast_ref's float64 sum of the same fp16 operands.  The fp16 activations the
     kernels read are proven bit-exact through the w2 input left in xh.  Also checks, in numpy only, that the bound is
     tight enough to see one lost 32-wide K block: zeroing one activation block of one token in the reference must put
     >= 99 % (95 % at 30B / 65B) of that token's outputs outside it."""
     from distributedllm_b200 import capi
-    monkeypatch.setenv("B200_FAST_V", str(version))
     sh = ggjt.SHAPES[shape]
     E, FF = sh.n_embd, sh.n_ff
     path = tmp_models(shape, wtype, 0, 0) if shape.startswith("tiny") else big_models(shape, wtype)
@@ -298,8 +290,8 @@ def test_each_fast_matmul_is_within_the_float64_bound(tmp_models, big_models, mo
             moved["w2"] = (x_2, lambda xm, t=t: fast_ref.store_error(y[t:t + 1, r_e], *fast_ref.reference(w_2, xm), ffin[t:t + 1, r_e]))
             for mat, e in errs.items():
                 worst[(n, mat)] = float(e.max())
-            print("\n[fast-matmul] %s %s v%d N=%d  max normalised error  %s" % (
-                shape, ggjt.TYPE_NAME[wtype], version, n, "  ".join("%s %.3g" % (m, worst[(n, m)]) for m in errs)))
+            print("\n[fast-matmul] %s %s N=%d  max normalised error  %s" % (
+                shape, ggjt.TYPE_NAME[wtype], n, "  ".join("%s %.3g" % (m, worst[(n, m)]) for m in errs)))
             bound = {mat: tau(FF if mat == "w2" else E) for mat in errs}
             for mat, e in errs.items():
                 assert e.max() <= bound[mat], "%s N=%d: normalised error %.3g > TAU %.3g at %d outputs" % (
@@ -310,13 +302,13 @@ def test_each_fast_matmul_is_within_the_float64_bound(tmp_models, big_models, mo
                 blk = (xm.shape[1] // 32) // 3
                 xm[0, blk * 32:(blk + 1) * 32] = 0
                 frac = _outside_fraction(err_of(xm), bound[mat])
-                print("[fast-matmul] %s %s v%d N=%d  %s: a lost K block moves %.4f of the outputs outside the bound" % (
-                    shape, ggjt.TYPE_NAME[wtype], version, n, mat, frac))
+                print("[fast-matmul] %s %s N=%d  %s: a lost K block moves %.4f of the outputs outside the bound" % (
+                    shape, ggjt.TYPE_NAME[wtype], n, mat, frac))
                 assert frac >= floor, "%s N=%d: a lost K block moves only %.3f of the outputs outside the bound" % (mat, n, frac)
     finally:
         gpu.close()
-    print("[fast-matmul] %s %s v%d  largest %.3g (2^%.2f)  %.1f s" % (
-        shape, ggjt.TYPE_NAME[wtype], version, max(worst.values()), np.log2(max(worst.values())), time.time() - t0))
+    print("[fast-matmul] %s %s  largest %.3g (2^%.2f)  %.1f s" % (
+        shape, ggjt.TYPE_NAME[wtype], max(worst.values()), np.log2(max(worst.values())), time.time() - t0))
 
 
 # ------------------------------------------------------------------------------------ fast mode is prefill-only
