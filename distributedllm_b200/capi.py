@@ -49,6 +49,8 @@ def lib() -> C.CDLL:
         L.b200_session_forward_device.argtypes = [vp, ci, vp, ci, vp, ci]
         L.b200_batch_forward.argtypes = [vp, vp, ci, vp, vp]
         L.b200_batch_forward_device.argtypes = [vp, vp, ci, vp, vp, ci]
+        L.b200_mixed_forward.argtypes = [vp, vp, vp, ci, vp, vp]
+        L.b200_mixed_forward_device.argtypes = [vp, vp, vp, ci, vp, vp, ci]
         L.b200_slice_unload.argtypes = [vp]
         L.b200_slice_clear.argtypes = [vp]
         L.b200_slice_rewind.argtypes = [vp, ci]
@@ -81,7 +83,8 @@ def lib() -> C.CDLL:
                            ("b200_pipeline_step", [vp, vp, ci, ci]),
                            ("b200_pipeline_mailbox_export", [vp, vp]), ("b200_pipeline_mailbox_connect", [vp, vp, ci]),
                            ("b200_pipeline_collect", [vp, ci, vp]), ("b200_pipeline_pingpong", [vp, ci, ci, vp]), ("b200_pipeline_transport", [vp]), ("b200_pipeline_set_transport", [vp, ci]), ("b200_pipeline_error", [vp]),
-                           ("b200_pipeline_step_session", [vp, ci, vp, ci, ci]), ("b200_pipeline_step_batch", [vp, vp, ci, vp, ci]), ("b200_pipeline_destroy", [vp]),
+                           ("b200_pipeline_step_session", [vp, ci, vp, ci, ci]), ("b200_pipeline_step_batch", [vp, vp, ci, vp, ci]),
+                           ("b200_pipeline_step_mixed", [vp, vp, vp, ci, vp, ci]), ("b200_pipeline_destroy", [vp]),
                            ("b200_extra_load", [C.c_char_p, ci, C.POINTER(vp)]), ("b200_extra_unload", [vp]),
                            ("b200_extra_dims", [vp, C.POINTER(ci), C.POINTER(ci)]),
                            ("b200_extra_embed", [vp, vp, ci, vp]), ("b200_extra_logits", [vp, vp, ci, ci, vp]),
@@ -132,6 +135,34 @@ class Slice:
     def batch_forward_device(self, sessions, d_in: int, d_out: int, sync: bool = False) -> None:
         ids = np.ascontiguousarray(sessions, dtype=np.int32)
         check(lib().b200_batch_forward_device(self._h, _ptr(ids), len(ids), C.c_void_p(d_in), C.c_void_p(d_out), int(sync)))
+
+    def mixed_forward(self, sessions, counts, x: np.ndarray) -> np.ndarray:
+        """counts[k] tokens of sessions[k] in one pass: x is [sum(counts)][n_embd], rows grouped by session in list order."""
+        ids = np.ascontiguousarray(sessions, dtype=np.int32)
+        cnt = np.ascontiguousarray(counts, dtype=np.int32)
+        if len(cnt) != len(ids):
+            raise ValueError("need one count per listed session")
+        x = np.ascontiguousarray(x, dtype=np.float32).reshape(-1, self.n_embd)
+        out = np.empty_like(x)
+        if x.shape[0] != int(cnt.astype(np.int64).sum()):
+            raise ValueError("need sum(counts) rows of n_embd floats")
+        check(lib().b200_mixed_forward(self._h, _ptr(ids), _ptr(cnt), len(ids), _ptr(x), _ptr(out)))
+        return out
+
+    def mixed_forward_device(self, sessions, counts, d_in: int, d_out: int, sync: bool = False) -> None:
+        ids = np.ascontiguousarray(sessions, dtype=np.int32)
+        cnt = np.ascontiguousarray(counts, dtype=np.int32)
+        if len(cnt) != len(ids):
+            raise ValueError("need one count per listed session")
+        check(lib().b200_mixed_forward_device(self._h, _ptr(ids), _ptr(cnt), len(ids), C.c_void_p(d_in), C.c_void_p(d_out), int(sync)))
+
+    def pipeline_step_mixed(self, sessions, counts, d_in: Optional[int], ring: int = 1) -> None:
+        """One mixed pass through the layer-slice pipeline (every rank passes the same lists)."""
+        ids = np.ascontiguousarray(sessions, dtype=np.int32)
+        cnt = np.ascontiguousarray(counts, dtype=np.int32)
+        if len(cnt) != len(ids):
+            raise ValueError("need one count per listed session")
+        check(lib().b200_pipeline_step_mixed(self._h, _ptr(ids), _ptr(cnt), len(ids), C.c_void_p(d_in), ring))
 
     def session_n_past(self, session: int) -> int:
         return lib().b200_session_n_past(self._h, session)

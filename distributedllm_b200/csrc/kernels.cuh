@@ -1233,6 +1233,7 @@ struct AttnArgs {
     float * out;                  // [N][E]
     float kq_scale;
     const int2 * cols; size_t sess_stride;   // batched step (independent sequences): column n = (session, position), T = position + 1
+    const int * col_T;            // with cols, optional: column n's row length T (the end of its session's segment in a mixed pass)
 };
 
 __global__ void __launch_bounds__(512) k_attention(const AttnArgs a) {
@@ -1241,7 +1242,10 @@ __global__ void __launch_bounds__(512) k_attention(const AttnArgs a) {
     grid_dep_wait();
     const int h = blockIdx.x, n = blockIdx.y, D = a.D, E = a.E;
     int T, tcount; const uint16_t * kcb = a.kc, * vcb = a.vc;
-    if (a.cols) { const int2 c = a.cols[n]; T = tcount = c.y + 1; kcb += (size_t) c.x * a.sess_stride; vcb += (size_t) c.x * a.sess_stride; }
+    if (a.cols) {
+        const int2 c = a.cols[n]; tcount = c.y + 1; T = a.col_T ? a.col_T[n] : tcount;
+        kcb += (size_t) c.x * a.sess_stride; vcb += (size_t) c.x * a.sess_stride;
+    }
     else { const int n_past = *a.n_past; T = n_past + a.N; tcount = n_past + n + 1; }
     float * sc = (float *) smem;                                   // [T]
     uint16_t * p16 = (uint16_t *)(sc + ((T + 3) & ~3));            // [T]
@@ -1355,7 +1359,10 @@ struct Attn128Args {
     int out_soff;                                                    // Q4_1 / Q5_1 weights: Q8_1 instead, block sums at da_out + out_soff
     int n_ctx; float kq_scale;
     unsigned long long * trace;
-    const int2 * cols; size_t sess_stride;   // batched step (FUSE only): column n = (session, position); each column is an N = 1 step
+    // column n = (session, position).  FUSE: each column is an N = 1 step (T = position + 1).  !FUSE (the prompt segments of a
+    // mixed pass): the columns' K / V rows are already appended, and col_T[n] is the row length T of column n's segment
+    const int2 * cols; size_t sess_stride;
+    const int * col_T;
     int pf_rows;                  // FUSE: rows of this CTA's K / V share staged in shared memory ahead of the dependency wait
     int lut_smem;                 // FUSE: also stage the negative half of the exp table (64 KB) -- softmax arguments are <= 0
 };
@@ -1405,7 +1412,10 @@ __global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(256) k_attn128(const
     const int h = blockIdx.x >> 2, g = blockIdx.x & 3, ny = blockIdx.y, n = a.n0 + ny, E = a.E;
     int T, tcount, pos;
     uint16_t * kc = a.kc, * vc = a.vc;
-    if (a.cols) { const int2 c = a.cols[n]; pos = c.y; T = tcount = pos + 1; kc += (size_t) c.x * a.sess_stride; vc += (size_t) c.x * a.sess_stride; }
+    if (a.cols) {
+        const int2 c = a.cols[n]; pos = c.y; tcount = pos + 1; T = (!FUSE && a.col_T) ? a.col_T[n] : tcount;
+        kc += (size_t) c.x * a.sess_stride; vc += (size_t) c.x * a.sess_stride;
+    }
     else { const int n_past = *a.n_past; T = n_past + a.N; tcount = n_past + n + 1; pos = n_past + n; }
     float * sc = (float *) smem;                                   // [T]
     uint16_t * p16 = (uint16_t *)(sc + ((T + 3) & ~3));            // [T]
@@ -1691,9 +1701,16 @@ __global__ void __launch_bounds__(1024) k_peer_send(const PeerSendArgs a) {
 //   V.p      32 f32 slots per channel (slot = t mod 32, vector j = slot / 8 -> warp-quad g), positions in ascending order,
 //            ((p0+p2)+(p1+p3)) per slot, the 8-slot tree, the (T mod 32) tail in double -- T = n_past + N of the CALL
 // Needs T = n_past + N <= kAttnTMax staged rows (139 KB); longer contexts keep the per-query cluster kernel.
+// Mixed passes (several sessions' prompt segments in one launch): blockIdx.y reads one AttnTile, i.e. up to kAttnQB queries of
+// ONE segment with that segment's session, n_past and N (T = n_past + N of the segment); tiles never mix sessions.
 // =============================================================================================
 constexpr int kAttnQB = 16;
 constexpr int kAttnTMax = 512;
+
+struct AttnTile {
+    int session, n_past, n;                        // the segment: its session, its first position and its token count
+    int q0, col;                                   // the tile's first query within the segment, and that query's column
+};
 
 struct AttnTiledArgs {
     const uint16_t * q16; const uint16_t * kc; const uint16_t * vc;
@@ -1703,16 +1720,24 @@ struct AttnTiledArgs {
     int * aq_out; float * da_out; int out_nbq; float out_dscale; int out_soff;
     float kq_scale;
     int t_rows, t_pad;                             // staged rows (>= n_past + N) and the padded score row length
+    const AttnTile * tiles; size_t sess_stride;    // mixed pass: one tile per blockIdx.y, cache base += session * stride
 };
 
 __global__ void __launch_bounds__(512) k_attn128_tiled(const AttnTiledArgs a) {
     extern __shared__ __align__(16) uint8_t smem[];
     if (threadIdx.x == 0) grid_dep_launch();
     grid_dep_wait();
-    const int h = blockIdx.x, n0 = blockIdx.y * kAttnQB, E = a.E;
+    const int h = blockIdx.x, E = a.E;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int n_past = *a.n_past, T = n_past + a.N;
-    const int nq = min(kAttnQB, a.N - n0);                               // queries of this block
+    // n0: the block's first query within its segment (positions n_past + n0 + q), c0: its column (rows of q16 / out)
+    int n_past, N, n0, c0; const uint16_t * kc = a.kc, * vc = a.vc;
+    if (a.tiles) {
+        const AttnTile tl = a.tiles[blockIdx.y];
+        n_past = tl.n_past; N = tl.n; n0 = tl.q0; c0 = tl.col;
+        kc += (size_t) tl.session * a.sess_stride; vc += (size_t) tl.session * a.sess_stride;
+    } else { n_past = *a.n_past; N = a.N; n0 = blockIdx.y * kAttnQB; c0 = n0; }
+    const int T = n_past + N;
+    const int nq = min(kAttnQB, N - n0);                                 // queries of this block
     const int tmax = n_past + n0 + nq;                                   // positions the block's last query sees
     uint8_t * KV = smem;                                                 // [t_rows][kAttnRow]
     float * sc = (float *)(smem + (size_t) a.t_rows * kAttnRow);         // [QB][t_pad]
@@ -1723,11 +1748,11 @@ __global__ void __launch_bounds__(512) k_attn128_tiled(const AttnTiledArgs a) {
     // ---- stage the head's key rows t < tmax and the block's query rows
     for (int idx = tid; idx < tmax * 16; idx += 512) {
         const int t = idx >> 4, ch = idx & 15;
-        cp_async16(KV + (size_t) t * kAttnRow + ch * 16, a.kc + (size_t) t * E + h * 128 + ch * 8);
+        cp_async16(KV + (size_t) t * kAttnRow + ch * 16, kc + (size_t) t * E + h * 128 + ch * 8);
     }
     for (int idx = tid; idx < nq * 16; idx += 512) {
         const int q = idx >> 4, ch = idx & 15;
-        cp_async16(q16s + q * 128 + ch * 8, a.q16 + (size_t)(n0 + q) * E + h * 128 + ch * 8);
+        cp_async16(q16s + q * 128 + ch * 8, a.q16 + (size_t)(c0 + q) * E + h * 128 + ch * 8);
     }
     cp_async_wait_all();
     __syncthreads();
@@ -1778,7 +1803,7 @@ __global__ void __launch_bounds__(512) k_attn128_tiled(const AttnTiledArgs a) {
     // ---- softmax: warp q owns query q; meanwhile the value rows replace the key rows
     for (int idx = tid; idx < tmax * 16; idx += 512) {
         const int t = idx >> 4, ch = idx & 15;
-        cp_async16(KV + (size_t) t * kAttnRow + ch * 16, a.vc + (size_t) t * E + h * 128 + ch * 8);
+        cp_async16(KV + (size_t) t * kAttnRow + ch * 16, vc + (size_t) t * E + h * 128 + ch * 8);
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
     if (warp < nq) {
@@ -1809,7 +1834,7 @@ __global__ void __launch_bounds__(512) k_attn128_tiled(const AttnTiledArgs a) {
     for (int q0 = 0; q0 < nq; q0 += 4) {
         const int q = q0 + grp;
         const bool live = q < nq;
-        const int n = n0 + q, tcount = n_past + n + 1, lim = live ? min(npT, tcount) : 0;
+        const int n = c0 + q, tcount = n_past + n0 + q + 1, lim = live ? min(npT, tcount) : 0;
         const uint16_t * p_q = p16 + (size_t) q * a.t_pad;
         float acc[4][8];
         #pragma unroll
@@ -1865,8 +1890,11 @@ __global__ void k_advance_sent(int * n_past, int by, MailboxHdr * mine) {
     grid_dep_wait();
     if (threadIdx.x == 0) { *n_past += by; mine->seq_out = mine->seq_out + 1; }
 }
-// batched step: every listed session moves one position
-__global__ void k_advance_cols(int * n_past, const int2 * cols, int n) { grid_dep_wait(); if ((int) threadIdx.x < n) n_past[cols[threadIdx.x].x] += 1; }
+// batched / mixed pass: segment i = (session, count) moves its session count positions (sessions are distinct)
+__global__ void k_advance_segs(int * n_past, const int2 * segs, int n) {
+    grid_dep_wait();
+    for (int i = threadIdx.x; i < n; i += blockDim.x) n_past[segs[i].x] += segs[i].y;
+}
 
 }  // namespace b200
 

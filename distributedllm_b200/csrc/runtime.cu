@@ -54,7 +54,13 @@ struct b200_slice {
     std::vector<int> past;                 // n_past per session
     int * d_npast = nullptr;               // [n_sessions], device copy (graph replays read it)
     size_t sess_stride = 0;                // elements between two sessions' KV caches
-    int2 * d_cols = nullptr; const int2 * cols = nullptr;   // batched step: column -> (session, position)
+    // batched and mixed passes (begin_pass): segment k runs segs[k].count tokens of session segs[k].session; the device table
+    // d_pass holds, per pass, column -> (session, position), segment -> (session, count) and, when a segment has more than
+    // one token, column -> row length (the end of its segment) and the tile table of the query-tiled attention
+    struct Seg { int session, past, count, col; };
+    std::vector<Seg> segs; std::vector<int> h_pass;
+    int * d_pass = nullptr; const int2 * cols = nullptr; const int * col_T = nullptr; const int2 * d_segs = nullptr;
+    const AttnTile * d_tiles = nullptr; int n_tiles = 0, tile_rows = 0;
     std::vector<LayerW> layers;
     std::vector<void *> allocs;
     uint16_t * kc = nullptr, * vc = nullptr, * q16 = nullptr;
@@ -416,6 +422,11 @@ static AttnSmem attn_smem(int n_ctx, int D) {
     return m;
 }
 
+// A prompt segment of a mixed pass whose whole context fits the staged window takes the query-tiled attention kernel
+static bool seg_tiled(const b200_slice * s, const b200_slice::Seg & g) {
+    return s->D == 128 && s->use_tiled_attn && g.count > 1 && g.past + g.count <= kAttnTMax;
+}
+
 // RoPE, KV-cache append and attention of layer il over s->qkv, into s->att.  With `preq` the head-size-128 kernels also
 // write their output quantised for the wo matmul (aq_att / da_att).
 static int attention(b200_slice * s, int il, int N, bool preq) {
@@ -433,7 +444,7 @@ static int attention(b200_slice * s, int il, int N, bool preq) {
         RopeArgs ra{s->qkv, E, H, D, N, d_npast, s->cs, s->q16, kc, vc, s->cols, s->sess_stride};
         if ((rc = launch(s, k_rope_append, dim3((E / 2 + 255) / 256, N, 1), dim3(256, 1, 1), 0, ra))) return rc;
         s->cur_class = 2;
-        AttnArgs aa{s->q16, kc, vc, d_npast, E, H, D, N, s->texp, s->att, kq_scale, s->cols, s->sess_stride};
+        AttnArgs aa{s->q16, kc, vc, d_npast, E, H, D, N, s->texp, s->att, kq_scale, s->cols, s->sess_stride, s->col_T};
         return launch(s, k_attention, dim3(H, N, 1), dim3(512, 1, 1), am.generic, aa);
     }
     // head size 128: cluster kernel; for single-token and batched steps RoPE + KV append are fused into its prologue
@@ -446,13 +457,61 @@ static int attention(b200_slice * s, int il, int N, bool preq) {
     aa.n_ctx = s->n_ctx; aa.kq_scale = kq_scale;
     const float dsc = preq ? wt_act_scale(s->wtype) : 0.f;
     if (preq) { aa.aq_out = s->aq_att; aa.da_out = s->da_att; aa.out_nbq = s->nbqE; aa.out_dscale = dsc; aa.out_soff = s->soffE; }
-    if (s->cols) {
-        // every column is an independent N = 1 step: the fused (RoPE + append) kernel, one cluster row per column
+    // the query-tiled kernel over a prompt chunk of one session (tiles null) or over every tile of a mixed pass; t_rows is the
+    // largest row length among the chunks it covers
+    auto launch_tiled = [&](int t_rows, int n_blocks, const AttnTile * tiles) {
+        AttnTiledArgs ta{};
+        ta.q16 = s->q16; ta.kc = kc; ta.vc = vc; ta.n_past = d_npast; ta.E = E; ta.H = H; ta.N = N; ta.texp = s->texp; ta.out = s->att;
+        if (preq) { ta.aq_out = s->aq_att; ta.da_out = s->da_att; ta.out_nbq = s->nbqE; ta.out_dscale = dsc; ta.out_soff = s->soffE; }
+        ta.kq_scale = kq_scale; ta.t_rows = t_rows; ta.t_pad = (t_rows + 31) & ~31;
+        ta.tiles = tiles; ta.sess_stride = s->sess_stride;
+        const size_t tsm = (size_t) ta.t_rows * kAttnRow + (size_t) kAttnQB * ta.t_pad * 6 + 4 * 8 * 128 * 4 + kAttnQB * 256 + 64;
+        if (int e = smem_attr<k_attn128_tiled>(s, kSmemLimit)) return e;
+        return launch(s, k_attn128_tiled, dim3(H, n_blocks, 1), dim3(512, 1, 1), tsm, ta);
+    };
+    // columns [c0, c0 + cnt) that are each an independent N = 1 step: the fused (RoPE + append) kernel, one cluster row per column
+    auto launch_fused_cols = [&](int c0, int cnt) {
+        for (int n0 = 0; n0 < cnt; n0 += kChunk) {
+            aa.n0 = c0 + n0;
+            if (int e = launch(s, k_attn128<true>, dim3(4 * H, std::min(cnt - n0, kChunk), 1), dim3(256, 1, 1), am.staged, aa)) return e;
+        }
+        return 0;
+    };
+    if (s->cols && !s->col_T) {
+        // batched step: every column is a single-token step
         s->cur_class = 2;
-        for (int n0 = 0; n0 < N; n0 += kChunk) {
-            aa.n0 = n0;
-            const int cnt = N - n0 < kChunk ? N - n0 : kChunk;
-            if ((rc = launch(s, k_attn128<true>, dim3(4 * H, cnt, 1), dim3(256, 1, 1), am.staged, aa))) return rc;
+        return launch_fused_cols(0, N);
+    }
+    if (s->cols) {
+        // Mixed pass.  A prompt segment's column j attends to the K / V rows its columns < j append in this layer, so the
+        // fused kernel only serves the single-token segments (runs of adjacent ones share a launch).  The prompt segments are
+        // appended first, then attended with T = the end of their segment: those within the staged window by one
+        // query-tiled launch over the pass's tile table, the longer ones by the per-query cluster kernel.  All kernels are
+        // on one stream, so every append is complete before an attention kernel reads the cache.
+        const std::vector<b200_slice::Seg> & sg = s->segs;
+        s->cur_class = 2;
+        for (size_t k = 0; k < sg.size();) {
+            size_t e = k;
+            while (e < sg.size() && sg[e].count == 1) e++;
+            if (e > k && (rc = launch_fused_cols(sg[k].col, sg[e - 1].col + 1 - sg[k].col))) return rc;
+            k = e + 1;
+        }
+        s->cur_class = 1;
+        for (const b200_slice::Seg & g : sg) {
+            if (g.count == 1) continue;
+            RopeArgs ra{s->qkv + (size_t) g.col * 3 * E, E, H, D, g.count, d_npast, s->cs, s->q16 + (size_t) g.col * E, kc, vc,
+                        s->cols + g.col, s->sess_stride};
+            if ((rc = launch(s, k_rope_append, dim3((E / 2 + 255) / 256, g.count, 1), dim3(256, 1, 1), 0, ra))) return rc;
+        }
+        s->cur_class = 2;
+        if (s->n_tiles && (rc = launch_tiled(s->tile_rows, s->n_tiles, s->d_tiles))) return rc;
+        aa.col_T = s->col_T;
+        for (const b200_slice::Seg & g : sg) {
+            if (g.count == 1 || seg_tiled(s, g)) continue;
+            for (int n0 = 0; n0 < g.count; n0 += kChunk) {
+                aa.n0 = g.col + n0;
+                if ((rc = launch(s, k_attn128<false>, dim3(4 * H, std::min(g.count - n0, kChunk), 1), dim3(256, 1, 1), am.plain, aa))) return rc;
+            }
         }
         return 0;
     }
@@ -467,17 +526,9 @@ static int attention(b200_slice * s, int il, int N, bool preq) {
     RopeArgs ra{s->qkv, E, H, D, N, d_npast, s->cs, s->q16, kc, vc, nullptr, 0};
     if ((rc = launch(s, k_rope_append, dim3((E / 2 + 255) / 256, N, 1), dim3(256, 1, 1), 0, ra))) return rc;
     s->cur_class = 2;
-    if (s->use_tiled_attn && s->past[s->cur] + N <= kAttnTMax) {
+    if (s->use_tiled_attn && s->past[s->cur] + N <= kAttnTMax)
         // prompt chunk whose whole context fits the staged window: query-tiled kernel, K / V read once per 16 queries
-        const int Tn = s->past[s->cur] + N;
-        AttnTiledArgs ta{};
-        ta.q16 = s->q16; ta.kc = kc; ta.vc = vc; ta.n_past = d_npast; ta.E = E; ta.H = H; ta.N = N; ta.texp = s->texp; ta.out = s->att;
-        if (preq) { ta.aq_out = s->aq_att; ta.da_out = s->da_att; ta.out_nbq = s->nbqE; ta.out_dscale = dsc; ta.out_soff = s->soffE; }
-        ta.kq_scale = kq_scale; ta.t_rows = Tn; ta.t_pad = (Tn + 31) & ~31;
-        const size_t tsm = (size_t) ta.t_rows * kAttnRow + (size_t) kAttnQB * ta.t_pad * 6 + 4 * 8 * 128 * 4 + kAttnQB * 256 + 64;
-        if ((rc = smem_attr<k_attn128_tiled>(s, kSmemLimit))) return rc;
-        return launch(s, k_attn128_tiled, dim3(H, (N + kAttnQB - 1) / kAttnQB, 1), dim3(512, 1, 1), tsm, ta);
-    }
+        return launch_tiled(s->past[s->cur] + N, (N + kAttnQB - 1) / kAttnQB, nullptr);
     for (int n0 = 0; n0 < N; n0 += kChunk) {
         aa.n0 = n0;
         const int cnt = N - n0 < kChunk ? N - n0 : kChunk;
@@ -612,8 +663,9 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
     for (int il = 0; il < s->L; il++) {
         const LayerW & Lw = s->layers[il];
         float * nxt = (il == s->L - 1) ? out : ((il & 1) ? s->xb : s->xa);
-        // fast mode is for prefill calls only: a single-token step or a batched step (cols: one token of each of N sessions)
-        // stays exact, so decode and batch_forward keep the reference's bits whatever min_tokens is
+        // fast mode is for single-session prefill calls only: a single-token step, a batched step or a mixed pass (cols:
+        // columns of several sessions) stays exact, so decode, batch_forward and mixed_forward keep the reference's bits
+        // whatever min_tokens is
         const bool fast = s->fast_prefill && N > 1 && !s->cols && N >= s->fast_min_tokens &&
                           (s->wtype == kWT_Q4_0 || s->wtype == kWT_Q8_0) &&
                           (Lw.qkv.n_tiles * Lw.qkv.TR) % 16 == 0 &&
@@ -632,7 +684,7 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
         s->send_pending = false;
         if ((rc = launch(s, k_peer_send, dim3(s->send_ctas, 1, 1), dim3(1024, 1, 1), 0, s->send_args))) return rc;
     }
-    if (s->cols) return launch(s, k_advance_cols, dim3(1), dim3(32), 0, s->d_npast, s->cols, N);
+    if (s->cols) return launch(s, k_advance_segs, dim3(1), dim3(32), 0, s->d_npast, s->d_segs, (int) s->segs.size());
     if (s->fold_send) return launch(s, k_advance_sent, dim3(1), dim3(32), 0, s->d_npast + s->cur, N, (MailboxHdr *) s->mb_block);
     return launch(s, k_advance, dim3(1), dim3(32), 0, s->d_npast + s->cur, N);
 }
@@ -721,43 +773,98 @@ static int forward_locked(b200_slice * s, const float * in, int N, float * out, 
     return 0;
 }
 
-// One token for each of B distinct sessions in a single pass: the weight matmuls see B columns (weights read once),
-// attention / RoPE / KV append run per column against that session's cache at that session's position.  Every column
-// is arithmetically the N = 1 step of its own sequence, so results are bit-identical to stepping the sessions one by one.
-static int batch_locked(b200_slice * s, const int * sessions, int B, const float * in, float * out, bool host) {
-    if (B <= 0 || B > s->n_sessions || B > s->n_ctx) return fail(B200_EINVAL, "batch of %d sequences with %d sessions", B, s->n_sessions);
-    std::vector<int2> cols(B);
+// ---------------------------------------------------------------- batched and mixed passes
+// One pass over n_seq distinct sessions: sessions[k] runs counts[k] tokens (counts == nullptr: one each) at its own
+// positions past .. past + counts[k] - 1, and its rows follow those of sessions[k - 1].  The weight matmuls see every row
+// as one column (weights read once); RoPE, the KV append and attention run per column against that session's cache.  Each
+// session's rows are arithmetically those of b200_session_forward on that session alone, so results are bit-identical.
+// Checks the whole list before anything moves; *total is the number of rows.
+static int check_pass(const b200_slice * s, const int * sessions, const int * counts, int n_seq, int * total) {
+    if (n_seq <= 0 || n_seq > s->n_sessions || n_seq > s->n_ctx) return fail(B200_EINVAL, "pass over %d sessions on a slice with %d sessions", n_seq, s->n_sessions);
     std::vector<char> seen(s->n_sessions, 0);
-    for (int b = 0; b < B; b++) {
-        const int k = sessions[b];
+    long long rows = 0;
+    for (int b = 0; b < n_seq; b++) {
+        const int k = sessions[b], c = counts ? counts[b] : 1;
         if (k < 0 || k >= s->n_sessions) return fail(B200_EINVAL, "session %d outside [0, %d)", k, s->n_sessions);
-        if (seen[k]) return fail(B200_EINVAL, "session %d listed twice in one batched step", k);
+        if (seen[k]) return fail(B200_EINVAL, "session %d listed twice in one pass", k);
         seen[k] = 1;
-        if (s->past[k] + 1 > s->n_ctx) return fail(B200_ECONTEXT, "context overflow: session %d n_past %d + 1 > n_ctx %d", k, s->past[k], s->n_ctx);
-        cols[b] = make_int2(k, s->past[k]);
+        if (c <= 0) return fail(B200_EINVAL, "session %d: token count %d must be positive", k, c);
+        if (s->past[k] + c > s->n_ctx)
+            return fail(B200_ECONTEXT, "context overflow: session %d n_past %d + %d > n_ctx %d", k, s->past[k], c, s->n_ctx);
+        rows += c;
     }
+    if (rows > s->n_ctx) return fail(B200_EINVAL, "%lld rows in one pass exceed n_ctx %d", rows, s->n_ctx);
+    *total = (int) rows;
+    return 0;
+}
+
+// Builds the pass's tables (see b200_slice::segs) and uploads them in one copy on the slice's stream; from here until
+// end_pass, enqueue_layers runs the pass.  An all-single-token pass (a batched step) has no row lengths and no tiles.
+static int begin_pass(b200_slice * s, const int * sessions, const int * counts, int n_seq, int N) {
+    std::vector<int> & h = s->h_pass;
+    h.assign((size_t) 2 * N + 2 * n_seq, 0);
+    s->segs.resize(n_seq);
+    bool multi = false;
+    for (int k = 0, col = 0; k < n_seq; k++) {
+        const int id = sessions[k], c = counts ? counts[k] : 1, past = s->past[id];
+        s->segs[k] = {id, past, c, col};
+        for (int j = 0; j < c; j++) { h[2 * (col + j)] = id; h[2 * (col + j) + 1] = past + j; }
+        h[2 * N + 2 * k] = id; h[2 * N + 2 * k + 1] = c;
+        col += c; multi |= c > 1;
+    }
+    s->n_tiles = 0; s->tile_rows = 0;
+    if (multi) {
+        for (const b200_slice::Seg & g : s->segs)
+            for (int j = 0; j < g.count; j++) h.push_back(g.past + g.count);
+        for (const b200_slice::Seg & g : s->segs) {
+            if (!seg_tiled(s, g)) continue;
+            s->tile_rows = std::max(s->tile_rows, g.past + g.count);
+            for (int q0 = 0; q0 < g.count; q0 += kAttnQB) { h.insert(h.end(), {g.session, g.past, g.count, q0, g.col + q0}); s->n_tiles++; }
+        }
+    }
+    // pageable source: the driver stages it before returning
+    B200_CUDA(cudaMemcpyAsync(s->d_pass, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
+    s->cur = 0;
+    s->cols = (const int2 *) s->d_pass;
+    s->d_segs = (const int2 *)(s->d_pass + 2 * N);
+    s->col_T = multi ? s->d_pass + 2 * N + 2 * n_seq : nullptr;
+    s->d_tiles = s->n_tiles ? (const AttnTile *)(s->d_pass + 3 * N + 2 * n_seq) : nullptr;
+    return 0;
+}
+
+static void end_pass(b200_slice * s) { s->cols = nullptr; s->col_T = nullptr; s->d_segs = nullptr; s->d_tiles = nullptr; s->n_tiles = 0; }
+
+static void advance_pass(b200_slice * s, const int * sessions, const int * counts, int n_seq) {
+    for (int k = 0; k < n_seq; k++) s->past[sessions[k]] += counts ? counts[k] : 1;
+}
+
+// rows of the pass table: columns (session, position) and row lengths, segments, tiles
+static size_t pass_table_ints(int n_ctx, int n_sessions) {
+    return (size_t) 3 * n_ctx + 2 * (size_t) n_sessions + 5 * ((size_t) n_ctx / kAttnQB + n_sessions);
+}
+
+static int pass_locked(b200_slice * s, const int * sessions, const int * counts, int n_seq, const float * in, float * out, bool host) {
+    int N = 0, rc;
+    if ((rc = check_pass(s, sessions, counts, n_seq, &N))) return rc;
     B200_CUDA(cudaSetDevice(s->device));
     B200_CUDA(cudaEventRecord(s->ev0, s->stream));
-    // pageable source: the driver stages it before returning, so the vector may go out of scope
-    B200_CUDA(cudaMemcpyAsync(s->d_cols, cols.data(), (size_t) B * sizeof(int2), cudaMemcpyHostToDevice, s->stream));
-    s->cur = 0; s->cols = s->d_cols;
-    int rc;
+    if ((rc = begin_pass(s, sessions, counts, n_seq, N))) return rc;
     if (host) {
-        B200_CUDA(cudaMemcpyAsync(s->d_in, in, (size_t) B * s->E * 4, cudaMemcpyHostToDevice, s->stream));
-        rc = enqueue_layers(s, s->d_in, B, s->d_out);
-        s->cols = nullptr;
+        B200_CUDA(cudaMemcpyAsync(s->d_in, in, (size_t) N * s->E * 4, cudaMemcpyHostToDevice, s->stream));
+        rc = enqueue_layers(s, s->d_in, N, s->d_out);
+        end_pass(s);
         if (rc) return rc;
         B200_CUDA(cudaEventRecord(s->ev1, s->stream));
-        B200_CUDA(cudaMemcpyAsync(out, s->d_out, (size_t) B * s->E * 4, cudaMemcpyDeviceToHost, s->stream));
+        B200_CUDA(cudaMemcpyAsync(out, s->d_out, (size_t) N * s->E * 4, cudaMemcpyDeviceToHost, s->stream));
         B200_CUDA(cudaStreamSynchronize(s->stream));
     } else {
-        rc = enqueue_layers(s, in, B, out);
-        s->cols = nullptr;
+        rc = enqueue_layers(s, in, N, out);
+        end_pass(s);
         if (rc) return rc;
         B200_CUDA(cudaEventRecord(s->ev1, s->stream));
     }
     s->timed = true;
-    for (int b = 0; b < B; b++) s->past[sessions[b]] += 1;
+    advance_pass(s, sessions, counts, n_seq);
     return 0;
 }
 
@@ -1036,7 +1143,7 @@ static int load_locked(b200_slice * s, const char * path) {
     s->sess_stride = (size_t) s->L * nE;
     s->past.assign(s->n_sessions, 0);
     if ((rc = dev_alloc(s, &s->kc, s->n_sessions * s->sess_stride)) || (rc = dev_alloc(s, &s->vc, s->n_sessions * s->sess_stride)) ||
-        (rc = dev_alloc(s, &s->d_cols, (size_t) s->n_ctx)) ||
+        (rc = dev_alloc(s, &s->d_pass, pass_table_ints(s->n_ctx, s->n_sessions))) ||
         (rc = dev_alloc(s, &s->q16, nE)) || (rc = dev_alloc(s, &s->xa, nE)) || (rc = dev_alloc(s, &s->xb, nE)) ||
         (rc = dev_alloc(s, &s->qkv, 3 * nE)) || (rc = dev_alloc(s, &s->att, nE)) || (rc = dev_alloc(s, &s->ffin, nE)) ||
         (rc = dev_alloc(s, &s->gate, (size_t) s->n_ctx * FF)) || (rc = dev_alloc(s, &s->d_in, nE)) ||
@@ -1282,13 +1389,28 @@ int b200_session_forward_device(b200_slice_t * s, int session, const float * d_i
 int b200_batch_forward(b200_slice_t * s, const int * sessions, int n_seq, const float * in, float * out) {
     if (!s || !sessions || !in || !out) return fail(B200_EINVAL, "null argument");
     std::lock_guard<std::mutex> lk(s->mu);
-    return batch_locked(s, sessions, n_seq, in, out, true);
+    return pass_locked(s, sessions, nullptr, n_seq, in, out, true);
 }
 
 int b200_batch_forward_device(b200_slice_t * s, const int * sessions, int n_seq, const float * d_in, float * d_out, int sync) {
     if (!s || !sessions || !d_in || !d_out) return fail(B200_EINVAL, "null argument");
     std::lock_guard<std::mutex> lk(s->mu);
-    int rc = batch_locked(s, sessions, n_seq, d_in, d_out, false);
+    int rc = pass_locked(s, sessions, nullptr, n_seq, d_in, d_out, false);
+    if (rc) return rc;
+    if (sync) B200_CUDA(cudaStreamSynchronize(s->stream));
+    return 0;
+}
+
+int b200_mixed_forward(b200_slice_t * s, const int * sessions, const int * counts, int n_seq, const float * in, float * out) {
+    if (!s || !sessions || !counts || !in || !out) return fail(B200_EINVAL, "null argument");
+    std::lock_guard<std::mutex> lk(s->mu);
+    return pass_locked(s, sessions, counts, n_seq, in, out, true);
+}
+
+int b200_mixed_forward_device(b200_slice_t * s, const int * sessions, const int * counts, int n_seq, const float * d_in, float * d_out, int sync) {
+    if (!s || !sessions || !counts || !d_in || !d_out) return fail(B200_EINVAL, "null argument");
+    std::lock_guard<std::mutex> lk(s->mu);
+    int rc = pass_locked(s, sessions, counts, n_seq, d_in, d_out, false);
     if (rc) return rc;
     if (sync) B200_CUDA(cudaStreamSynchronize(s->stream));
     return 0;
@@ -1494,7 +1616,8 @@ int b200_pipeline_init(b200_slice_t * s, int rank, int nranks, const void * id12
 // store into the next rank's mailbox + a flag, issued by k_peer_send right behind this slice's last matmul and picked
 // up by k_peer_recv in front of the next slice's first matmul.  For a single-token step the whole sequence
 // [recv ->] layers -> send [-> recv of the ring result] is ONE captured graph per rank: no host code between slices.
-static int pipeline_step_peer(b200_slice * s, const float * d_in, int n_rows, int ring, int session, const int * sessions) {
+static int pipeline_step_peer(b200_slice * s, const float * d_in, int n_rows, int ring, int session, const int * sessions,
+                              const int * counts, int n_seq) {
     const int r = s->pp_rank, W = s->pp_world;
     const size_t count = (size_t) n_rows * s->E;
     if (count > s->mb_slot_floats) return fail(B200_EINVAL, "hand-off of %zu floats exceeds the mailbox slot (%zu)", count, s->mb_slot_floats);
@@ -1527,14 +1650,11 @@ static int pipeline_step_peer(b200_slice * s, const float * d_in, int n_rows, in
     };
     B200_CUDA(cudaEventRecord(s->ev0, s->stream));
     if (sessions) {
-        std::vector<int2> cols(n_rows);
-        for (int b = 0; b < n_rows; b++) cols[b] = make_int2(sessions[b], s->past[sessions[b]]);
-        B200_CUDA(cudaMemcpyAsync(s->d_cols, cols.data(), (size_t) n_rows * sizeof(int2), cudaMemcpyHostToDevice, s->stream));
-        s->cur = 0; s->cols = s->d_cols;
+        if ((rc = begin_pass(s, sessions, counts, n_seq, n_rows))) return rc;
         rc = body();
-        s->cols = nullptr;
+        end_pass(s);
         if (rc) return rc;
-        for (int b = 0; b < n_rows; b++) s->past[sessions[b]] += 1;
+        advance_pass(s, sessions, counts, n_seq);
     } else if (n_rows == 1 && s->use_graph && !s->profiling) {
         GraphKey key{in, nullptr, (ring & 3) | (fold ? 4 : 0) | (session << 3)};
         auto it = s->pp_graphs.find(key);
@@ -1568,38 +1688,33 @@ static int pipeline_step_peer(b200_slice * s, const float * d_in, int n_rows, in
 }
 
 // recv <- rank-1, the slice's layers, send -> rank+1 (ring: the last rank hands its output back to rank 0).
-// sessions == nullptr: n_rows tokens of session `session`; else one token for each of the n_rows listed sessions.
-static int pipeline_step_locked(b200_slice * s, const float * d_in, int n_rows, int ring, int session, const int * sessions) {
+// sessions == nullptr: n_rows tokens of session `session`; else a pass over the n_rows listed sessions, counts[k] tokens of
+// sessions[k] (counts == nullptr: one each), and the hand-off is [sum of counts][n_embd].
+static int pipeline_step_locked(b200_slice * s, const float * d_in, int n_rows, int ring, int session, const int * sessions,
+                                const int * counts = nullptr) {
     NcclApi & n = nccl();
     B200_CUDA(cudaSetDevice(s->device));
     if (n_rows <= 0 || n_rows > s->n_ctx) return fail(B200_EINVAL, "n_tokens %d outside [1, n_ctx]", n_rows);
-    const size_t count = (size_t) n_rows * s->E;
+    const int n_seq = n_rows;
     const int r = s->pp_rank, W = s->pp_world;
     int rc;
     // validate the step BEFORE anything is posted: a rejected step must not leave the peer's send unmatched
     if (sessions) {
-        if (n_rows > s->n_sessions) return fail(B200_EINVAL, "batch of %d sequences with %d sessions", n_rows, s->n_sessions);
-        std::vector<char> seen(s->n_sessions, 0);
-        for (int b = 0; b < n_rows; b++) {
-            const int k = sessions[b];
-            if (k < 0 || k >= s->n_sessions) return fail(B200_EINVAL, "session %d outside [0, %d)", k, s->n_sessions);
-            if (seen[k]) return fail(B200_EINVAL, "session %d listed twice in one batched step", k);
-            seen[k] = 1;
-            if (s->past[k] + 1 > s->n_ctx) return fail(B200_ECONTEXT, "context overflow: session %d n_past %d + 1 > n_ctx %d", k, s->past[k], s->n_ctx);
-        }
+        if ((rc = check_pass(s, sessions, counts, n_seq, &n_rows))) return rc;
     } else {
         if (session < 0 || session >= s->n_sessions) return fail(B200_EINVAL, "session %d outside [0, %d)", session, s->n_sessions);
         if (s->past[session] + n_rows > s->n_ctx)
             return fail(B200_ECONTEXT, "context overflow: n_past %d + n_tokens %d > n_ctx %d", s->past[session], n_rows, s->n_ctx);
     }
+    const size_t count = (size_t) n_rows * s->E;
     if (r == 0 && !d_in) return fail(B200_EINVAL, "rank 0 needs an input buffer");
-    if (s->mb_on && W > 1) return pipeline_step_peer(s, d_in, n_rows, ring, session, sessions);
+    if (s->mb_on && W > 1) return pipeline_step_peer(s, d_in, n_rows, ring, session, sessions, counts, n_seq);
     const float * in = d_in;
     if (r > 0) {
         if ((rc = n.Recv(s->d_in, count, kNcclFloat32, r - 1, s->nccl_comm, s->stream))) return nccl_fail("ncclRecv", rc);
         in = s->d_in;
     }
-    if (sessions) rc = batch_locked(s, sessions, n_rows, in, s->d_out, false);
+    if (sessions) rc = pass_locked(s, sessions, counts, n_seq, in, s->d_out, false);
     else          rc = forward_locked(s, in, n_rows, s->d_out, false, session);
     if (rc) return rc;
     if (r < W - 1) {
@@ -1632,6 +1747,13 @@ int b200_pipeline_step_batch(b200_slice_t * s, const int * sessions, int n_seq, 
     if (!sessions) return fail(B200_EINVAL, "null session list");
     std::lock_guard<std::mutex> lk(s->mu);
     return pipeline_step_locked(s, d_in, n_seq, ring, 0, sessions);
+}
+
+int b200_pipeline_step_mixed(b200_slice_t * s, const int * sessions, const int * counts, int n_seq, const float * d_in, int ring) {
+    if (!s || !s->nccl_comm) return fail(B200_EINVAL, "pipeline not initialised");
+    if (!sessions || !counts) return fail(B200_EINVAL, "null session or count list");
+    std::lock_guard<std::mutex> lk(s->mu);
+    return pipeline_step_locked(s, d_in, n_seq, ring, 0, sessions, counts);
 }
 
 /* ---- peer-memory hand-off: mailboxes mapped across processes with cudaIpc --------------------------------------- */

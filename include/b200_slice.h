@@ -102,12 +102,25 @@ int b200_session_forward_device(b200_slice_t * s, int session, const float * d_i
 int b200_batch_forward(b200_slice_t * s, const int * sessions, int n_seq, const float * in, float * out);      /* host buffers */
 int b200_batch_forward_device(b200_slice_t * s, const int * sessions, int n_seq, const float * d_in, float * d_out, int sync);
 
+/* Mixed pass ("chunked prefill"): counts[k] tokens of sessions[k], for n_seq DISTINCT sessions, in a single pass, so a
+ * prompt chunk of one session rides along with the decode tokens of the others.  in / out are [sum of counts][n_embd]; rows
+ * are grouped by session in list order (the first counts[0] rows belong to sessions[0], the next counts[1] to sessions[1],
+ * ...), and session k's rows run at its positions n_past .. n_past + counts[k] - 1.  The weights are streamed once for all
+ * rows.  Session k's output rows are bit-identical to b200_session_forward(sessions[k], its rows, counts[k]) on that
+ * session alone (so to the reference fed the same chunks); a pass of all-1 counts is b200_batch_forward.  Fast prefill
+ * never applies.  All-or-nothing: on an error no position moves and no cache is written.
+ *   B200_EINVAL: n_seq < 1, a session out of range or listed twice, a count < 1, sum of counts > n_ctx, a null argument;
+ *   B200_ECONTEXT: n_past + counts[k] > n_ctx for some k. */
+int b200_mixed_forward(b200_slice_t * s, const int * sessions, const int * counts, int n_seq, const float * in, float * out);   /* host buffers */
+int b200_mixed_forward_device(b200_slice_t * s, const int * sessions, const int * counts, int n_seq, const float * d_in, float * d_out,
+                              int sync);
+
 /* Fast mode for prefill calls (n_tokens >= min_tokens): the Q4_0 / Q8_0 weight matmuls run on the wgmma tensor cores with
  * the dequantisation fused in (csrc/fastgemm2.cuh; Q4_1, Q5_0, Q5_1, Q4_K / Q6_K and F16 slices ignore the switch and stay exact).
  * NOT bit-exact: operands are rounded to fp16 after the reference's Q8_0 activation quantisation and summed in fp32.
  * Each matmul output is within TAU * sum_k |w16 * x16| of the float64 sum of the same fp16 operands (TAU <= 2^-16, see
  * tests/test_gpu_fast_prefill.py, which also bounds the deviation from exact mode).  Off by default (or
- * B200_FAST_PREFILL=1).  Fast mode never applies to a single-token step or to a batched step (b200_batch_forward),
+ * B200_FAST_PREFILL=1).  Fast mode never applies to a single-token step, a batched step (b200_batch_forward) or a mixed pass (b200_mixed_forward),
  * whatever min_tokens is: decode always runs in exact mode. */
 int b200_slice_set_fast_prefill(b200_slice_t * s, int on, int min_tokens);
 
@@ -171,6 +184,9 @@ int b200_pipeline_step(b200_slice_t * s, const float * d_in, int n_tokens, int r
  * between the slices).  Every rank passes the same session list. */
 int b200_pipeline_step_session(b200_slice_t * s, int session, const float * d_in, int n_tokens, int ring);
 int b200_pipeline_step_batch(b200_slice_t * s, const int * sessions, int n_seq, const float * d_in, int ring);
+/* The same for a mixed pass (b200_mixed_forward): [sum of counts][n_embd] moves between the slices.  Every rank passes the
+ * same session and count lists. */
+int b200_pipeline_step_mixed(b200_slice_t * s, const int * sessions, const int * counts, int n_seq, const float * d_in, int ring);
 /* Peer-memory hand-off (the on-box GPU-native hop): every rank owns a MAILBOX in its HBM (sequence flags + two inbox slots of
  * [n_ctx][n_embd] f32) that its ring neighbours map over NVLink with cudaIpc.  After b200_pipeline_init, each rank
  * exports its 64-byte handle, the host gathers all of them (torch.distributed all_gather, a file, ...) and every rank
