@@ -89,7 +89,8 @@ def lib() -> C.CDLL:
                            ("b200_extra_dims", [vp, C.POINTER(ci), C.POINTER(ci)]),
                            ("b200_extra_embed", [vp, vp, ci, vp]), ("b200_extra_logits", [vp, vp, ci, ci, vp]),
                            ("b200_extra_next_token", [vp, vp, ci, C.POINTER(C.c_int32)]),
-                           ("b200_extra_tokenize", [vp, C.c_char_p, vp, ci])):
+                           ("b200_extra_tokenize", [vp, C.c_char_p, vp, ci]),
+                           ("b200_generate_greedy", [vp, ci, vp, vp, vp, ci, vp, ci, vp])):
             if hasattr(L, name):
                 getattr(L, name).argtypes = args
         if hasattr(L, "b200_extra_token_text"):
@@ -275,3 +276,75 @@ class Slice:
             self.close()
         except Exception:
             pass
+
+
+class Extra:
+    """The client-side extra layers (tokenizer, tok_embeddings, norm, output) resident on one GPU."""
+
+    def __init__(self, path: str, device: int = 0):
+        self._h = C.c_void_p()
+        check(lib().b200_extra_load(os.fsencode(path), device, C.byref(self._h)))
+        self.device = device
+        v, e = C.c_int(), C.c_int()
+        check(lib().b200_extra_dims(self._h, C.byref(v), C.byref(e)))
+        self.n_vocab, self.n_embd = v.value, e.value
+
+    @property
+    def handle(self) -> C.c_void_p:
+        return self._h
+
+    def tokenize(self, prompt: str) -> list:
+        text = prompt.encode("utf-8")
+        n = lib().b200_extra_tokenize(self._h, text, None, 0)
+        if n < 0:
+            check(-n)
+        out = np.zeros(max(n, 1), np.int32)
+        lib().b200_extra_tokenize(self._h, text, _ptr(out), n)
+        return out[:n].tolist()
+
+    def embed(self, tokens) -> np.ndarray:
+        t = np.ascontiguousarray(tokens, dtype=np.int32)
+        out = np.empty((len(t), self.n_embd), np.float32)
+        check(lib().b200_extra_embed(self._h, _ptr(t), len(t), _ptr(out)))
+        return out
+
+    def logits(self, x: np.ndarray) -> np.ndarray:
+        """[n][n_embd] hidden states -> [n][n_vocab] logits (final RMSNorm + output.weight)."""
+        x = np.ascontiguousarray(x, dtype=np.float32).reshape(-1, self.n_embd)
+        out = np.empty((x.shape[0], self.n_vocab), np.float32)
+        check(lib().b200_extra_logits(self._h, _ptr(x), x.shape[0], 1, _ptr(out)))
+        return out
+
+    def next_token(self, x: np.ndarray) -> int:
+        """Argmax of the last row's logits (first maximum wins)."""
+        x = np.ascontiguousarray(x, dtype=np.float32).reshape(-1, self.n_embd)
+        tok = C.c_int32()
+        check(lib().b200_extra_next_token(self._h, _ptr(x), x.shape[0], C.byref(tok)))
+        return tok.value
+
+    def close(self) -> None:
+        if self._h:
+            check(lib().b200_extra_unload(self._h))
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def generate_greedy(slices, extra: Extra, sessions, prompts, n_steps: int) -> np.ndarray:
+    """Greedy decoding on the device (b200_generate_greedy): session sessions[k] is fed prompts[k] (a list of token ids),
+    then n_steps - 1 of its own ids.  `slices` are in layer order, all on the extra layers' GPU.  -> [n_steps][n_seq] ids."""
+    ids = np.ascontiguousarray(sessions, dtype=np.int32)
+    if len(prompts) != len(ids):
+        raise ValueError("need one prompt per listed session")
+    counts = np.array([len(p) for p in prompts], np.int32)
+    toks = np.ascontiguousarray(np.concatenate([np.asarray(p, np.int64) for p in prompts]) if len(prompts) else [],
+                                dtype=np.int32)
+    handles = (C.c_void_p * max(len(slices), 1))(*[s.handle for s in slices])
+    out = np.zeros((max(n_steps, 0), len(ids)), np.int32)
+    check(lib().b200_generate_greedy(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks),
+                                     n_steps, _ptr(out)))
+    return out

@@ -149,6 +149,25 @@ class LocalPipeline:
         devices = list(devices) if devices is not None else list(range(len(slice_paths)))
         self.slices = [capi.Slice(p, d, n_ctx) for p, d in zip(slice_paths, devices)]
         self.slices.sort(key=lambda s: s.info.first_layer)
+        self._extra = None
+
+    def generate_greedy(self, extra_path: str, prompt: str, max_steps: int = 200) -> List[int]:
+        """DistributedLLM.generate_greedy on this box: clear the contexts, tokenize, then max_steps argmax steps, all on
+        the GPU with no host round trip between tokens (capi.generate_greedy).  Needs every slice on one device."""
+        devices = sorted({s.info.device for s in self.slices})
+        if len(devices) != 1:
+            raise self.capi.B200Error(1, "greedy generation on the device needs every slice on one GPU; the slices are on "
+                                         "devices %s" % ", ".join(map(str, devices)))
+        if self._extra is None or self._extra[0] != extra_path:
+            if self._extra is not None:
+                self._extra[1].close()
+            self._extra = (extra_path, self.capi.Extra(extra_path, devices[0]))
+        extra = self._extra[1]
+        self.clear_context()
+        tokens = extra.tokenize(prompt)
+        if max_steps < 1:
+            return []
+        return self.capi.generate_greedy(self.slices, extra, [0], [tokens], max_steps)[:, 0].tolist()
 
     def propagate_tensor(self, embeddings) -> np.ndarray:
         x = np.ascontiguousarray(embeddings, dtype=np.float32)
@@ -161,5 +180,8 @@ class LocalPipeline:
             s.clear_context()
 
     def close(self):
+        if self._extra is not None:
+            self._extra[1].close()
+            self._extra = None
         for s in self.slices:
             s.close()

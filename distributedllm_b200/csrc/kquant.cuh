@@ -12,8 +12,7 @@
 //         d = y.d * fp16(x.d); min term acc_m[i] = fma(-y.d * fp16(x.dmin), (float)(m[2i] q8s[2i] + m[2i+1] q8s[2i+1]),
 //         acc_m[i]) with q8s[k] = the sum of sub-block k's 32 quants; result hsum_float_8(acc) + ((m0 + m2) + (m1 + m3)).
 //   Q6_K: sumi_l = sum_{j<2, k<4} sc[8j + 2k + (l >= 4)] * ((q6 - 32) . q8); result hsum_float_8(acc).
-// k_lmhead_q6k (kernels.cuh) computes the same Q6_K dot on its own 288-B layout; it is left as it is, so the lm_head's
-// code and results do not move.
+// A Q6_K output.weight (the client-side lm_head) is packed and multiplied like the layers' Q6_K matrices.
 #pragma once
 #include "kernels.cuh"
 

@@ -876,7 +876,7 @@ static int pass_locked(b200_slice * s, const int * sessions, const int * counts,
 struct LoadJob {
     const GgjtTensor * src[3] = {nullptr, nullptr, nullptr};
     int nsrc = 0;
-    int kind = 0;                 // 0: block-quantised matrix (k_repack), 1: F16 (k_repack_f16), 2: raw copy, 3: Q6_K (k_repack_q6k)
+    int kind = 0;                 // 0: block-quantised or k-quant matrix (k_repack, k_repack_kq), 1: F16 (k_repack_f16), 2: raw copy
     int mode = 0, G = 1;
     PackedW * out = nullptr;      // kind 0
     uint16_t ** outf = nullptr; uint16_t * into = nullptr;   // kind 1
@@ -988,9 +988,6 @@ static int run_load_jobs(b200_slice * s, const GgjtFile & f, std::vector<LoadJob
             if (!dst && (rc = dev_alloc(s, &dst, (size_t) rows * nc8 * 256 + 8))) break;
             k_repack_f16<<<s->n_sm * 8, 256, 0, s->stream>>>((const uint16_t *) lp.scratch[slot], dst, dst /*no tail: K%32==0*/, rows, K);
             *job.outf = dst;
-        } else if (job.kind == 3) {
-            const GgjtTensor & t = *job.src[0];
-            k_repack_q6k<<<s->n_sm * 8, 256, 0, s->stream>>>(lp.scratch[slot], job.raw_dst, (int) t.ne[1], (int) t.ne[0] / 256);
         } else {
             e = cudaMemcpyAsync(job.raw_dst, lp.scratch[slot], job.src[0]->nbytes, cudaMemcpyDeviceToDevice, s->stream);
             if (e != cudaSuccess) { rc = fail(B200_ECUDA, "weight copy failed: %s", cudaGetErrorString(e)); break; }
@@ -1934,8 +1931,9 @@ struct b200_extra {
     int n_vocab = 0, E = 0, emb_type = 0, out_type = 0;
     uint8_t * emb_raw = nullptr;          // tok_embeddings as stored (row = token)
     float * norm_w = nullptr;
-    PackedW out{}; uint16_t * out_f16 = nullptr; uint8_t * out_q6k = nullptr;
+    PackedW out{}; uint16_t * out_f16 = nullptr;
     float * d_x = nullptr, * d_logits = nullptr; int32_t * d_tok = nullptr, * d_best = nullptr; int cap_tokens = 0;
+    int32_t * d_ids = nullptr; int cap_ids = 0;    // b200_generate_greedy: [n_steps][n_seq] ids
     std::vector<std::pair<std::string, float>> vocab;
     std::unordered_map<std::string, int> token_to_id;
     std::mutex mu;
@@ -1984,16 +1982,37 @@ static int extra_reserve(b200_extra * e, int n) {
     b200_slice * s = &e->ctx;
     // growth: release the old staging buffers first (they are tracked in `allocs` for unload)
     cudaStreamSynchronize(s->stream);
-    for (void * old : {(void *) e->d_x, (void *) e->d_logits, (void *) e->d_tok, (void *) e->d_best}) {
+    for (void * old : {(void *) e->d_x, (void *) e->d_logits, (void *) e->d_tok, (void *) e->d_best, (void *) s->kq_aq, (void *) s->kq_ad}) {
         if (!old) continue;
         s->allocs.erase(std::remove(s->allocs.begin(), s->allocs.end(), old), s->allocs.end());
         cudaFree(old);
     }
     e->d_x = nullptr; e->d_logits = nullptr; e->d_tok = nullptr; e->d_best = nullptr; e->cap_tokens = 0;
+    s->kq_aq = nullptr; s->kq_ad = nullptr;
     int rc;
     if ((rc = dev_alloc(s, &e->d_x, (size_t) n * e->E)) || (rc = dev_alloc(s, &e->d_logits, (size_t) n * e->n_vocab)) ||
         (rc = dev_alloc(s, &e->d_tok, (size_t) n)) || (rc = dev_alloc(s, &e->d_best, (size_t) 1))) return rc;
+    if (e->out_type == kWT_Q6_K) {
+        // the Q8_K rows of a Q6_K lm_head (quant_kq): its planes are laid out for ctx.n_ctx columns
+        const int nbq = e->out.nbq;
+        if ((rc = dev_alloc(s, &s->kq_aq, (size_t) n * nbq * (64 + 8))) || (rc = dev_alloc(s, &s->kq_ad, (size_t) n * kq_nbd(nbq)))) return rc;
+        s->n_ctx = n;
+    }
     e->cap_tokens = n;
+    return 0;
+}
+
+static int extra_reserve_ids(b200_extra * e, int n) {
+    if (n <= e->cap_ids) return 0;
+    b200_slice * s = &e->ctx;
+    cudaStreamSynchronize(s->stream);
+    if (e->d_ids) {
+        s->allocs.erase(std::remove(s->allocs.begin(), s->allocs.end(), (void *) e->d_ids), s->allocs.end());
+        cudaFree(e->d_ids);
+    }
+    e->d_ids = nullptr; e->cap_ids = 0;
+    if (int rc = dev_alloc(s, &e->d_ids, (size_t) n)) return rc;
+    e->cap_ids = n;
     return 0;
 }
 
@@ -2018,6 +2037,33 @@ __global__ void __launch_bounds__(1024) k_argmax_first(const float * logits, int
             if (better(v, i, bv, bi)) { bv = v; bi = i; }
         }
         if (threadIdx.x == 0) *out = bi == 0x7fffffff ? 0 : bi;
+    }
+}
+
+// The same rule for each of gridDim.x rows of [rows][n] logits, one block per row (the body is k_argmax_first's, kept
+// apart so that kernel's code does not change).  Row k's id goes to tok[k], which the next step's embedding reads, and
+// to ids[k].
+__global__ void __launch_bounds__(1024) k_argmax_rows(const float * logits, int n, int32_t * tok, int32_t * ids) {
+    __shared__ float sv[32]; __shared__ int si[32];
+    const int k = blockIdx.x;
+    logits += (size_t) k * n;
+    float bv = -(1000000000000.0f); int bi = 0x7fffffff;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) { const float v = logits[i]; if (v > bv) { bv = v; bi = i; } }
+    auto better = [](float v, int i, float bv, int bi) { return v > bv || (v == bv && i < bi); };
+    for (int o = 16; o > 0; o >>= 1) {
+        const float v = __shfl_xor_sync(0xffffffffu, bv, o); const int i = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (better(v, i, bv, bi)) { bv = v; bi = i; }
+    }
+    if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = bv; si[threadIdx.x >> 5] = bi; }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        bv = threadIdx.x < (blockDim.x >> 5) ? sv[threadIdx.x] : -(1000000000000.0f);
+        bi = threadIdx.x < (blockDim.x >> 5) ? si[threadIdx.x] : 0x7fffffff;
+        for (int o = 16; o > 0; o >>= 1) {
+            const float v = __shfl_xor_sync(0xffffffffu, bv, o); const int i = __shfl_xor_sync(0xffffffffu, bi, o);
+            if (better(v, i, bv, bi)) { bv = v; bi = i; }
+        }
+        if (threadIdx.x == 0) { const int best = bi == 0x7fffffff ? 0 : bi; tok[k] = best; ids[k] = best; }
     }
 }
 
@@ -2120,11 +2166,8 @@ int b200_extra_load(const char * path, int device, b200_extra_t ** out) {
         std::vector<LoadJob> jobs;
         LoadJob je; je.kind = 2; je.nsrc = 1; je.src[0] = &te; je.raw_dst = e->emb_raw; jobs.push_back(je);
         LoadJob jo; jo.nsrc = 1; jo.src[0] = &to;
-        if (to.type == GT_Q6_K) {
-            if ((rc = dev_alloc(s, &e->out_q6k, (size_t) V * (E / 256) * kQ6Packed))) return rc;
-            jo.kind = 3; jo.raw_dst = e->out_q6k;
-        } else if (to.type == GT_F16) { jo.kind = 1; jo.outf = &e->out_f16; }
-        else { jo.kind = 0; jo.mode = 0; jo.G = 1; jo.out = &e->out; }
+        if (to.type == GT_F16) { jo.kind = 1; jo.outf = &e->out_f16; }
+        else { jo.kind = 0; jo.mode = 0; jo.G = 1; jo.out = &e->out; }     // Q6_K: the layers' k-quant packing
         jobs.push_back(jo);
         if ((rc = run_load_jobs(s, f, jobs))) return rc;
     } catch (const std::exception & ex) { return fail(B200_EFILE, "error loading extra layers: %s", ex.what()); }
@@ -2175,25 +2218,31 @@ int b200_extra_embed(b200_extra_t * e, const int32_t * tokens, int n_tokens, flo
     return 0;
 }
 
+// Final RMSNorm + lm_head of n rows of device activations x ([n][n_embd], n <= cap_tokens) into d_logits [n][n_vocab].
+// Every output type groups columns, so output.weight streams once for up to 8 rows.  A Q6_K output.weight is packed like
+// the layers' Q6_K matrices: k_quant_q8k quantises each row once (RMSNorm fused), then k_gemv_kq<Q6_K> runs the dot.
+static int extra_lmhead(b200_extra * e, const float * x, int n) {
+    b200_slice * s = &e->ctx;
+    if (e->out_type == kWT_F16) {
+        GemvF16Args f{}; f.K = e->E; f.x = x; f.ldx = e->E; f.norm_w = e->norm_w; f.N = n;
+        f.rows = e->n_vocab; f.W = e->out_f16; f.y = e->d_logits; f.ldy = e->n_vocab;
+        return launch_f16<PRO_NORM, EPI_STORE>(s, f);
+    }
+    GemvArgs g{}; g.W = e->out; g.x = x; g.ldx = e->E; g.norm_w = e->norm_w; g.y = e->d_logits; g.ldy = e->n_vocab;
+    g.N = n; g.out_rows = e->n_vocab;
+    if (e->out_type == kWT_Q6_K) {
+        if (int rc = quant_kq(s, g, true)) return rc;
+        return launch_gemv_kq<1, PRO_PREQ, EPI_STORE>(s, g);
+    }
+    return launch_gemv<1, PRO_NORM, EPI_STORE>(s, g);
+}
+
 static int extra_logits_device(b200_extra * e, const float * emb, int n_tokens) {
     b200_slice * s = &e->ctx;
     int rc = extra_reserve(e, n_tokens);
     if (rc) return rc;
     B200_CUDA(cudaMemcpyAsync(e->d_x, emb, (size_t) n_tokens * e->E * 4, cudaMemcpyHostToDevice, s->stream));
-    if (e->out_type == kWT_Q6_K) {
-        LmHeadQ6Args q{e->out_q6k, e->n_vocab, e->E, e->d_x, e->E, e->norm_w, e->d_logits, e->n_vocab, n_tokens};
-        const size_t smem = (size_t)(e->E / 256) * (64 * 4 + 4) + (size_t) e->E * 4 + 64;
-        if ((rc = smem_attr<k_lmhead_q6k>(s, 200 * 1024))) return rc;
-        return launch(s, k_lmhead_q6k, dim3((e->n_vocab + 31) / 32, n_tokens, 1), dim3(256, 1, 1), smem, q);
-    }
-    if (e->out_type == kWT_F16) {
-        GemvF16Args f{}; f.K = e->E; f.x = e->d_x; f.ldx = e->E; f.norm_w = e->norm_w; f.N = n_tokens;
-        f.rows = e->n_vocab; f.W = e->out_f16; f.y = e->d_logits; f.ldy = e->n_vocab;
-        return launch_f16<PRO_NORM, EPI_STORE>(s, f);
-    }
-    GemvArgs g{}; g.W = e->out; g.x = e->d_x; g.ldx = e->E; g.norm_w = e->norm_w; g.y = e->d_logits; g.ldy = e->n_vocab;
-    g.N = n_tokens; g.out_rows = e->n_vocab;
-    return launch_gemv<1, PRO_NORM, EPI_STORE>(s, g);
+    return extra_lmhead(e, e->d_x, n_tokens);
 }
 
 int b200_extra_logits(b200_extra_t * e, const float * emb, int n_tokens, int all_logits, float * out) {
@@ -2226,6 +2275,121 @@ int b200_extra_next_token(b200_extra_t * e, const float * emb, int n_tokens, int
     B200_CUDA(cudaMemcpyAsync(token, e->d_best, 4, cudaMemcpyDeviceToHost, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     return 0;
+}
+
+}  // extern "C"
+
+namespace b200 {
+
+// Everything b200_generate_greedy checks before it enqueues anything (the handles' mutexes are held).
+static int generate_check(b200_slice * const * slices, int n_slices, const b200_extra * e, const int * sessions,
+                          const int * counts, int n_seq, const int32_t * tokens, int n_steps) {
+    for (int i = 0; i < n_slices; i++) {
+        const b200_slice * s = slices[i];
+        if (s->E != e->E) return fail(B200_EINVAL, "slice %d has n_embd %d, the extra layers %d", i, s->E, e->E);
+        if (s->device != e->ctx.device)
+            return fail(B200_EINVAL, "slice %d is on device %d, the extra layers on device %d: the loop runs on one GPU", i, s->device, e->ctx.device);
+        if (s->pp_world > 1 || s->nccl_comm) return fail(B200_EINVAL, "slice %d is joined to a pipeline", i);
+        if (i > 0 && s->first_layer != slices[i - 1]->first_layer + slices[i - 1]->L)
+            return fail(B200_EINVAL, "slice %d starts at layer %d, not where slice %d ends (%d)", i, s->first_layer, i - 1,
+                        slices[i - 1]->first_layer + slices[i - 1]->L);
+    }
+    if (n_steps < 1) return fail(B200_EINVAL, "n_steps must be positive (got %d)", n_steps);
+    int total = 0;
+    for (const b200_slice * const * sp = slices; sp < slices + n_slices; sp++)
+        if (int rc = check_pass(*sp, sessions, counts, n_seq, &total)) return rc;
+    for (int i = 0; i < total; i++)
+        if (tokens[i] < 0 || tokens[i] >= e->n_vocab) return fail(B200_EINVAL, "prompt token %d is %d, outside [0, %d)", i, tokens[i], e->n_vocab);
+    for (int i = 0; i < n_slices; i++)
+        for (int k = 0; k < n_seq; k++) {
+            const b200_slice * s = slices[i];
+            if ((long long) s->past[sessions[k]] + counts[k] + n_steps - 1 > s->n_ctx)
+                return fail(B200_ECONTEXT, "context overflow: slice %d session %d n_past %d + %d prompt tokens + %d steps > n_ctx %d",
+                            i, sessions[k], s->past[sessions[k]], counts[k], n_steps - 1, s->n_ctx);
+        }
+    return 0;
+}
+
+// The loop borrows the extra layers' stream for every slice (each slice's own stream is idle when it starts), so the whole
+// sequence of every token is stream-ordered without events; the slices get their streams back when it ends.
+struct StreamLoan {
+    std::vector<b200_slice *> slices; std::vector<cudaStream_t> own; cudaStream_t loop;
+    StreamLoan(b200_slice * const * s, int n, cudaStream_t st) : slices(s, s + n), loop(st) {
+        for (b200_slice * p : slices) { own.push_back(p->stream); p->stream = st; }
+    }
+    ~StreamLoan() {
+        cudaStreamSynchronize(loop);
+        for (size_t i = 0; i < slices.size(); i++) slices[i]->stream = own[i];
+    }
+};
+
+static int generate_locked(b200_slice * const * slices, int n_slices, b200_extra * e, const int * sessions,
+                           const int * counts, int n_seq, const int32_t * tokens, int n_steps, int32_t * ids) {
+    b200_slice * x = &e->ctx;
+    B200_CUDA(cudaSetDevice(x->device));
+    int total = 0;
+    for (int k = 0; k < n_seq; k++) total += counts[k];
+    int rc;
+    if ((rc = extra_reserve(e, total)) || (rc = extra_reserve_ids(e, n_steps * n_seq))) return rc;
+    for (int i = 0; i < n_slices; i++) B200_CUDA(cudaStreamSynchronize(slices[i]->stream));
+    B200_CUDA(cudaMemcpyAsync(e->d_tok, tokens, (size_t) total * 4, cudaMemcpyHostToDevice, x->stream));
+    {
+        StreamLoan loan(slices, n_slices, x->stream);
+        for (int step = 0; step < n_steps; step++) {
+            // step 0: every session's prompt in one mixed pass; later steps: the id each session produced, one batched
+            // step (a single session replays its captured decode graph).  Both are exact mode, as b200_mixed_forward.
+            const int N = step == 0 ? total : n_seq;
+            k_embed_rows<<<dim3((e->E + 255) / 256, N), 256, 0, x->stream>>>(e->emb_raw, e->emb_type, e->E, e->d_tok, e->n_vocab, e->d_x);
+            B200_CUDA(cudaGetLastError());
+            x->launches++;
+            const float * cur = e->d_x;
+            for (int i = 0; i < n_slices; i++) {
+                b200_slice * s = slices[i];
+                if (step == 0)       rc = pass_locked(s, sessions, counts, n_seq, cur, s->d_out, false);
+                else if (n_seq == 1) rc = forward_locked(s, cur, 1, s->d_out, false, sessions[0]);
+                else                 rc = pass_locked(s, sessions, nullptr, n_seq, cur, s->d_out, false);
+                if (rc) return rc;
+                cur = s->d_out;
+            }
+            if (step == 0 && total > n_seq) {        // each session's last prompt row, packed for the lm_head
+                for (int k = 0, end = 0; k < n_seq; k++) {
+                    end += counts[k];
+                    B200_CUDA(cudaMemcpyAsync(e->d_x + (size_t) k * e->E, cur + (size_t)(end - 1) * e->E, (size_t) e->E * 4,
+                                              cudaMemcpyDeviceToDevice, x->stream));
+                }
+                cur = e->d_x;
+            }
+            if ((rc = extra_lmhead(e, cur, n_seq))) return rc;
+            k_argmax_rows<<<n_seq, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, e->d_tok, e->d_ids + (size_t) step * n_seq);
+            B200_CUDA(cudaGetLastError());
+            x->launches++;
+        }
+    }
+    B200_CUDA(cudaMemcpyAsync(ids, e->d_ids, (size_t) n_steps * n_seq * 4, cudaMemcpyDeviceToHost, x->stream));
+    B200_CUDA(cudaStreamSynchronize(x->stream));
+    return 0;
+}
+
+}  // namespace b200
+
+extern "C" {
+
+int b200_generate_greedy(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
+                         const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps, int32_t * ids) {
+    if (!slices || n_slices < 1 || !e || !sessions || !prompt_counts || n_seq < 1 || !prompt_tokens || !ids)
+        return fail(B200_EINVAL, "b200_generate_greedy: null argument or empty list");
+    // every handle's mutex, in address order: two loops that share handles cannot deadlock
+    std::vector<std::mutex *> mus{&e->mu};
+    for (int i = 0; i < n_slices; i++) {
+        if (!slices[i]) return fail(B200_EINVAL, "slice %d is a null handle", i);
+        mus.push_back(&slices[i]->mu);
+    }
+    std::sort(mus.begin(), mus.end());
+    if (std::adjacent_find(mus.begin(), mus.end()) != mus.end()) return fail(B200_EINVAL, "a slice handle is listed twice");
+    std::vector<std::unique_lock<std::mutex>> locks;
+    for (std::mutex * m : mus) locks.emplace_back(*m);
+    if (int rc = generate_check(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps)) return rc;
+    return generate_locked(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps, ids);
 }
 
 int b200_extra_tokenize(b200_extra_t * e, const char * prompt, int32_t * out, int cap) {

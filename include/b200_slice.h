@@ -223,6 +223,25 @@ int b200_extra_embed(b200_extra_t * e, const int32_t * tokens, int n_tokens, flo
 int b200_extra_logits(b200_extra_t * e, const float * emb, int n_tokens, int all_logits, float * out);
 /* llm.get_next_token(path, emb): argmax of the last token's logits (first maximum wins). */
 int b200_extra_next_token(b200_extra_t * e, const float * emb, int n_tokens, int32_t * token);
+/* Greedy generation on the device: the client's loop (cli_api/common.py:94-111 with get_next_token,
+ * tensor_processor.cpp:1894-1908) for n_seq sessions of a model whose slices all live on one GPU.
+ * Step 0 feeds each session its prompt (one mixed pass), every later step feeds each session the id it
+ * produced (one batched step); after each step the extra layers' norm + lm_head + argmax pick the next id.
+ * ids: [n_steps][n_seq].  Session k's ids equal a single-session run, which equals the host loop
+ * (b200_extra_embed -> b200_session_forward on each slice -> b200_extra_next_token) with fast prefill off.
+ *   - slices: in layer order, each starting where the one before ends; prompt_tokens: sum of prompt_counts ids, grouped
+ *     by session in list order.  Each session continues from its current position; afterwards its n_past is
+ *     old + prompt_counts[k] + n_steps - 1 on every slice.
+ *   - The host enqueues the whole loop and synchronises once.  Every step runs in exact mode (fast prefill never applies).
+ *   - Every handle's mutex is held for the call, taken in address order.
+ *   - All-or-nothing: on an error no position moves and no cache is written.
+ *     B200_EINVAL: a null argument, slices not contiguous in layer order, a slice of another n_embd than the extra layers,
+ *     handles on different devices, a handle listed twice or joined to a pipeline, a session out of range or listed
+ *     twice, a prompt count < 1, a token id outside [0, n_vocab), n_steps < 1;
+ *     B200_ECONTEXT: n_past + prompt_counts[k] + n_steps - 1 > n_ctx on some slice. */
+int b200_generate_greedy(b200_slice_t * const * slices, int n_slices, b200_extra_t * e,
+                         const int * sessions, const int * prompt_counts, int n_seq,
+                         const int32_t * prompt_tokens, int n_steps, int32_t * ids);
 /* llm.tokenize_prompt(path, prompt): BOS + sentencepiece-style merge (tensor_processor.cpp:1596-1714).
  * Returns the token count (may exceed cap; only cap are written) or a negative error. */
 int b200_extra_tokenize(b200_extra_t * e, const char * prompt, int32_t * out, int cap);
