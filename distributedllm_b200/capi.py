@@ -26,6 +26,12 @@ class SliceInfo(C.Structure):
                                                                         ("kv_bytes_per_pos", C.c_int64)]
 
 
+class Sampling(C.Structure):
+    """b200_sampling_t."""
+    _fields_ = [("temperature", C.c_double), ("repeat_penalty", C.c_double), ("seeds", C.c_void_p),
+                ("first_draw", C.c_int64), ("history", C.c_void_p), ("history_counts", C.c_void_p)]
+
+
 _lib: Optional[C.CDLL] = None
 
 
@@ -90,7 +96,9 @@ def lib() -> C.CDLL:
                            ("b200_extra_embed", [vp, vp, ci, vp]), ("b200_extra_logits", [vp, vp, ci, ci, vp]),
                            ("b200_extra_next_token", [vp, vp, ci, C.POINTER(C.c_int32)]),
                            ("b200_extra_tokenize", [vp, C.c_char_p, vp, ci]),
-                           ("b200_generate_greedy", [vp, ci, vp, vp, vp, ci, vp, ci, vp])):
+                           ("b200_generate_greedy", [vp, ci, vp, vp, vp, ci, vp, ci, vp]),
+                           ("b200_generate_sample", [vp, ci, vp, vp, vp, ci, vp, ci, vp, vp]),
+                           ("b200_extra_sample", [vp, vp, ci, vp, vp])):
             if hasattr(L, name):
                 getattr(L, name).argtypes = args
         if hasattr(L, "b200_extra_token_text"):
@@ -322,6 +330,24 @@ class Extra:
         check(lib().b200_extra_next_token(self._h, _ptr(x), x.shape[0], C.byref(tok)))
         return tok.value
 
+    def token_text(self, token_id: int) -> str:
+        """llm.decode_token: the token's text (invalid UTF-8 replaced)."""
+        n = C.c_int()
+        p = lib().b200_extra_token_text(self._h, int(token_id), C.byref(n))
+        if not p:
+            raise IndexError("token id %d out of range" % token_id)
+        return C.string_at(p, n.value).decode("utf-8", "replace")
+
+    def sample(self, logits: np.ndarray, temperature: float, repeat_penalty: float, seeds, first_draw: int = 0,
+               history=None) -> np.ndarray:
+        """The client's Sampler on the device (b200_extra_sample): row k of [n][n_vocab] logits takes draw first_draw of
+        the Philox stream keyed seeds[k], with history[k] (ids already sampled) penalised.  -> [n] ids."""
+        x = np.ascontiguousarray(logits, dtype=np.float32).reshape(-1, self.n_vocab)
+        sp, keep = _sampling(len(x), temperature, repeat_penalty, seeds, first_draw, history)
+        out = np.zeros(len(x), np.int32)
+        check(lib().b200_extra_sample(self._h, _ptr(x), len(x), C.byref(sp), _ptr(out)))
+        return out
+
     def close(self) -> None:
         if self._h:
             check(lib().b200_extra_unload(self._h))
@@ -347,4 +373,40 @@ def generate_greedy(slices, extra: Extra, sessions, prompts, n_steps: int) -> np
     out = np.zeros((max(n_steps, 0), len(ids)), np.int32)
     check(lib().b200_generate_greedy(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks),
                                      n_steps, _ptr(out)))
+    return out
+
+
+def _sampling(n: int, temperature: float, repeat_penalty: float, seeds, first_draw: int, history):
+    """-> (b200_sampling_t, the arrays it points into)."""
+    keys = np.ascontiguousarray([int(k) for k in seeds], dtype=np.uint64)
+    if len(keys) != n:
+        raise ValueError("need one seed per session (%d), got %d" % (n, len(keys)))
+    sp = Sampling(float(temperature), float(repeat_penalty), keys.ctypes.data, int(first_draw), None, None)
+    keep = [keys]
+    if history is not None:
+        if len(history) != n:
+            raise ValueError("need one history per session (%d), got %d" % (n, len(history)))
+        counts = np.array([len(h) for h in history], np.int32)
+        ids = np.ascontiguousarray([int(t) for h in history for t in h] or [0], dtype=np.int32)
+        sp.history, sp.history_counts = ids.ctypes.data, counts.ctypes.data
+        keep += [counts, ids]
+    return sp, keep
+
+
+def generate_sample(slices, extra: Extra, sessions, prompts, n_steps: int, temperature: float, repeat_penalty: float,
+                    seeds, first_draw: int = 0, history=None) -> np.ndarray:
+    """Sampled generation on the device (b200_generate_sample): generate_greedy's loop with the client's Sampler in place
+    of the argmax.  Session sessions[k] draws from numpy.random.Philox(key=seeds[k]) starting at draw first_draw, with
+    history[k] (ids it sampled before) penalised.  -> [n_steps][n_seq] ids."""
+    ids = np.ascontiguousarray(sessions, dtype=np.int32)
+    if len(prompts) != len(ids):
+        raise ValueError("need one prompt per listed session")
+    sp, keep = _sampling(len(ids), temperature, repeat_penalty, seeds, first_draw, history)
+    counts = np.array([len(p) for p in prompts], np.int32)
+    toks = np.ascontiguousarray(np.concatenate([np.asarray(p, np.int64) for p in prompts]) if len(prompts) else [],
+                                dtype=np.int32)
+    handles = (C.c_void_p * max(len(slices), 1))(*[s.handle for s in slices])
+    out = np.zeros((max(n_steps, 0), len(ids)), np.int32)
+    check(lib().b200_generate_sample(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks),
+                                     n_steps, C.byref(sp), _ptr(out)))
     return out

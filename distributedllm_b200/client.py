@@ -85,11 +85,13 @@ class DistributedLLM:
         self.wire = wire
         self.llm = import_llm()
 
-    def generate(self, prompt, max_steps=200, temperature=0.0, repeat_penalty=1.1):
+    def generate(self, prompt, max_steps=200, temperature=0.0, repeat_penalty=1.1, rng=None):
+        """rng: the Sampler's random generator (default numpy's global one, as the reference);
+        numpy.random.Generator(numpy.random.Philox(key=seed)) gives LocalPipeline.generate's ids for that seed."""
         self.clear_context()
         extra = self.extra_layers_path
         tokens = self.llm.tokenize_prompt(extra, prompt)
-        sampler = Sampler(temperature, repeat_penalty)
+        sampler = Sampler(temperature, repeat_penalty, rng=rng)
         for _ in range(max_steps):
             emb = self.propagate_tensor(self.llm.prepare_embeddings(extra, tokens))
             token_id = sampler(self.llm.get_logits(extra, emb, False))
@@ -151,23 +153,45 @@ class LocalPipeline:
         self.slices.sort(key=lambda s: s.info.first_layer)
         self._extra = None
 
-    def generate_greedy(self, extra_path: str, prompt: str, max_steps: int = 200) -> List[int]:
-        """DistributedLLM.generate_greedy on this box: clear the contexts, tokenize, then max_steps argmax steps, all on
-        the GPU with no host round trip between tokens (capi.generate_greedy).  Needs every slice on one device."""
+    def _device_extra(self, extra_path: str, what: str):
+        """The extra layers on the slices' one GPU, loaded once per path."""
         devices = sorted({s.info.device for s in self.slices})
         if len(devices) != 1:
-            raise self.capi.B200Error(1, "greedy generation on the device needs every slice on one GPU; the slices are on "
-                                         "devices %s" % ", ".join(map(str, devices)))
+            raise self.capi.B200Error(1, "%s generation on the device needs every slice on one GPU; the slices are on "
+                                         "devices %s" % (what, ", ".join(map(str, devices))))
         if self._extra is None or self._extra[0] != extra_path:
             if self._extra is not None:
                 self._extra[1].close()
             self._extra = (extra_path, self.capi.Extra(extra_path, devices[0]))
-        extra = self._extra[1]
+        return self._extra[1]
+
+    def generate_greedy(self, extra_path: str, prompt: str, max_steps: int = 200) -> List[int]:
+        """DistributedLLM.generate_greedy on this box: clear the contexts, tokenize, then max_steps argmax steps, all on
+        the GPU with no host round trip between tokens (capi.generate_greedy).  Needs every slice on one device."""
+        extra = self._device_extra(extra_path, "greedy")
         self.clear_context()
         tokens = extra.tokenize(prompt)
         if max_steps < 1:
             return []
         return self.capi.generate_greedy(self.slices, extra, [0], [tokens], max_steps)[:, 0].tolist()
+
+    def generate(self, extra_path: str, prompt: str, max_steps: int = 200, temperature: float = 0.0,
+                 repeat_penalty: float = 1.1, seed: int = None):
+        """DistributedLLM.generate on this box: clear the contexts, tokenize, then max_steps steps of the client's Sampler,
+        all on the GPU with no host round trip between tokens (capi.generate_sample); yields the token strings.  The
+        draws come from numpy.random.Philox(key=seed), so DistributedLLM.generate(..., rng=numpy.random.Generator(
+        numpy.random.Philox(key=seed))) yields the same strings.  seed=None draws a key from numpy's global generator,
+        so unseeded runs vary as the reference's do.  Needs every slice on one device."""
+        extra = self._device_extra(extra_path, "sampled")
+        if seed is None:
+            seed = int(np.random.randint(0, 2 ** 64, dtype=np.uint64))
+        self.clear_context()
+        tokens = extra.tokenize(prompt)
+        if max_steps < 1:
+            return
+        ids = self.capi.generate_sample(self.slices, extra, [0], [tokens], max_steps, temperature, repeat_penalty, [seed])
+        for token_id in ids[:, 0].tolist():
+            yield extra.token_text(token_id)
 
     def propagate_tensor(self, embeddings) -> np.ndarray:
         x = np.ascontiguousarray(embeddings, dtype=np.float32)

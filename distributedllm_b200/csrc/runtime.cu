@@ -12,6 +12,7 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <climits>
 #include <cmath>
 #include <condition_variable>
 #include <dlfcn.h>
@@ -1934,6 +1935,8 @@ struct b200_extra {
     PackedW out{}; uint16_t * out_f16 = nullptr;
     float * d_x = nullptr, * d_logits = nullptr; int32_t * d_tok = nullptr, * d_best = nullptr; int cap_tokens = 0;
     int32_t * d_ids = nullptr; int cap_ids = 0;    // b200_generate_greedy: [n_steps][n_seq] ids
+    // sampling (k_sample_rows): per-row penalty bitmaps [rows][(n_vocab + 31) / 32], Philox keys, the first bad row
+    uint32_t * d_pen = nullptr; uint64_t * d_seeds = nullptr; int * d_bad = nullptr; int cap_sample = 0;
     std::vector<std::pair<std::string, float>> vocab;
     std::unordered_map<std::string, int> token_to_id;
     std::mutex mu;
@@ -2016,6 +2019,23 @@ static int extra_reserve_ids(b200_extra * e, int n) {
     return 0;
 }
 
+static int extra_reserve_sample(b200_extra * e, int rows) {
+    if (rows <= e->cap_sample) return 0;
+    b200_slice * s = &e->ctx;
+    cudaStreamSynchronize(s->stream);
+    for (void * old : {(void *) e->d_pen, (void *) e->d_seeds, (void *) e->d_bad}) {
+        if (!old) continue;
+        s->allocs.erase(std::remove(s->allocs.begin(), s->allocs.end(), old), s->allocs.end());
+        cudaFree(old);
+    }
+    e->d_pen = nullptr; e->d_seeds = nullptr; e->d_bad = nullptr; e->cap_sample = 0;
+    int rc;
+    if ((rc = dev_alloc(s, &e->d_pen, (size_t) rows * ((e->n_vocab + 31) / 32))) || (rc = dev_alloc(s, &e->d_seeds, (size_t) rows)) ||
+        (rc = dev_alloc(s, &e->d_bad, (size_t) 1))) return rc;
+    e->cap_sample = rows;
+    return 0;
+}
+
 // sample_next_token (tensor_processor.cpp:1894-1908): best = -1e12, id = 0; `if (logit > best)` in index order, i.e. the
 // FIRST maximum wins, NaNs never win, and a row that never exceeds -1e12 yields id 0.  One block over the row.
 __global__ void __launch_bounds__(1024) k_argmax_first(const float * logits, int n, int32_t * out) {
@@ -2064,6 +2084,129 @@ __global__ void __launch_bounds__(1024) k_argmax_rows(const float * logits, int 
             if (better(v, i, bv, bi)) { bv = v; bi = i; }
         }
         if (threadIdx.x == 0) { const int best = bi == 0x7fffffff ? 0 : bi; tok[k] = best; ids[k] = best; }
+    }
+}
+
+// Word d (0-based) of numpy.random.Philox(key=seed): word d % 4 of Philox4x64-10 on counter (d / 4 + 1, 0, 0, 0) and
+// key (seed, 0) -- numpy increments the counter before its first block.
+__device__ __forceinline__ uint64_t philox_word(uint64_t seed, long long d) {
+    uint64_t c0 = (uint64_t)(d >> 2) + 1, c1 = 0, c2 = 0, c3 = 0, k0 = seed, k1 = 0;
+    for (int r = 0; r < 10; r++) {
+        if (r) { k0 += 0x9E3779B97F4A7C15ull; k1 += 0xBB67AE8584CAA73Bull; }
+        const uint64_t hi0 = __umul64hi(0xD2E7470EE14C6C93ull, c0), lo0 = 0xD2E7470EE14C6C93ull * c0;
+        const uint64_t hi1 = __umul64hi(0xCA5A826395121157ull, c2), lo1 = 0xCA5A826395121157ull * c2;
+        c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+    }
+    const int w = (int)(d & 3);
+    return w == 0 ? c0 : w == 1 ? c1 : w == 2 ? c2 : c3;
+}
+
+// Exclusive prefix sum over a warp in index order: lane l adds lanes 0 .. l-1 one at a time, so lane l + 1's result is
+// lane l's result + v, bit for bit, and the prefixes never decrease.
+__device__ __forceinline__ double warp_prefix_ordered(double v) {
+    const int lane = threadIdx.x & 31;
+    double p = 0.0;
+    for (int j = 0; j < 31; j++) { const double w = __shfl_sync(0xffffffffu, v, j); if (j < lane) p = __dadd_rn(p, w); }
+    return p;
+}
+
+// k_sample_rows: row k of [rows][n] logits is session k of the call.
+struct SampleArgs {
+    const float * logits; int n;
+    double dt, dp;                   // the divisors: T + 1e-5, and rp * (T + 1e-5) for an id in prev
+    const uint64_t * seeds; long long draw;   // row k takes draw `draw` of stream seeds[k]
+    uint32_t * pen;                  // [rows][(n + 31) / 32]: bit i of row k = id i is in session k's prev
+    int32_t * tok, * ids;            // the chosen id -> tok[k] (the next step's embedding reads it) and ids[k]
+    int * bad; int bad_base;         // a row without a distribution: id -1, atomicMin(bad, bad_base + k)
+};
+
+__device__ __forceinline__ double sample_weight(const SampleArgs & a, const float * x, const uint32_t * bits, int i, double m) {
+    const double d = (bits[i >> 5] >> (i & 31)) & 1u ? a.dp : a.dt;
+    return exp(__dsub_rn(__ddiv_rn((double) x[i], d), m));
+}
+
+// The client's Sampler (cli_api/common.py:64-86) on each of gridDim.x rows, one block per row.  Thread t owns the
+// contiguous chunk [t*C, t*C + C) of the row.
+//   1. max y: the divisor takes two values and a correctly rounded division is monotone, so max y is the larger of
+//      (max x over ids outside prev) / dt and (max x over ids in prev) / dp.  A NaN, or a max that is not finite, is a
+//      row numpy rejects.
+//   2. e_i = exp(y_i - max y) in float64; each thread sums its chunk in order; the chunk offsets O_t are an ordered scan
+//      (warp_prefix_ordered within and across warps), so they never decrease and O_t + total_t is O_{t+1} exactly.
+//   3. The thread whose [O_t, O_{t+1}) holds u*S (S the total; the last chunk with weight when u*S rounds to S) claims
+//      the draw; warp 0 re-walks that chunk in order from O_t and picks the first id whose running sum passes u*S,
+//      falling back to the chunk's last id of positive weight.  An id of weight 0 never moves the sum, so it is never
+//      picked.  The row's logits are read from L2 in each pass.
+__global__ void __launch_bounds__(1024) k_sample_rows(SampleArgs a) {
+    __shared__ float smf[32], smp[32];
+    __shared__ double swt[32], swo[32], s_m, s_u, s_total, s_target, s_o;
+    __shared__ int s_chunk;
+    const int k = blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5, nwarp = blockDim.x >> 5;
+    const float * x = a.logits + (size_t) k * a.n;
+    uint32_t * bits = a.pen + (size_t) k * ((a.n + 31) >> 5);
+    const int C = (a.n + blockDim.x - 1) / blockDim.x, i0 = min(a.n, t * C), i1 = min(a.n, i0 + C);
+    float mf = -INFINITY, mp = -INFINITY; bool nan = false;
+    for (int i = i0; i < i1; i++) {
+        const float v = x[i];
+        nan |= v != v;
+        if ((bits[i >> 5] >> (i & 31)) & 1u) mp = fmaxf(mp, v); else mf = fmaxf(mf, v);
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        mf = fmaxf(mf, __shfl_xor_sync(0xffffffffu, mf, o)); mp = fmaxf(mp, __shfl_xor_sync(0xffffffffu, mp, o));
+    }
+    if (lane == 0) { smf[wid] = mf; smp[wid] = mp; }
+    if (t == 0) s_chunk = 0x7fffffff;
+    const bool any_nan = __syncthreads_or(nan);
+    if (wid == 0) {
+        mf = lane < nwarp ? smf[lane] : -INFINITY; mp = lane < nwarp ? smp[lane] : -INFINITY;
+        for (int o = 16; o > 0; o >>= 1) {
+            mf = fmaxf(mf, __shfl_xor_sync(0xffffffffu, mf, o)); mp = fmaxf(mp, __shfl_xor_sync(0xffffffffu, mp, o));
+        }
+        if (lane == 0) {
+            s_m = fmax(__ddiv_rn((double) mf, a.dt), __ddiv_rn((double) mp, a.dp));
+            s_u = (double)(philox_word(a.seeds[k], a.draw) >> 11) * 0x1.0p-53;
+        }
+    }
+    __syncthreads();
+    const double m = s_m;
+    if (any_nan || !isfinite(m)) {
+        if (t == 0) { a.tok[k] = -1; a.ids[k] = -1; atomicMin(a.bad, a.bad_base + k); }
+        return;
+    }
+    double tot = 0.0;
+    for (int i = i0; i < i1; i++) tot = __dadd_rn(tot, sample_weight(a, x, bits, i, m));
+    const double P = warp_prefix_ordered(tot), Pin = __dadd_rn(P, tot);
+    if (lane == 31) swt[wid] = Pin;
+    __syncthreads();
+    if (wid == 0) {
+        const double v = lane < nwarp ? swt[lane] : 0.0, W = warp_prefix_ordered(v);
+        swo[lane] = W;
+        if (lane == 31) { const double S = __dadd_rn(W, v); s_target = __dmul_rn(s_u, S); s_total = S; }
+    }
+    __syncthreads();
+    const double S = s_total, target = s_target;
+    const double O = __dadd_rn(swo[wid], P), Oend = __dadd_rn(swo[wid], Pin);
+    if (tot > 0.0 && O <= target && (target < Oend || Oend == S)) atomicMin(&s_chunk, t);
+    __syncthreads();
+    if (t == s_chunk) s_o = O;
+    __syncthreads();
+    if (wid != 0) return;
+    const int j0 = min(a.n, s_chunk * C), j1 = min(a.n, j0 + C);
+    double r = s_o; int id = -1, last = -1;
+    for (int b = j0; b < j1 && id < 0; b += 32) {
+        const int i = b + lane;
+        const double e = i < j1 ? sample_weight(a, x, bits, i, m) : 0.0;
+        double q = r;                                  // r + e_b + ... + e_i, added in index order
+        for (int j = 0; j < 32; j++) { const double w = __shfl_sync(0xffffffffu, e, j); if (j <= lane) q = __dadd_rn(q, w); }
+        const unsigned hit = __ballot_sync(0xffffffffu, i < j1 && q > target);
+        const unsigned pos = __ballot_sync(0xffffffffu, i < j1 && e > 0.0);
+        if (hit) id = b + __ffs(hit) - 1;
+        if (pos) last = b + 31 - __clz(pos);
+        r = __shfl_sync(0xffffffffu, q, 31);
+    }
+    if (lane == 0) {
+        if (id < 0) id = last;
+        a.tok[k] = id; a.ids[k] = id;
+        bits[id >> 5] |= 1u << (id & 31);
     }
 }
 
@@ -2323,8 +2466,70 @@ struct StreamLoan {
     }
 };
 
+// Everything a sampling call checks about its settings before it enqueues anything.
+static int sample_check(const b200_sampling_t * sp, int n_seq, int n_vocab) {
+    if (!sp || !sp->seeds) return fail(B200_EINVAL, "null sampling settings or seeds");
+    if (!(sp->temperature >= 0) || !std::isfinite(sp->temperature))
+        return fail(B200_EINVAL, "temperature must be finite and >= 0 (got %g)", sp->temperature);
+    if (!(sp->repeat_penalty > 0) || !std::isfinite(sp->repeat_penalty))
+        return fail(B200_EINVAL, "repeat penalty must be finite and > 0 (got %g)", sp->repeat_penalty);
+    if (sp->first_draw < 0) return fail(B200_EINVAL, "first_draw must be >= 0 (got %lld)", (long long) sp->first_draw);
+    if (!sp->history) return 0;
+    if (!sp->history_counts) return fail(B200_EINVAL, "a history needs history_counts");
+    for (int k = 0, at = 0; k < n_seq; k++) {
+        if (sp->history_counts[k] < 0) return fail(B200_EINVAL, "history count %d is %d", k, sp->history_counts[k]);
+        for (int j = 0; j < sp->history_counts[k]; j++, at++)
+            if (sp->history[at] < 0 || sp->history[at] >= n_vocab)
+                return fail(B200_EINVAL, "history id %d of session %d is %d, outside [0, %d)", j, k, sp->history[at], n_vocab);
+    }
+    return 0;
+}
+
+// Uploads the keys and each row's penalty bitmap (cleared, then the bits of its history) and resets the bad-row word.
+static int sample_start(b200_extra * e, const b200_sampling_t * sp, int n_seq) {
+    if (int rc = extra_reserve_sample(e, n_seq)) return rc;
+    const int nw = (e->n_vocab + 31) / 32;
+    std::vector<uint32_t> pen((size_t) n_seq * nw, 0u);
+    if (sp->history)
+        for (int k = 0, at = 0; k < n_seq; k++)
+            for (int j = 0; j < sp->history_counts[k]; j++, at++)
+                pen[(size_t) k * nw + (sp->history[at] >> 5)] |= 1u << (sp->history[at] & 31);
+    const int none = INT_MAX;
+    cudaStream_t st = e->ctx.stream;
+    B200_CUDA(cudaMemcpyAsync(e->d_pen, pen.data(), pen.size() * 4, cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaMemcpyAsync(e->d_seeds, sp->seeds, (size_t) n_seq * 8, cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaMemcpyAsync(e->d_bad, &none, 4, cudaMemcpyHostToDevice, st));
+    return 0;
+}
+
+// k_sample_rows on the first `rows` rows of d_logits with draw first_draw + step; a bad row k is recorded as
+// step * rows + k.
+static int sample_launch(b200_extra * e, const b200_sampling_t * sp, int rows, int step, int32_t * ids) {
+    const double dt = sp->temperature + 1e-5;
+    SampleArgs a{e->d_logits, e->n_vocab, dt, sp->repeat_penalty * dt, e->d_seeds, (long long) sp->first_draw + step,
+                 e->d_pen, e->d_tok, ids, e->d_bad, step * rows};
+    k_sample_rows<<<rows, 1024, 0, e->ctx.stream>>>(a);
+    B200_CUDA(cudaGetLastError());
+    e->ctx.launches++;
+    return 0;
+}
+
+// After the call's synchronise: B200_EINVAL naming the first row that had no distribution.
+static int sample_finish(b200_extra * e, int rows, const int * sessions) {
+    int bad = INT_MAX;
+    B200_CUDA(cudaMemcpy(&bad, e->d_bad, 4, cudaMemcpyDeviceToHost));
+    if (bad == INT_MAX) return 0;
+    const int step = bad / rows, k = bad % rows;
+    if (sessions)
+        return fail(B200_EINVAL, "step %d session %d: the logits hold a NaN or +inf, are all -inf or overflow float64 once "
+                    "scaled, so they have no distribution (its id is -1; positions have moved)", step, sessions[k]);
+    return fail(B200_EINVAL, "row %d: the logits are all -inf or overflow float64 once scaled, so they have no distribution", k);
+}
+
+// The loop of b200_generate_greedy (sp == NULL: argmax, k_argmax_rows) and b200_generate_sample (k_sample_rows).
 static int generate_locked(b200_slice * const * slices, int n_slices, b200_extra * e, const int * sessions,
-                           const int * counts, int n_seq, const int32_t * tokens, int n_steps, int32_t * ids) {
+                           const int * counts, int n_seq, const int32_t * tokens, int n_steps, const b200_sampling_t * sp,
+                           int32_t * ids) {
     b200_slice * x = &e->ctx;
     B200_CUDA(cudaSetDevice(x->device));
     int total = 0;
@@ -2332,6 +2537,7 @@ static int generate_locked(b200_slice * const * slices, int n_slices, b200_extra
     int rc;
     if ((rc = extra_reserve(e, total)) || (rc = extra_reserve_ids(e, n_steps * n_seq))) return rc;
     for (int i = 0; i < n_slices; i++) B200_CUDA(cudaStreamSynchronize(slices[i]->stream));
+    if (sp && (rc = sample_start(e, sp, n_seq))) return rc;
     B200_CUDA(cudaMemcpyAsync(e->d_tok, tokens, (size_t) total * 4, cudaMemcpyHostToDevice, x->stream));
     {
         StreamLoan loan(slices, n_slices, x->stream);
@@ -2360,6 +2566,10 @@ static int generate_locked(b200_slice * const * slices, int n_slices, b200_extra
                 cur = e->d_x;
             }
             if ((rc = extra_lmhead(e, cur, n_seq))) return rc;
+            if (sp) {
+                if ((rc = sample_launch(e, sp, n_seq, step, e->d_ids + (size_t) step * n_seq))) return rc;
+                continue;
+            }
             k_argmax_rows<<<n_seq, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, e->d_tok, e->d_ids + (size_t) step * n_seq);
             B200_CUDA(cudaGetLastError());
             x->launches++;
@@ -2367,17 +2577,23 @@ static int generate_locked(b200_slice * const * slices, int n_slices, b200_extra
     }
     B200_CUDA(cudaMemcpyAsync(ids, e->d_ids, (size_t) n_steps * n_seq * 4, cudaMemcpyDeviceToHost, x->stream));
     B200_CUDA(cudaStreamSynchronize(x->stream));
-    return 0;
+    return sp ? sample_finish(e, n_seq, sessions) : 0;
 }
 
 }  // namespace b200
 
 extern "C" {
 
-int b200_generate_greedy(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
-                         const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps, int32_t * ids) {
+}  // extern "C"
+
+namespace b200 {
+
+// Both generation entries: the checks, every handle's mutex, then the loop (greedy when not sampled).
+static int generate(bool sampled, b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
+                    const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps,
+                    const b200_sampling_t * sp, int32_t * ids) {
     if (!slices || n_slices < 1 || !e || !sessions || !prompt_counts || n_seq < 1 || !prompt_tokens || !ids)
-        return fail(B200_EINVAL, "b200_generate_greedy: null argument or empty list");
+        return fail(B200_EINVAL, "%s: null argument or empty list", sampled ? "b200_generate_sample" : "b200_generate_greedy");
     // every handle's mutex, in address order: two loops that share handles cannot deadlock
     std::vector<std::mutex *> mus{&e->mu};
     for (int i = 0; i < n_slices; i++) {
@@ -2389,7 +2605,45 @@ int b200_generate_greedy(b200_slice_t * const * slices, int n_slices, b200_extra
     std::vector<std::unique_lock<std::mutex>> locks;
     for (std::mutex * m : mus) locks.emplace_back(*m);
     if (int rc = generate_check(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps)) return rc;
-    return generate_locked(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps, ids);
+    if (sampled)
+        if (int rc = sample_check(sp, n_seq, e->n_vocab)) return rc;
+    return generate_locked(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps, sp, ids);
+}
+
+}  // namespace b200
+
+extern "C" {
+
+int b200_generate_greedy(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
+                         const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps, int32_t * ids) {
+    return generate(false, slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps,
+                    nullptr, ids);
+}
+
+int b200_generate_sample(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
+                         const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps,
+                         const b200_sampling_t * sp, int32_t * ids) {
+    return generate(true, slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps,
+                    sp, ids);
+}
+
+int b200_extra_sample(b200_extra_t * e, const float * logits, int n_rows, const b200_sampling_t * sp, int32_t * ids) {
+    if (!e || !logits || n_rows < 1 || !ids) return fail(B200_EINVAL, "b200_extra_sample: null argument or no rows");
+    std::lock_guard<std::mutex> lk(e->mu);
+    if (int rc = sample_check(sp, n_rows, e->n_vocab)) return rc;
+    const size_t V = (size_t) e->n_vocab;
+    for (size_t i = 0; i < (size_t) n_rows * V; i++)
+        if (std::isnan(logits[i]) || logits[i] == INFINITY)
+            return fail(B200_EINVAL, "row %d has a non-finite logit at id %d (%g)", (int)(i / V), (int)(i % V), (double) logits[i]);
+    b200_slice * s = &e->ctx;
+    B200_CUDA(cudaSetDevice(s->device));
+    int rc;
+    if ((rc = extra_reserve(e, n_rows)) || (rc = extra_reserve_ids(e, n_rows)) || (rc = sample_start(e, sp, n_rows))) return rc;
+    B200_CUDA(cudaMemcpyAsync(e->d_logits, logits, (size_t) n_rows * V * 4, cudaMemcpyHostToDevice, s->stream));
+    if ((rc = sample_launch(e, sp, n_rows, 0, e->d_ids))) return rc;
+    B200_CUDA(cudaMemcpyAsync(ids, e->d_ids, (size_t) n_rows * 4, cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    return sample_finish(e, n_rows, nullptr);
 }
 
 int b200_extra_tokenize(b200_extra_t * e, const char * prompt, int32_t * out, int cap) {

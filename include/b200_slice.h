@@ -242,6 +242,37 @@ int b200_extra_next_token(b200_extra_t * e, const float * emb, int n_tokens, int
 int b200_generate_greedy(b200_slice_t * const * slices, int n_slices, b200_extra_t * e,
                          const int * sessions, const int * prompt_counts, int n_seq,
                          const int32_t * prompt_tokens, int n_steps, int32_t * ids);
+/* Sampling settings of the client's Sampler (cli_api/common.py:64-86) for n_seq sessions or rows. */
+typedef struct b200_sampling {
+    double temperature;          /* >= 0, finite */
+    double repeat_penalty;       /* > 0, finite */
+    const uint64_t * seeds;      /* [n_seq]: Philox4x64-10 key (seeds[k], 0) = numpy.random.Philox(key=seeds[k]) */
+    int64_t first_draw;          /* draws each stream has already given (0 = fresh generator) */
+    const int32_t * history;     /* NULL, or ids already sampled, grouped by session: history_counts[k] for session k */
+    const int * history_counts;
+} b200_sampling_t;
+/* Sampled generation on the device: b200_generate_greedy's loop with the client's Sampler in place of the argmax.
+ * For each row of logits x, with prev = the session's history plus the ids this call has drawn for it so far:
+ *   y_i = x_i / d_i in float64, d_i = repeat_penalty * (T + 1e-5) if i is in prev, else T + 1e-5;
+ *   p = softmax(y); the id is the first i with cumsum(p)[i] > u, u = draw (first_draw + step) of session k's
+ *   Philox4x64-10 stream as Generator.random() makes it: (word >> 11) * 2^-53.
+ * So client.Sampler(T, rp, rng=numpy.random.Generator(numpy.random.Philox(key=seeds[k]))) is the host twin, draw for
+ * draw; ids can differ from it only where u lies within ~1e-12 of a CDF boundary (the last ulp of exp and the summation
+ * order).  On the device there is no such freedom: a session's ids are the same alone, in a batch, or split across calls
+ * (a call with the earlier ids as history, first_draw = their count and the last id as prompt continues another).
+ * An id whose probability is exactly 0 is never chosen.  Everything else, including the error codes, is as
+ * b200_generate_greedy; B200_EINVAL also covers a null sp or seeds, temperature < 0 or not finite, repeat_penalty <= 0
+ * or not finite, first_draw < 0, history without history_counts, a history count < 0 and a history id outside
+ * [0, n_vocab), and those leave every position unchanged.
+ * A row whose logits hold a NaN or +inf, are all -inf, or scale past the float64 range has no distribution (numpy
+ * raises "probabilities contain NaN"): its id is -1, the rest of the loop still runs, and the call returns B200_EINVAL
+ * naming the first such step and session.  The positions HAVE moved by then, as after a successful call. */
+int b200_generate_sample(b200_slice_t * const * slices, int n_slices, b200_extra_t * e,
+                         const int * sessions, const int * prompt_counts, int n_seq,
+                         const int32_t * prompt_tokens, int n_steps, const b200_sampling_t * sp, int32_t * ids);
+/* The sampling rule alone on host logits [n_rows][n_vocab]: row k is session k (seeds[k], history of row k) and takes
+ * draw first_draw of its stream.  A non-finite logit (NaN or +inf) is B200_EINVAL before anything runs. */
+int b200_extra_sample(b200_extra_t * e, const float * logits, int n_rows, const b200_sampling_t * sp, int32_t * ids);
 /* llm.tokenize_prompt(path, prompt): BOS + sentencepiece-style merge (tensor_processor.cpp:1596-1714).
  * Returns the token count (may exceed cap; only cap are written) or a negative error. */
 int b200_extra_tokenize(b200_extra_t * e, const char * prompt, int32_t * out, int cap);
