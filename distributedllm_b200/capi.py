@@ -98,7 +98,8 @@ def lib() -> C.CDLL:
                            ("b200_extra_tokenize", [vp, C.c_char_p, vp, ci]),
                            ("b200_generate_greedy", [vp, ci, vp, vp, vp, ci, vp, ci, vp]),
                            ("b200_generate_sample", [vp, ci, vp, vp, vp, ci, vp, ci, vp, vp]),
-                           ("b200_extra_sample", [vp, vp, ci, vp, vp])):
+                           ("b200_extra_sample", [vp, vp, ci, vp, vp]),
+                           ("b200_score", [vp, ci, vp, vp, vp, ci, vp, vp]), ("b200_extra_nll", [vp, vp, ci, vp, vp])):
             if hasattr(L, name):
                 getattr(L, name).argtypes = args
         if hasattr(L, "b200_extra_token_text"):
@@ -348,6 +349,17 @@ class Extra:
         check(lib().b200_extra_sample(self._h, _ptr(x), len(x), C.byref(sp), _ptr(out)))
         return out
 
+    def nll(self, logits: np.ndarray, targets) -> np.ndarray:
+        """The client's perplexity term on the device (b200_extra_nll): -log softmax(row k)[targets[k]] in float64 for
+        each row of [n][n_vocab] logits.  -> [n] float64."""
+        x = np.ascontiguousarray(logits, dtype=np.float32).reshape(-1, self.n_vocab)
+        t = np.ascontiguousarray(targets, dtype=np.int32)
+        if len(t) != len(x):
+            raise ValueError("need one target per row (%d), got %d" % (len(x), len(t)))
+        out = np.zeros(len(x), np.float64)
+        check(lib().b200_extra_nll(self._h, _ptr(x), len(x), _ptr(t), _ptr(out)))
+        return out
+
     def close(self) -> None:
         if self._h:
             check(lib().b200_extra_unload(self._h))
@@ -410,3 +422,20 @@ def generate_sample(slices, extra: Extra, sessions, prompts, n_steps: int, tempe
     check(lib().b200_generate_sample(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks),
                                      n_steps, C.byref(sp), _ptr(out)))
     return out
+
+
+def score(slices, extra: Extra, sessions, token_lists) -> list:
+    """Scoring on the device (b200_score): session sessions[k] is fed token_lists[k][:-1] from its current position, and
+    its entry of the result holds -log p(token_lists[k][j + 1] | everything before) for every j, in float64.  `slices`
+    are in layer order, all on the extra layers' GPU.  -> one array of len(token_lists[k]) - 1 values per session."""
+    ids = np.ascontiguousarray(sessions, dtype=np.int32)
+    if len(token_lists) != len(ids):
+        raise ValueError("need one token list per listed session")
+    counts = np.array([len(t) for t in token_lists], np.int32)
+    toks = np.ascontiguousarray(np.concatenate([np.asarray(t, np.int64) for t in token_lists]) if len(token_lists) else [],
+                                dtype=np.int32)
+    handles = (C.c_void_p * max(len(slices), 1))(*[s.handle for s in slices])
+    fed = np.maximum(counts.astype(np.int64) - 1, 0)
+    out = np.zeros(max(int(fed.sum()), 1), np.float64)
+    check(lib().b200_score(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks), _ptr(out)))
+    return np.split(out[:int(fed.sum())], np.cumsum(fed)[:-1])

@@ -157,7 +157,7 @@ class LocalPipeline:
         """The extra layers on the slices' one GPU, loaded once per path."""
         devices = sorted({s.info.device for s in self.slices})
         if len(devices) != 1:
-            raise self.capi.B200Error(1, "%s generation on the device needs every slice on one GPU; the slices are on "
+            raise self.capi.B200Error(1, "%s on the device needs every slice on one GPU; the slices are on "
                                          "devices %s" % (what, ", ".join(map(str, devices))))
         if self._extra is None or self._extra[0] != extra_path:
             if self._extra is not None:
@@ -168,7 +168,7 @@ class LocalPipeline:
     def generate_greedy(self, extra_path: str, prompt: str, max_steps: int = 200) -> List[int]:
         """DistributedLLM.generate_greedy on this box: clear the contexts, tokenize, then max_steps argmax steps, all on
         the GPU with no host round trip between tokens (capi.generate_greedy).  Needs every slice on one device."""
-        extra = self._device_extra(extra_path, "greedy")
+        extra = self._device_extra(extra_path, "greedy generation")
         self.clear_context()
         tokens = extra.tokenize(prompt)
         if max_steps < 1:
@@ -182,7 +182,7 @@ class LocalPipeline:
         draws come from numpy.random.Philox(key=seed), so DistributedLLM.generate(..., rng=numpy.random.Generator(
         numpy.random.Philox(key=seed))) yields the same strings.  seed=None draws a key from numpy's global generator,
         so unseeded runs vary as the reference's do.  Needs every slice on one device."""
-        extra = self._device_extra(extra_path, "sampled")
+        extra = self._device_extra(extra_path, "sampled generation")
         if seed is None:
             seed = int(np.random.randint(0, 2 ** 64, dtype=np.uint64))
         self.clear_context()
@@ -192,6 +192,20 @@ class LocalPipeline:
         ids = self.capi.generate_sample(self.slices, extra, [0], [tokens], max_steps, temperature, repeat_penalty, [seed])
         for token_id in ids[:, 0].tolist():
             yield extra.token_text(token_id)
+
+    def perplexity(self, extra_path: str, text: str) -> float:
+        """DistributedLLM.perplexity on this box: clear the contexts, tokenize, then score the text on the GPU
+        (capi.score: one pass, lm_head and softmax on the device, only the per-token NLLs come back).  The NLLs are
+        summed in the reference's order (one `nll -= log p` per token, cli_api/common.py:136-139).  Needs every slice
+        on one device."""
+        extra = self._device_extra(extra_path, "scoring")
+        self.clear_context()
+        tokens = extra.tokenize(text)
+        n = len(tokens) - 1
+        nll = 0.0
+        for v in self.capi.score(self.slices, extra, [0], [tokens])[0]:
+            nll += v
+        return float(np.exp(nll / n))
 
     def propagate_tensor(self, embeddings) -> np.ndarray:
         x = np.ascontiguousarray(embeddings, dtype=np.float32)

@@ -1934,9 +1934,11 @@ struct b200_extra {
     float * norm_w = nullptr;
     PackedW out{}; uint16_t * out_f16 = nullptr;
     float * d_x = nullptr, * d_logits = nullptr; int32_t * d_tok = nullptr, * d_best = nullptr; int cap_tokens = 0;
-    int32_t * d_ids = nullptr; int cap_ids = 0;    // b200_generate_greedy: [n_steps][n_seq] ids
+    int32_t * d_ids = nullptr; int cap_ids = 0;    // generation: [n_steps][n_seq] ids; scoring: fed ids, then targets
     // sampling (k_sample_rows): per-row penalty bitmaps [rows][(n_vocab + 31) / 32], Philox keys, the first bad row
     uint32_t * d_pen = nullptr; uint64_t * d_seeds = nullptr; int * d_bad = nullptr; int cap_sample = 0;
+    // scoring (b200_score): the embedded rows of one pass [rows][n_embd], and the NLL of every scored row
+    float * d_sx = nullptr; int cap_sx = 0; double * d_nll = nullptr; int cap_nll = 0;
     std::vector<std::pair<std::string, float>> vocab;
     std::unordered_map<std::string, int> token_to_id;
     std::mutex mu;
@@ -2033,6 +2035,21 @@ static int extra_reserve_sample(b200_extra * e, int rows) {
     if ((rc = dev_alloc(s, &e->d_pen, (size_t) rows * ((e->n_vocab + 31) / 32))) || (rc = dev_alloc(s, &e->d_seeds, (size_t) rows)) ||
         (rc = dev_alloc(s, &e->d_bad, (size_t) 1))) return rc;
     e->cap_sample = rows;
+    return 0;
+}
+
+// Grows one of the extra layers' scratch buffers to n elements of T (its contents are not kept).
+template <typename T> static int extra_regrow(b200_extra * e, T *& p, int & cap, size_t per, int n) {
+    if (n <= cap) return 0;
+    b200_slice * s = &e->ctx;
+    cudaStreamSynchronize(s->stream);
+    if (p) {
+        s->allocs.erase(std::remove(s->allocs.begin(), s->allocs.end(), (void *) p), s->allocs.end());
+        cudaFree(p);
+    }
+    p = nullptr; cap = 0;
+    if (int rc = dev_alloc(s, &p, (size_t) n * per)) return rc;
+    cap = n;
     return 0;
 }
 
@@ -2207,6 +2224,44 @@ __global__ void __launch_bounds__(1024) k_sample_rows(SampleArgs a) {
         if (id < 0) id = last;
         a.tok[k] = id; a.ids[k] = id;
         bits[id >> 5] |= 1u << (id & 31);
+    }
+}
+
+// The client's perplexity term (cli_api/common.py:129-139) for each of gridDim.x rows of [rows][n] logits, one block per
+// row: nll[k] = -log(e_t / S) with t = tgt[k], e_i = exp((double) x_i - m), m = max x and S = sum e_i, all in float64.
+// Thread t sums its contiguous chunk [t*C, t*C + C) in order and the chunk totals combine in index order
+// (warp_prefix_ordered within and across warps, as in k_sample_rows), so a row's value depends only on its logits and its
+// target.  Non-finite rows follow numpy: a NaN or +inf logit, or a row that is all -inf, gives NaN; a target whose e_t
+// underflows gives +inf.
+__global__ void __launch_bounds__(1024) k_nll_rows(const float * logits, int n, const int32_t * tgt, double * nll) {
+    __shared__ float smx[32];
+    __shared__ double swt[32];
+    const int k = blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5, nwarp = blockDim.x >> 5;
+    const float * x = logits + (size_t) k * n;
+    const int C = (n + blockDim.x - 1) / blockDim.x, i0 = min(n, t * C), i1 = min(n, i0 + C);
+    float mx = -INFINITY; bool bad = false;
+    for (int i = i0; i < i1; i++) { const float v = x[i]; bad |= v != v || v == INFINITY; mx = fmaxf(mx, v); }
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (lane == 0) smx[wid] = mx;
+    const bool any_bad = __syncthreads_or(bad);
+    mx = lane < nwarp ? smx[lane] : -INFINITY;          // every warp reduces the warp maxima: m is block-uniform
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (any_bad || mx == -INFINITY) {
+        if (t == 0) nll[k] = __longlong_as_double(0x7ff8000000000000ll);
+        return;
+    }
+    const double m = (double) mx;
+    double tot = 0.0;
+#pragma unroll 1                                         // unrolled, the float64 exp spills at 32 registers (2 CTAs / SM)
+    for (int i = i0; i < i1; i++) tot = __dadd_rn(tot, exp(__dsub_rn((double) x[i], m)));
+    const double P = warp_prefix_ordered(tot);
+    if (lane == 31) swt[wid] = __dadd_rn(P, tot);
+    __syncthreads();
+    if (wid != 0) return;
+    const double v = lane < nwarp ? swt[lane] : 0.0, W = warp_prefix_ordered(v);
+    if (lane == 31) {
+        const double S = __dadd_rn(W, v), et = exp(__dsub_rn((double) x[tgt[k]], m));
+        nll[k] = -log(__ddiv_rn(et, S));
     }
 }
 
@@ -2424,9 +2479,9 @@ int b200_extra_next_token(b200_extra_t * e, const float * emb, int n_tokens, int
 
 namespace b200 {
 
-// Everything b200_generate_greedy checks before it enqueues anything (the handles' mutexes are held).
-static int generate_check(b200_slice * const * slices, int n_slices, const b200_extra * e, const int * sessions,
-                          const int * counts, int n_seq, const int32_t * tokens, int n_steps) {
+// Every device loop's handles: the slices follow each other in layer order on the extra layers' GPU, with its n_embd,
+// outside any pipeline.
+static int chain_check(b200_slice * const * slices, int n_slices, const b200_extra * e) {
     for (int i = 0; i < n_slices; i++) {
         const b200_slice * s = slices[i];
         if (s->E != e->E) return fail(B200_EINVAL, "slice %d has n_embd %d, the extra layers %d", i, s->E, e->E);
@@ -2437,12 +2492,24 @@ static int generate_check(b200_slice * const * slices, int n_slices, const b200_
             return fail(B200_EINVAL, "slice %d starts at layer %d, not where slice %d ends (%d)", i, s->first_layer, i - 1,
                         slices[i - 1]->first_layer + slices[i - 1]->L);
     }
+    return 0;
+}
+
+static int check_tokens(const int32_t * tokens, int n, int n_vocab, const char * what) {
+    for (int i = 0; i < n; i++)
+        if (tokens[i] < 0 || tokens[i] >= n_vocab) return fail(B200_EINVAL, "%s %d is %d, outside [0, %d)", what, i, tokens[i], n_vocab);
+    return 0;
+}
+
+// Everything b200_generate_greedy checks before it enqueues anything (the handles' mutexes are held).
+static int generate_check(b200_slice * const * slices, int n_slices, const b200_extra * e, const int * sessions,
+                          const int * counts, int n_seq, const int32_t * tokens, int n_steps) {
+    if (int rc = chain_check(slices, n_slices, e)) return rc;
     if (n_steps < 1) return fail(B200_EINVAL, "n_steps must be positive (got %d)", n_steps);
     int total = 0;
     for (const b200_slice * const * sp = slices; sp < slices + n_slices; sp++)
         if (int rc = check_pass(*sp, sessions, counts, n_seq, &total)) return rc;
-    for (int i = 0; i < total; i++)
-        if (tokens[i] < 0 || tokens[i] >= e->n_vocab) return fail(B200_EINVAL, "prompt token %d is %d, outside [0, %d)", i, tokens[i], e->n_vocab);
+    if (int rc = check_tokens(tokens, total, e->n_vocab, "prompt token")) return rc;
     for (int i = 0; i < n_slices; i++)
         for (int k = 0; k < n_seq; k++) {
             const b200_slice * s = slices[i];
@@ -2588,13 +2655,9 @@ extern "C" {
 
 namespace b200 {
 
-// Both generation entries: the checks, every handle's mutex, then the loop (greedy when not sampled).
-static int generate(bool sampled, b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
-                    const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps,
-                    const b200_sampling_t * sp, int32_t * ids) {
-    if (!slices || n_slices < 1 || !e || !sessions || !prompt_counts || n_seq < 1 || !prompt_tokens || !ids)
-        return fail(B200_EINVAL, "%s: null argument or empty list", sampled ? "b200_generate_sample" : "b200_generate_greedy");
-    // every handle's mutex, in address order: two loops that share handles cannot deadlock
+// Every handle's mutex of a device loop, in address order, so that two loops that share handles cannot deadlock.
+static int lock_handles(b200_slice_t * const * slices, int n_slices, b200_extra_t * e,
+                        std::vector<std::unique_lock<std::mutex>> & locks) {
     std::vector<std::mutex *> mus{&e->mu};
     for (int i = 0; i < n_slices; i++) {
         if (!slices[i]) return fail(B200_EINVAL, "slice %d is a null handle", i);
@@ -2602,12 +2665,121 @@ static int generate(bool sampled, b200_slice_t * const * slices, int n_slices, b
     }
     std::sort(mus.begin(), mus.end());
     if (std::adjacent_find(mus.begin(), mus.end()) != mus.end()) return fail(B200_EINVAL, "a slice handle is listed twice");
-    std::vector<std::unique_lock<std::mutex>> locks;
     for (std::mutex * m : mus) locks.emplace_back(*m);
+    return 0;
+}
+
+// Both generation entries: the checks, every handle's mutex, then the loop (greedy when not sampled).
+static int generate(bool sampled, b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
+                    const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps,
+                    const b200_sampling_t * sp, int32_t * ids) {
+    if (!slices || n_slices < 1 || !e || !sessions || !prompt_counts || n_seq < 1 || !prompt_tokens || !ids)
+        return fail(B200_EINVAL, "%s: null argument or empty list", sampled ? "b200_generate_sample" : "b200_generate_greedy");
+    std::vector<std::unique_lock<std::mutex>> locks;
+    if (int rc = lock_handles(slices, n_slices, e, locks)) return rc;
     if (int rc = generate_check(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps)) return rc;
     if (sampled)
         if (int rc = sample_check(sp, n_seq, e->n_vocab)) return rc;
     return generate_locked(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps, sp, ids);
+}
+
+// Rows the scoring loop's lm_head and k_nll_rows take at a time: its logits scratch is kScoreRows x n_vocab floats
+// (8 MB at 32000 ids) however long the texts are.  Rows of the lm_head are independent, so the blocks change no bit.
+static constexpr int kScoreRows = 64;
+
+// b200_score's passes: the sessions, whole and in list order, packed into passes of at most n_ctx fed rows (the smallest
+// n_ctx of the slices).  A session's rows are never split across passes: a mixed pass's rows depend on their segment's
+// row length, so only one segment per session gives the rows of a single call over the whole text.
+// -> the list index of each pass's first session, then n_seq.
+static std::vector<int> score_passes(b200_slice * const * slices, int n_slices, const int * fed, int n_seq) {
+    int cap = INT_MAX;
+    for (int i = 0; i < n_slices; i++) cap = std::min(cap, slices[i]->n_ctx);
+    std::vector<int> starts{0};
+    for (int k = 0, rows = 0; k < n_seq; k++) {
+        if (rows > 0 && rows + fed[k] > cap) { starts.push_back(k); rows = 0; }
+        rows += fed[k];
+    }
+    starts.push_back(n_seq);
+    return starts;
+}
+
+// Everything b200_score checks before it enqueues anything (the handles' mutexes are held); fills fed and the passes.
+static int score_check(b200_slice * const * slices, int n_slices, const b200_extra * e, const int * sessions,
+                       const int * counts, int n_seq, const int32_t * tokens, std::vector<int> & fed,
+                       std::vector<int> & starts) {
+    if (int rc = chain_check(slices, n_slices, e)) return rc;
+    long long total = 0;
+    for (int k = 0; k < n_seq; k++) {
+        if (counts[k] < 2) return fail(B200_EINVAL, "session %d: scoring needs at least 2 tokens (got %d)", sessions[k], counts[k]);
+        fed.push_back(counts[k] - 1);
+        total += counts[k];
+    }
+    starts = score_passes(slices, n_slices, fed.data(), n_seq);
+    for (int i = 0; i < n_slices; i++)
+        for (size_t p = 0; p + 1 < starts.size(); p++) {
+            int rows = 0;
+            if (int rc = check_pass(slices[i], sessions + starts[p], fed.data() + starts[p], starts[p + 1] - starts[p], &rows))
+                return rc;
+        }
+    std::vector<char> seen(slices[0]->n_sessions, 0);   // every session is in range on every slice by now
+    for (int k = 0; k < n_seq; k++) {
+        if (seen[sessions[k]]) return fail(B200_EINVAL, "session %d listed twice", sessions[k]);
+        seen[sessions[k]] = 1;
+    }
+    return check_tokens(tokens, (int) total, e->n_vocab, "token");
+}
+
+// Each pass: embed its fed rows, run them through every slice (one segment per session, exact mode), then the lm_head and
+// k_nll_rows over the last slice's output in blocks of kScoreRows rows.  The ids go up once, the NLLs come back once.
+static int score_locked(b200_slice * const * slices, int n_slices, b200_extra * e, const int * sessions, const int * counts,
+                        const std::vector<int> & fed, const std::vector<int> & starts, const int32_t * tokens, double * nll) {
+    b200_slice * x = &e->ctx;
+    B200_CUDA(cudaSetDevice(x->device));
+    const int n_seq = starts.back();
+    std::vector<int> pass_rows;
+    int R = 0;
+    for (size_t p = 0; p + 1 < starts.size(); p++) {
+        int rows = 0;
+        for (int k = starts[p]; k < starts[p + 1]; k++) rows += fed[k];
+        pass_rows.push_back(rows);
+        R += rows;
+    }
+    std::vector<int32_t> ids((size_t) 2 * R);            // the fed ids, then the targets, each grouped by session
+    for (int k = 0, at = 0, r = 0; k < n_seq; at += counts[k], k++)
+        for (int j = 0; j < fed[k]; j++, r++) { ids[r] = tokens[at + j]; ids[R + r] = tokens[at + j + 1]; }
+    int rc;
+    if ((rc = extra_reserve(e, kScoreRows)) || (rc = extra_reserve_ids(e, 2 * R)) ||
+        (rc = extra_regrow(e, e->d_sx, e->cap_sx, (size_t) e->E, *std::max_element(pass_rows.begin(), pass_rows.end()))) ||
+        (rc = extra_regrow(e, e->d_nll, e->cap_nll, 1, R)))
+        return rc;
+    for (int i = 0; i < n_slices; i++) B200_CUDA(cudaStreamSynchronize(slices[i]->stream));
+    B200_CUDA(cudaMemcpyAsync(e->d_ids, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice, x->stream));
+    {
+        StreamLoan loan(slices, n_slices, x->stream);
+        for (size_t p = 0, row0 = 0; p + 1 < starts.size(); row0 += pass_rows[p], p++) {
+            const int a = starts[p], N = pass_rows[p];
+            k_embed_rows<<<dim3((e->E + 255) / 256, N), 256, 0, x->stream>>>(e->emb_raw, e->emb_type, e->E, e->d_ids + row0,
+                                                                               e->n_vocab, e->d_sx);
+            B200_CUDA(cudaGetLastError());
+            x->launches++;
+            const float * cur = e->d_sx;
+            for (int i = 0; i < n_slices; i++) {
+                b200_slice * s = slices[i];
+                if ((rc = pass_locked(s, sessions + a, fed.data() + a, starts[p + 1] - a, cur, s->d_out, false))) return rc;
+                cur = s->d_out;
+            }
+            for (int b = 0; b < N; b += kScoreRows) {
+                const int nb = std::min(kScoreRows, N - b);
+                if ((rc = extra_lmhead(e, cur + (size_t) b * e->E, nb))) return rc;
+                k_nll_rows<<<nb, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, e->d_ids + R + row0 + b, e->d_nll + row0 + b);
+                B200_CUDA(cudaGetLastError());
+                x->launches++;
+            }
+        }
+    }
+    B200_CUDA(cudaMemcpyAsync(nll, e->d_nll, (size_t) R * 8, cudaMemcpyDeviceToHost, x->stream));
+    B200_CUDA(cudaStreamSynchronize(x->stream));
+    return 0;
 }
 
 }  // namespace b200
@@ -2644,6 +2816,36 @@ int b200_extra_sample(b200_extra_t * e, const float * logits, int n_rows, const 
     B200_CUDA(cudaMemcpyAsync(ids, e->d_ids, (size_t) n_rows * 4, cudaMemcpyDeviceToHost, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     return sample_finish(e, n_rows, nullptr);
+}
+
+int b200_score(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions, const int * counts,
+               int n_seq, const int32_t * tokens, double * nll) {
+    if (!slices || n_slices < 1 || !e || !sessions || !counts || n_seq < 1 || !tokens || !nll)
+        return fail(B200_EINVAL, "b200_score: null argument or empty list");
+    std::vector<std::unique_lock<std::mutex>> locks;
+    if (int rc = lock_handles(slices, n_slices, e, locks)) return rc;
+    std::vector<int> fed, starts;
+    if (int rc = score_check(slices, n_slices, e, sessions, counts, n_seq, tokens, fed, starts)) return rc;
+    return score_locked(slices, n_slices, e, sessions, counts, fed, starts, tokens, nll);
+}
+
+int b200_extra_nll(b200_extra_t * e, const float * logits, int n_rows, const int32_t * targets, double * nll) {
+    if (!e || !logits || n_rows < 1 || !targets || !nll) return fail(B200_EINVAL, "b200_extra_nll: null argument or no rows");
+    std::lock_guard<std::mutex> lk(e->mu);
+    if (int rc = check_tokens(targets, n_rows, e->n_vocab, "target")) return rc;
+    b200_slice * s = &e->ctx;
+    B200_CUDA(cudaSetDevice(s->device));
+    int rc;
+    if ((rc = extra_reserve(e, n_rows)) || (rc = extra_reserve_ids(e, n_rows)) || (rc = extra_regrow(e, e->d_nll, e->cap_nll, 1, n_rows)))
+        return rc;
+    B200_CUDA(cudaMemcpyAsync(e->d_logits, logits, (size_t) n_rows * e->n_vocab * 4, cudaMemcpyHostToDevice, s->stream));
+    B200_CUDA(cudaMemcpyAsync(e->d_ids, targets, (size_t) n_rows * 4, cudaMemcpyHostToDevice, s->stream));
+    k_nll_rows<<<n_rows, 1024, 0, s->stream>>>(e->d_logits, e->n_vocab, e->d_ids, e->d_nll);
+    B200_CUDA(cudaGetLastError());
+    s->launches++;
+    B200_CUDA(cudaMemcpyAsync(nll, e->d_nll, (size_t) n_rows * 8, cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    return 0;
 }
 
 int b200_extra_tokenize(b200_extra_t * e, const char * prompt, int32_t * out, int cap) {

@@ -273,6 +273,24 @@ int b200_generate_sample(b200_slice_t * const * slices, int n_slices, b200_extra
 /* The sampling rule alone on host logits [n_rows][n_vocab]: row k is session k (seeds[k], history of row k) and takes
  * draw first_draw of its stream.  A non-finite logit (NaN or +inf) is B200_EINVAL before anything runs. */
 int b200_extra_sample(b200_extra_t * e, const float * logits, int n_rows, const b200_sampling_t * sp, int32_t * ids);
+/* Scores sessions[k]'s tokens (counts[k] >= 2 ids, grouped by session in list order): feeds tokens 0..counts[k]-2 at the
+ * session's own positions, and writes nll[j] = -log p(token j+1 | context, tokens 0..j) in float64, grouped by session
+ * (sum of counts[k]-1 values).  Afterwards each session's n_past is old + counts[k] - 1 on every slice.
+ *   - p is the client's perplexity arithmetic (cli_api/common.py:129-139): softmax of the row's logits in float64,
+ *     m = max x, e_i = exp(x_i - m), S = sum e_i in a fixed order, nll = -log(e_t / S).  A row holding a NaN or +inf
+ *     logit, or all -inf, gives NaN; a target whose e_t underflows gives +inf (the call still succeeds).
+ *   - Each session's fed tokens run as one segment of one mixed pass in exact mode; sessions are packed whole, in list
+ *     order, into passes of at most n_ctx rows.  So each session's logits equal one b200_session_forward of its fed
+ *     tokens (fast prefill off) whatever else the call holds, and its NLLs are bit-identical alone, in a batch, or
+ *     packed differently.
+ *   - The host uploads the ids once, synchronises once, and reads back only nll.
+ *   - Locking, slice checks and all-or-nothing errors are as b200_generate_greedy: B200_EINVAL for what it refuses
+ *     (except n_steps), a count < 2 or a null nll; B200_ECONTEXT for n_past + counts[k] - 1 > n_ctx on some slice. */
+int b200_score(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
+               const int * counts, int n_seq, const int32_t * tokens, double * nll);
+/* k_nll_rows on host logits [n_rows][n_vocab]: the kernel's test door, as b200_extra_sample is k_sample_rows'.
+ * nll[k] as b200_score computes it for row k and target targets[k]; a target outside [0, n_vocab) is B200_EINVAL. */
+int b200_extra_nll(b200_extra_t * e, const float * logits, int n_rows, const int32_t * targets, double * nll);
 /* llm.tokenize_prompt(path, prompt): BOS + sentencepiece-style merge (tensor_processor.cpp:1596-1714).
  * Returns the token count (may exceed cap; only cap are written) or a negative error. */
 int b200_extra_tokenize(b200_extra_t * e, const char * prompt, int32_t * out, int cap);
