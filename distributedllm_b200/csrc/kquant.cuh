@@ -102,10 +102,12 @@ __device__ __forceinline__ void warp_quant_q8k(const float * xs, const float * n
         #pragma unroll
         for (int j = 0; j < 8; j++) v[j] = fmul(fmul(v[j], scale), wv[j]);
     }
-    // the FIRST element of the largest magnitude (`if (ax > amax)` in index order): key = (|v| bits, reversed index)
+    // the FIRST element of the largest magnitude (`if (ax > amax)` in index order): key = (|v| bits, reversed index).
+    // A NaN never passes `ax > amax`, so it is never the maximum, and a block of NaNs and zeros is a zero block (an
+    // attention row whose scores are all NaN, from K cached as fp16 inf, reaches wo that way).
     uint32_t babs = 0; float best = 0.f; int bj = 0;
     #pragma unroll
-    for (int j = 0; j < 8; j++) { const uint32_t u = __float_as_uint(fabsf(v[j])); if (u > babs) { babs = u; best = v[j]; bj = j; } }
+    for (int j = 0; j < 8; j++) { const uint32_t u = __float_as_uint(fabsf(v[j])); if (u > babs && u <= 0x7F800000u) { babs = u; best = v[j]; bj = j; } }
     unsigned long long key = babs ? ((unsigned long long) babs << 32) | (unsigned)(255 - (lane * 8 + bj)) : 0ull;
     #pragma unroll
     for (int o = 16; o > 0; o >>= 1) { const unsigned long long k2 = __shfl_xor_sync(0xffffffffu, key, o); key = k2 > key ? k2 : key; }
@@ -123,7 +125,8 @@ __device__ __forceinline__ void warp_quant_q8k(const float * xs, const float * n
     #pragma unroll
     for (int j = 0; j < 8; j++) {
         const float val = fadd(fmul(iscale, v[j]), 12582912.f);                       // nearest_int (k_quants.c:50-55)
-        const int q = min(127, (int)((__float_as_uint(val) & 0x007fffffu) - 0x00400000));
+        // nearest_int of a NaN reads the mantissa of x86's default NaN (0x400000): 0.  The GPU's NaN has mantissa 0x7FFFFF.
+        const int q = val != val ? 0 : min(127, (int)((__float_as_uint(val) & 0x007fffffu) - 0x00400000));
         sum += q;
         pk[j >> 2] |= ((uint32_t)(q & 0xFF)) << (8 * (j & 3));
     }
