@@ -99,7 +99,11 @@ def lib() -> C.CDLL:
                            ("b200_generate_greedy", [vp, ci, vp, vp, vp, ci, vp, ci, vp]),
                            ("b200_generate_sample", [vp, ci, vp, vp, vp, ci, vp, ci, vp, vp]),
                            ("b200_extra_sample", [vp, vp, ci, vp, vp]),
-                           ("b200_score", [vp, ci, vp, vp, vp, ci, vp, vp]), ("b200_extra_nll", [vp, vp, ci, vp, vp])):
+                           ("b200_score", [vp, ci, vp, vp, vp, ci, vp, vp]), ("b200_extra_nll", [vp, vp, ci, vp, vp]),
+                           ("b200_stream_open", [vp, ci, vp, ci, ci, C.POINTER(vp)]),
+                           ("b200_stream_add", [vp, ci, vp, ci, ci, vp, vp, ci]),
+                           ("b200_stream_read", [vp, vp, vp, ci, C.POINTER(ci)]),
+                           ("b200_stream_cancel", [vp, ci]), ("b200_stream_close", [vp])):
             if hasattr(L, name):
                 getattr(L, name).argtypes = args
         if hasattr(L, "b200_extra_token_text"):
@@ -439,3 +443,113 @@ def score(slices, extra: Extra, sessions, token_lists) -> list:
     out = np.zeros(max(int(fed.sum()), 1), np.float64)
     check(lib().b200_score(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks), _ptr(out)))
     return np.split(out[:int(fed.sum())], np.cumsum(fed)[:-1])
+
+
+def _int(name: str, v, lo: int, hi: int) -> int:
+    """v as a Python int in [lo, hi], or ValueError / TypeError naming the argument."""
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+        raise TypeError("%s must be an integer, got %r" % (name, v))
+    v = int(v)
+    if not lo <= v <= hi:
+        raise ValueError("%s must be in [%d, %d], got %d" % (name, lo, hi, v))
+    return v
+
+
+def _ids(name: str, seq, n_vocab: int, min_len: int) -> np.ndarray:
+    """A list of token ids as int32, each in [0, n_vocab)."""
+    if isinstance(seq, (str, bytes)) or not hasattr(seq, "__len__"):
+        raise TypeError("%s must be a sequence of token ids" % name)
+    out = np.array([_int("%s[%d]" % (name, i), t, 0, n_vocab - 1) for i, t in enumerate(seq)] or [0], np.int32)
+    if len(seq) < min_len:
+        raise ValueError("%s needs at least %d id(s)" % (name, min_len))
+    return out
+
+
+class Stream:
+    """A generation stream (b200_stream_*) over slices in layer order on the extra layers' GPU.  add() queues a session
+    with its prompt and budget; read() returns (session, id) pairs as the device draws them; a session leaves at its
+    budget, at a stop id (delivered), on cancel() or at close().  Each session's ids equal generate_greedy /
+    generate_sample for it alone.  While the stream is open its handles belong to it.  A context manager (close on exit)
+    and an iterator of (session, id) pairs, read one at a time, that ends when no session is left."""
+
+    def __init__(self, slices, extra: Extra, max_rows: int = 0, lookahead: int = 0):
+        self._h = None
+        slices = list(slices)
+        if not slices:
+            raise ValueError("a stream needs at least one slice")
+        max_rows = _int("max_rows", max_rows, -2 ** 31, 2 ** 31 - 1)
+        lookahead = _int("lookahead", lookahead, -2 ** 31, 2 ** 31 - 1)
+        self.n_vocab = extra.n_vocab
+        handles = (C.c_void_p * len(slices))(*[s.handle for s in slices])
+        h = C.c_void_p()
+        check(lib().b200_stream_open(handles, len(slices), extra.handle, max_rows, lookahead, C.byref(h)))
+        self._h = h
+
+    def _handle(self) -> C.c_void_p:
+        if not self._h:
+            raise ValueError("the stream is closed")
+        return self._h
+
+    def add(self, session: int, prompt, max_tokens: int, temperature: Optional[float] = None, repeat_penalty: float = 1.1,
+            seed: int = 0, first_draw: int = 0, history=None, stop_ids=()) -> None:
+        """Queue `session` with `prompt` (token ids) for at most max_tokens ids.  temperature None: greedy (the argmax of
+        the raw logits); else the client's Sampler with repeat_penalty on numpy.random.Philox(key=seed), starting at draw
+        first_draw, with history (ids sampled before) penalised.  The session ends after the first id in stop_ids."""
+        session = _int("session", session, 0, 2 ** 31 - 1)
+        p = _ids("prompt", prompt, self.n_vocab, 1)
+        max_tokens = _int("max_tokens", max_tokens, 1, 2 ** 31 - 1)
+        stops = _ids("stop_ids", stop_ids, self.n_vocab, 0)
+        sp, keep = None, None
+        if temperature is not None:
+            t, rp = float(temperature), float(repeat_penalty)
+            if not (np.isfinite(t) and t >= 0):
+                raise ValueError("temperature must be finite and >= 0, got %r" % temperature)
+            if not (np.isfinite(rp) and rp > 0):
+                raise ValueError("repeat_penalty must be finite and > 0, got %r" % repeat_penalty)
+            seed = _int("seed", seed, 0, 2 ** 64 - 1)
+            first_draw = _int("first_draw", first_draw, 0, 2 ** 63 - 1)
+            if history is not None:
+                history = [_ids("history", history, self.n_vocab, 0)[:len(history)].tolist()]
+            sp, keep = _sampling(1, t, rp, [seed], first_draw, history)
+        elif history is not None or first_draw:
+            raise ValueError("history and first_draw apply to sampled sessions (give a temperature)")
+        check(lib().b200_stream_add(self._handle(), session, _ptr(p), len(prompt), max_tokens,
+                                    None if sp is None else C.byref(sp), _ptr(stops), len(stop_ids)))
+
+    def read(self, cap: int = 64) -> list:
+        """Up to cap (session, id) pairs in the order they were drawn; blocks until there is at least one.  [] only when
+        no session is active or queued.  An id of -1 ends its session: its logits had no distribution."""
+        cap = _int("cap", cap, 1, 2 ** 20)
+        h = self._handle()
+        sess, ids, n = np.zeros(cap, np.int32), np.zeros(cap, np.int32), C.c_int()
+        check(lib().b200_stream_read(h, _ptr(sess), _ptr(ids), cap, C.byref(n)))
+        return list(zip(sess[:n.value].tolist(), ids[:n.value].tolist()))
+
+    def cancel(self, session: int) -> None:
+        """End a queued or active session now: its positions reflect the ids read so far."""
+        session = _int("session", session, 0, 2 ** 31 - 1)
+        check(lib().b200_stream_cancel(self._handle(), session))
+
+    def close(self) -> None:
+        if self._h:
+            h, self._h = self._h, None
+            check(lib().b200_stream_close(h))
+
+    def __enter__(self) -> "Stream":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()
+
+    def __iter__(self):
+        while True:
+            pairs = self.read(1)
+            if not pairs:
+                return
+            yield pairs[0]
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

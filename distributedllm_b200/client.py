@@ -141,6 +141,10 @@ class DistributedLLM:
         return x.tolist()
 
 
+# llama_token_eos(): the end-of-sequence id of the LLaMA vocabulary (LocalPipeline.generate(stop_at_eos=True))
+EOS_ID = 2
+
+
 class LocalPipeline:
     """All slices of a nodes_map on the GPUs of THIS box: slice i on device i, activations chained device to
     device (peer copy) -- the single-process equivalent of the NCCL pipeline bench.py runs with one rank per GPU."""
@@ -176,12 +180,15 @@ class LocalPipeline:
         return self.capi.generate_greedy(self.slices, extra, [0], [tokens], max_steps)[:, 0].tolist()
 
     def generate(self, extra_path: str, prompt: str, max_steps: int = 200, temperature: float = 0.0,
-                 repeat_penalty: float = 1.1, seed: int = None):
-        """DistributedLLM.generate on this box: clear the contexts, tokenize, then max_steps steps of the client's Sampler,
-        all on the GPU with no host round trip between tokens (capi.generate_sample); yields the token strings.  The
-        draws come from numpy.random.Philox(key=seed), so DistributedLLM.generate(..., rng=numpy.random.Generator(
-        numpy.random.Philox(key=seed))) yields the same strings.  seed=None draws a key from numpy's global generator,
-        so unseeded runs vary as the reference's do.  Needs every slice on one device."""
+                 repeat_penalty: float = 1.1, seed: int = None, stop_at_eos: bool = False):
+        """DistributedLLM.generate on this box: clear the contexts, tokenize, then up to max_steps steps of the client's
+        Sampler, all on the GPU with no host round trip between tokens (a one-session capi.Stream).  Yields each token
+        string as soon as its id is drawn; leaving the loop early cancels the steps that remain, and the slices' n_past
+        is then len(prompt tokens) + (strings yielded) - 1.  The draws come from numpy.random.Philox(key=seed), so
+        DistributedLLM.generate(..., rng=numpy.random.Generator(numpy.random.Philox(key=seed))) yields the same strings.
+        seed=None draws a key from numpy's global generator, so unseeded runs vary as the reference's do.
+        stop_at_eos=True ends the run after the end-of-sequence id (EOS_ID, yielded); the default runs max_steps steps,
+        as the reference does.  Needs every slice on one device."""
         extra = self._device_extra(extra_path, "sampled generation")
         if seed is None:
             seed = int(np.random.randint(0, 2 ** 64, dtype=np.uint64))
@@ -189,9 +196,13 @@ class LocalPipeline:
         tokens = extra.tokenize(prompt)
         if max_steps < 1:
             return
-        ids = self.capi.generate_sample(self.slices, extra, [0], [tokens], max_steps, temperature, repeat_penalty, [seed])
-        for token_id in ids[:, 0].tolist():
-            yield extra.token_text(token_id)
+        with self.capi.Stream(self.slices, extra) as st:
+            st.add(0, tokens, max_steps, temperature, repeat_penalty, seed, stop_ids=[EOS_ID] if stop_at_eos else ())
+            for j, (_, token_id) in enumerate(st):
+                if token_id < 0:
+                    raise self.capi.B200Error(1, "step %d: the logits hold a NaN or +inf, are all -inf or overflow "
+                                                 "float64 once scaled, so they have no distribution" % j)
+                yield extra.token_text(token_id)
 
     def perplexity(self, extra_path: str, text: str) -> float:
         """DistributedLLM.perplexity on this box: clear the contexts, tokenize, then score the text on the GPU

@@ -100,6 +100,9 @@ struct b200_slice {
     // k-quant slices: the Q8_K input of the next matmul, quantised once per column (k_quant_q8k, PRO_PREQ)
     int * kq_aq = nullptr; float * kq_ad = nullptr;
     std::map<GraphKey, cudaGraphExec_t> pp_graphs;
+    // the generation stream (b200_stream_open) this handle belongs to until b200_stream_close; every other entry point
+    // refuses the handle meanwhile
+    const b200_stream * owner = nullptr;
 };
 
 namespace b200 {
@@ -1222,6 +1225,13 @@ static void destroy(b200_slice * s) {
     delete s;
 }
 
+// A handle inside an open generation stream belongs to it: a call from elsewhere fails at once instead of waiting for the
+// stream to end or racing the steps it has enqueued.
+static int refuse_owned(const b200_slice * s) {
+    return fail(B200_EINVAL, "the handle belongs to the open generation stream %p: b200_stream_close it first", (const void *) s->owner);
+}
+#define B200_UNOWNED(h) do { if ((h)->owner) return b200::refuse_owned(h); } while (0)
+
 }  // namespace b200
 
 // ============================================================================ C ABI
@@ -1271,7 +1281,7 @@ int b200_slice_load_ex(const char * path, int device, int n_ctx, int n_sessions,
 
 int b200_slice_unload(b200_slice_t * s) {
     if (!s) return fail(B200_EINVAL, "null handle");
-    { std::lock_guard<std::mutex> lk(s->mu); }       // let a call that is inside the library finish (see the header: no NEW call may race unload)
+    { std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s); }   // let a call that is inside the library finish (see the header: no NEW call may race unload)
     destroy(s);
     return 0;
 }
@@ -1290,7 +1300,7 @@ int b200_device_init(int device) {
 
 int b200_slice_clear(b200_slice_t * s) {
     if (!s) return fail(B200_EINVAL, "null handle");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     B200_CUDA(cudaSetDevice(s->device));
     B200_CUDA(cudaMemsetAsync(s->d_npast, 0, 4, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));
@@ -1300,7 +1310,7 @@ int b200_slice_clear(b200_slice_t * s) {
 
 int b200_slice_rewind(b200_slice_t * s, int n_past) {
     if (!s) return fail(B200_EINVAL, "null handle");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     if (n_past < 0 || n_past > s->past[0]) return fail(B200_EINVAL, "rewind target %d outside [0, %d]", n_past, s->past[0]);
     B200_CUDA(cudaSetDevice(s->device));
     B200_CUDA(cudaMemcpyAsync(s->d_npast, &n_past, 4, cudaMemcpyHostToDevice, s->stream));
@@ -1311,6 +1321,7 @@ int b200_slice_rewind(b200_slice_t * s, int n_past) {
 
 int b200_slice_info(b200_slice_t * s, b200_slice_info_t * info) {
     if (!s || !info) return fail(B200_EINVAL, "null argument");
+    B200_UNOWNED(s);
     info->n_embd = s->E; info->n_head = s->H; info->n_ff = s->FF; info->n_layer = s->L; info->first_layer = s->first_layer;
     info->n_ctx = s->n_ctx; info->n_past = s->past[0]; info->weight_type = s->wtype; info->device = s->device;
     info->weight_bytes = s->weight_bytes; info->kv_bytes_per_pos = (int64_t) s->L * 2 * s->E * 2;
@@ -1319,13 +1330,13 @@ int b200_slice_info(b200_slice_t * s, b200_slice_info_t * info) {
 
 int b200_slice_forward(b200_slice_t * s, const float * in, int n_tokens, float * out) {
     if (!s || !in || !out) return fail(B200_EINVAL, "null argument");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     return forward_locked(s, in, n_tokens, out, true);
 }
 
 int b200_slice_forward_device(b200_slice_t * s, const float * d_in, int n_tokens, float * d_out, int sync) {
     if (!s || !d_in || !d_out) return fail(B200_EINVAL, "null argument");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     int rc = forward_locked(s, d_in, n_tokens, d_out, false);
     if (rc) return rc;
     if (sync) B200_CUDA(cudaStreamSynchronize(s->stream));
@@ -1338,13 +1349,14 @@ int b200_session_count(b200_slice_t * s) { return s ? s->n_sessions : 0; }
 int b200_session_n_past(b200_slice_t * s, int session) {
     if (!s || session < 0 || session >= s->n_sessions) return -1;
     std::lock_guard<std::mutex> lk(s->mu);
+    if (s->owner) { refuse_owned(s); return -1; }
     return s->past[session];
 }
 
 int b200_session_clear(b200_slice_t * s, int session) {
     if (!s) return fail(B200_EINVAL, "null handle");
     if (session < -1 || session >= s->n_sessions) return fail(B200_EINVAL, "session %d outside [0, %d)", session, s->n_sessions);
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     B200_CUDA(cudaSetDevice(s->device));
     if (session < 0) {
         B200_CUDA(cudaMemsetAsync(s->d_npast, 0, 4 * (size_t) s->n_sessions, s->stream));
@@ -1360,7 +1372,7 @@ int b200_session_clear(b200_slice_t * s, int session) {
 int b200_session_rewind(b200_slice_t * s, int session, int n_past) {
     if (!s) return fail(B200_EINVAL, "null handle");
     if (session < 0 || session >= s->n_sessions) return fail(B200_EINVAL, "session %d outside [0, %d)", session, s->n_sessions);
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     if (n_past < 0 || n_past > s->past[session]) return fail(B200_EINVAL, "rewind target %d outside [0, %d]", n_past, s->past[session]);
     B200_CUDA(cudaSetDevice(s->device));
     B200_CUDA(cudaMemcpyAsync(s->d_npast + session, &n_past, 4, cudaMemcpyHostToDevice, s->stream));
@@ -1371,13 +1383,13 @@ int b200_session_rewind(b200_slice_t * s, int session, int n_past) {
 
 int b200_session_forward(b200_slice_t * s, int session, const float * in, int n_tokens, float * out) {
     if (!s || !in || !out) return fail(B200_EINVAL, "null argument");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     return forward_locked(s, in, n_tokens, out, true, session);
 }
 
 int b200_session_forward_device(b200_slice_t * s, int session, const float * d_in, int n_tokens, float * d_out, int sync) {
     if (!s || !d_in || !d_out) return fail(B200_EINVAL, "null argument");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     int rc = forward_locked(s, d_in, n_tokens, d_out, false, session);
     if (rc) return rc;
     if (sync) B200_CUDA(cudaStreamSynchronize(s->stream));
@@ -1386,13 +1398,13 @@ int b200_session_forward_device(b200_slice_t * s, int session, const float * d_i
 
 int b200_batch_forward(b200_slice_t * s, const int * sessions, int n_seq, const float * in, float * out) {
     if (!s || !sessions || !in || !out) return fail(B200_EINVAL, "null argument");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     return pass_locked(s, sessions, nullptr, n_seq, in, out, true);
 }
 
 int b200_batch_forward_device(b200_slice_t * s, const int * sessions, int n_seq, const float * d_in, float * d_out, int sync) {
     if (!s || !sessions || !d_in || !d_out) return fail(B200_EINVAL, "null argument");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     int rc = pass_locked(s, sessions, nullptr, n_seq, d_in, d_out, false);
     if (rc) return rc;
     if (sync) B200_CUDA(cudaStreamSynchronize(s->stream));
@@ -1401,13 +1413,13 @@ int b200_batch_forward_device(b200_slice_t * s, const int * sessions, int n_seq,
 
 int b200_mixed_forward(b200_slice_t * s, const int * sessions, const int * counts, int n_seq, const float * in, float * out) {
     if (!s || !sessions || !counts || !in || !out) return fail(B200_EINVAL, "null argument");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     return pass_locked(s, sessions, counts, n_seq, in, out, true);
 }
 
 int b200_mixed_forward_device(b200_slice_t * s, const int * sessions, const int * counts, int n_seq, const float * d_in, float * d_out, int sync) {
     if (!s || !sessions || !counts || !d_in || !d_out) return fail(B200_EINVAL, "null argument");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     int rc = pass_locked(s, sessions, counts, n_seq, d_in, d_out, false);
     if (rc) return rc;
     if (sync) B200_CUDA(cudaStreamSynchronize(s->stream));
@@ -1416,6 +1428,7 @@ int b200_mixed_forward_device(b200_slice_t * s, const int * sessions, const int 
 
 int b200_slice_sync(b200_slice_t * s) {
     if (!s) return fail(B200_EINVAL, "null handle");
+    B200_UNOWNED(s);
     B200_CUDA(cudaSetDevice(s->device));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     return 0;
@@ -1436,7 +1449,7 @@ float * b200_slice_dev_out(b200_slice_t * s) { return s ? s->d_out : nullptr; }
 
 int b200_slice_set_fast_prefill(b200_slice_t * s, int on, int min_tokens) {
     if (!s) return fail(B200_EINVAL, "null handle");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     s->fast_prefill = on != 0;
     if (min_tokens > 0) s->fast_min_tokens = min_tokens;
     return 0;
@@ -1446,13 +1459,14 @@ int b200_slice_set_fast_prefill(b200_slice_t * s, int on, int min_tokens) {
  * attention launch is skipped, so hidden states are meaningless and the KV cache is not appended). */
 int b200_debug_skip_attention(b200_slice_t * s, int on) {
     if (!s) return fail(B200_EINVAL, "null handle");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     s->skip_attention = on != 0;
     return 0;
 }
 
 int b200_slice_mark(b200_slice_t * s, int which) {
     if (!s || which < 0 || which > 1) return fail(B200_EINVAL, "bad argument");
+    B200_UNOWNED(s);
     B200_CUDA(cudaSetDevice(s->device));
     if (!s->mark[which]) B200_CUDA(cudaEventCreate(&s->mark[which]));
     B200_CUDA(cudaEventRecord(s->mark[which], s->stream));
@@ -1470,14 +1484,14 @@ float b200_slice_mark_elapsed_ms(b200_slice_t * s) {
 
 int b200_slice_profile(b200_slice_t * s, int enable) {
     if (!s) return fail(B200_EINVAL, "null handle");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     s->profiling = enable != 0; s->prof_used = 0; s->prof_cls.clear();
     return 0;
 }
 
 int b200_slice_profile_read(b200_slice_t * s, float * ms_by_class, int * launches_by_class, int n_class) {
     if (!s || !ms_by_class || !launches_by_class) return fail(B200_EINVAL, "null argument");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     B200_CUDA(cudaSetDevice(s->device));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     for (int i = 0; i < n_class; i++) { ms_by_class[i] = 0.f; launches_by_class[i] = 0; }
@@ -1494,7 +1508,7 @@ int b200_slice_profile_read(b200_slice_t * s, float * ms_by_class, int * launche
 /* Switch the in-kernel timeline on or off at run time (drops the captured decode graphs so the next step re-captures). */
 int b200_debug_trace_enable(b200_slice_t * s, int on) {
     if (!s) return fail(B200_EINVAL, "null handle");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     B200_CUDA(cudaSetDevice(s->device));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     for (auto & kv : s->graphs) cudaGraphExecDestroy(kv.second);
@@ -1528,6 +1542,7 @@ int b200_debug_trace_read(b200_slice_t * s, unsigned long long * out, int * cls,
  * last fast-mode matmul). */
 int b200_debug_read(b200_slice_t * s, int which, size_t offset_words, size_t count, void * out) {
     if (!s || !out) return fail(B200_EINVAL, "null argument");
+    B200_UNOWNED(s);
     const void * src[10] = {s->qkv, s->att, s->ffin, s->gate, s->xa, s->xb, s->q16, s->kc, s->vc, s->xh};
     if (which < 0 || which > 9) return fail(B200_EINVAL, "bad buffer id %d", which);
     B200_CUDA(cudaSetDevice(s->device));
@@ -1600,7 +1615,7 @@ int b200_pipeline_init(b200_slice_t * s, int rank, int nranks, const void * id12
     if (!s || !id128 || rank < 0 || rank >= nranks) return fail(B200_EINVAL, "bad pipeline arguments");
     NcclApi & n = nccl();
     if (!n.lib || !n.CommInitRank) return fail(B200_ENCCL, "libnccl.so.2 not found (set B200_NCCL_LIB)");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     B200_CUDA(cudaSetDevice(s->device));
     NcclId id; memcpy(id.bytes, id128, 128);
     int rc = n.CommInitRank(&s->nccl_comm, nranks, id, rank);
@@ -1730,34 +1745,34 @@ static int pipeline_step_locked(b200_slice * s, const float * d_in, int n_rows, 
 
 int b200_pipeline_step(b200_slice_t * s, const float * d_in, int n_tokens, int ring) {
     if (!s || !s->nccl_comm) return fail(B200_EINVAL, "pipeline not initialised");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     return pipeline_step_locked(s, d_in, n_tokens, ring, 0, nullptr);
 }
 
 int b200_pipeline_step_session(b200_slice_t * s, int session, const float * d_in, int n_tokens, int ring) {
     if (!s || !s->nccl_comm) return fail(B200_EINVAL, "pipeline not initialised");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     return pipeline_step_locked(s, d_in, n_tokens, ring, session, nullptr);
 }
 
 int b200_pipeline_step_batch(b200_slice_t * s, const int * sessions, int n_seq, const float * d_in, int ring) {
     if (!s || !s->nccl_comm) return fail(B200_EINVAL, "pipeline not initialised");
     if (!sessions) return fail(B200_EINVAL, "null session list");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     return pipeline_step_locked(s, d_in, n_seq, ring, 0, sessions);
 }
 
 int b200_pipeline_step_mixed(b200_slice_t * s, const int * sessions, const int * counts, int n_seq, const float * d_in, int ring) {
     if (!s || !s->nccl_comm) return fail(B200_EINVAL, "pipeline not initialised");
     if (!sessions || !counts) return fail(B200_EINVAL, "null session or count list");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     return pipeline_step_locked(s, d_in, n_seq, ring, 0, sessions, counts);
 }
 
 /* ---- peer-memory hand-off: mailboxes mapped across processes with cudaIpc --------------------------------------- */
 int b200_pipeline_mailbox_export(b200_slice_t * s, void * handle64) {
     if (!s || !handle64) return fail(B200_EINVAL, "null argument");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     B200_CUDA(cudaSetDevice(s->device));
     s->mb_slot_floats = (size_t) s->n_ctx * s->E;
     const size_t bytes = sizeof(MailboxHdr) + (size_t) kMbSlots * s->mb_slot_floats * 8;      // 8-byte {value, seq} elements
@@ -1781,7 +1796,7 @@ int b200_pipeline_mailbox_export(b200_slice_t * s, void * handle64) {
 
 int b200_pipeline_mailbox_connect(b200_slice_t * s, const void * handles, int nranks) {
     if (!s || !handles) return fail(B200_EINVAL, "null argument");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     if (!s->mb_block) return fail(B200_EINVAL, "export this rank's mailbox first");
     if (nranks != s->pp_world || nranks < 2) return fail(B200_EINVAL, "mailbox_connect: %d handles for a pipeline of %d ranks", nranks, s->pp_world);
     if (env_int("B200_PP_PEER", 1) == 0) { s->mb_on = false; return 0; }       // keep the NCCL send/recv path (tested fallback)
@@ -1808,7 +1823,7 @@ int b200_pipeline_mailbox_connect(b200_slice_t * s, const void * handles, int nr
  * (one iteration = `world` hops).  Every rank must call it. */
 int b200_pipeline_pingpong(b200_slice_t * s, int n_rows, int iters, float * us_per_iter) {
     if (!s || !s->nccl_comm || !us_per_iter) return fail(B200_EINVAL, "pipeline not initialised");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     B200_CUDA(cudaSetDevice(s->device));
     const int r = s->pp_rank, W = s->pp_world;
     const size_t count = (size_t) n_rows * s->E;
@@ -1854,7 +1869,7 @@ int b200_pipeline_transport(b200_slice_t * s) { return s && s->mb_on ? 1 : 0; }
  * 1 = peer mailboxes (only valid after a successful connect). */
 int b200_pipeline_set_transport(b200_slice_t * s, int peer) {
     if (!s) return fail(B200_EINVAL, "null handle");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     if (peer && !(s->mb_next && s->mb_prev)) return fail(B200_EINVAL, "peer transport needs connected mailboxes");
     s->mb_on = peer != 0;
     return 0;
@@ -1876,7 +1891,7 @@ int b200_pipeline_error(b200_slice_t * s) {
  * collects session k's result only when it needs it (rank r then works on session k while rank r+1 works on k-1). */
 int b200_pipeline_collect(b200_slice_t * s, int n_rows, float * d_dst) {
     if (!s || !s->nccl_comm) return fail(B200_EINVAL, "pipeline not initialised");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     if (s->pp_rank != 0 || s->pp_world < 2) return 0;
     if (n_rows <= 0 || n_rows > s->n_ctx) return fail(B200_EINVAL, "n_rows %d outside [1, n_ctx]", n_rows);
     B200_CUDA(cudaSetDevice(s->device));
@@ -1902,7 +1917,7 @@ float * b200_pipeline_result(b200_slice_t * s) { return s ? (s->pp_world > 1 && 
 
 int b200_pipeline_destroy(b200_slice_t * s) {
     if (!s) return fail(B200_EINVAL, "null handle");
-    std::lock_guard<std::mutex> lk(s->mu);
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     if (s->nccl_comm) {
         cudaSetDevice(s->device);
         cudaStreamSynchronize(s->stream);
@@ -2077,13 +2092,9 @@ __global__ void __launch_bounds__(1024) k_argmax_first(const float * logits, int
     }
 }
 
-// The same rule for each of gridDim.x rows of [rows][n] logits, one block per row (the body is k_argmax_first's, kept
-// apart so that kernel's code does not change).  Row k's id goes to tok[k], which the next step's embedding reads, and
-// to ids[k].
-__global__ void __launch_bounds__(1024) k_argmax_rows(const float * logits, int n, int32_t * tok, int32_t * ids) {
+// k_argmax_first's rule on one row of n logits, for a whole block: the id is valid in thread 0.
+__device__ __forceinline__ int argmax_row(const float * logits, int n) {
     __shared__ float sv[32]; __shared__ int si[32];
-    const int k = blockIdx.x;
-    logits += (size_t) k * n;
     float bv = -(1000000000000.0f); int bi = 0x7fffffff;
     for (int i = threadIdx.x; i < n; i += blockDim.x) { const float v = logits[i]; if (v > bv) { bv = v; bi = i; } }
     auto better = [](float v, int i, float bv, int bi) { return v > bv || (v == bv && i < bi); };
@@ -2100,8 +2111,16 @@ __global__ void __launch_bounds__(1024) k_argmax_rows(const float * logits, int 
             const float v = __shfl_xor_sync(0xffffffffu, bv, o); const int i = __shfl_xor_sync(0xffffffffu, bi, o);
             if (better(v, i, bv, bi)) { bv = v; bi = i; }
         }
-        if (threadIdx.x == 0) { const int best = bi == 0x7fffffff ? 0 : bi; tok[k] = best; ids[k] = best; }
     }
+    return bi == 0x7fffffff ? 0 : bi;
+}
+
+// The same rule for each of gridDim.x rows of [rows][n] logits, one block per row (k_argmax_first itself is kept apart so
+// its code does not change).  Row k's id goes to tok[k], which the next step's embedding reads, and to ids[k].
+__global__ void __launch_bounds__(1024) k_argmax_rows(const float * logits, int n, int32_t * tok, int32_t * ids) {
+    const int k = blockIdx.x;
+    const int best = argmax_row(logits + (size_t) k * n, n);
+    if (threadIdx.x == 0) { tok[k] = best; ids[k] = best; }
 }
 
 // Word d (0-based) of numpy.random.Philox(key=seed): word d % 4 of Philox4x64-10 on counter (d / 4 + 1, 0, 0, 0) and
@@ -2137,13 +2156,14 @@ struct SampleArgs {
     int * bad; int bad_base;         // a row without a distribution: id -1, atomicMin(bad, bad_base + k)
 };
 
-__device__ __forceinline__ double sample_weight(const SampleArgs & a, const float * x, const uint32_t * bits, int i, double m) {
-    const double d = (bits[i >> 5] >> (i & 31)) & 1u ? a.dp : a.dt;
+__device__ __forceinline__ double sample_weight(double dt, double dp, const float * x, const uint32_t * bits, int i, double m) {
+    const double d = (bits[i >> 5] >> (i & 31)) & 1u ? dp : dt;
     return exp(__dsub_rn(__ddiv_rn((double) x[i], d), m));
 }
 
-// The client's Sampler (cli_api/common.py:64-86) on each of gridDim.x rows, one block per row.  Thread t owns the
-// contiguous chunk [t*C, t*C + C) of the row.
+// The client's Sampler (cli_api/common.py:64-86) on one row x of n logits, for a whole block: divisors dt / dp, penalty
+// bitmap bits, u = draw `draw` of Philox stream `seed`.  The id is valid in thread 0; -1 when the row has no
+// distribution.  Thread t owns the contiguous chunk [t*C, t*C + C) of the row.
 //   1. max y: the divisor takes two values and a correctly rounded division is monotone, so max y is the larger of
 //      (max x over ids outside prev) / dt and (max x over ids in prev) / dp.  A NaN, or a max that is not finite, is a
 //      row numpy rejects.
@@ -2153,14 +2173,13 @@ __device__ __forceinline__ double sample_weight(const SampleArgs & a, const floa
 //      the draw; warp 0 re-walks that chunk in order from O_t and picks the first id whose running sum passes u*S,
 //      falling back to the chunk's last id of positive weight.  An id of weight 0 never moves the sum, so it is never
 //      picked.  The row's logits are read from L2 in each pass.
-__global__ void __launch_bounds__(1024) k_sample_rows(SampleArgs a) {
+__device__ __forceinline__ int sample_row(const float * x, int n, const uint32_t * bits, double dt, double dp, uint64_t seed,
+                                          long long draw) {
     __shared__ float smf[32], smp[32];
     __shared__ double swt[32], swo[32], s_m, s_u, s_total, s_target, s_o;
     __shared__ int s_chunk;
-    const int k = blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5, nwarp = blockDim.x >> 5;
-    const float * x = a.logits + (size_t) k * a.n;
-    uint32_t * bits = a.pen + (size_t) k * ((a.n + 31) >> 5);
-    const int C = (a.n + blockDim.x - 1) / blockDim.x, i0 = min(a.n, t * C), i1 = min(a.n, i0 + C);
+    const int t = threadIdx.x, lane = t & 31, wid = t >> 5, nwarp = blockDim.x >> 5;
+    const int C = (n + blockDim.x - 1) / blockDim.x, i0 = min(n, t * C), i1 = min(n, i0 + C);
     float mf = -INFINITY, mp = -INFINITY; bool nan = false;
     for (int i = i0; i < i1; i++) {
         const float v = x[i];
@@ -2179,18 +2198,15 @@ __global__ void __launch_bounds__(1024) k_sample_rows(SampleArgs a) {
             mf = fmaxf(mf, __shfl_xor_sync(0xffffffffu, mf, o)); mp = fmaxf(mp, __shfl_xor_sync(0xffffffffu, mp, o));
         }
         if (lane == 0) {
-            s_m = fmax(__ddiv_rn((double) mf, a.dt), __ddiv_rn((double) mp, a.dp));
-            s_u = (double)(philox_word(a.seeds[k], a.draw) >> 11) * 0x1.0p-53;
+            s_m = fmax(__ddiv_rn((double) mf, dt), __ddiv_rn((double) mp, dp));
+            s_u = (double)(philox_word(seed, draw) >> 11) * 0x1.0p-53;
         }
     }
     __syncthreads();
     const double m = s_m;
-    if (any_nan || !isfinite(m)) {
-        if (t == 0) { a.tok[k] = -1; a.ids[k] = -1; atomicMin(a.bad, a.bad_base + k); }
-        return;
-    }
+    if (any_nan || !isfinite(m)) return -1;
     double tot = 0.0;
-    for (int i = i0; i < i1; i++) tot = __dadd_rn(tot, sample_weight(a, x, bits, i, m));
+    for (int i = i0; i < i1; i++) tot = __dadd_rn(tot, sample_weight(dt, dp, x, bits, i, m));
     const double P = warp_prefix_ordered(tot), Pin = __dadd_rn(P, tot);
     if (lane == 31) swt[wid] = Pin;
     __syncthreads();
@@ -2206,12 +2222,12 @@ __global__ void __launch_bounds__(1024) k_sample_rows(SampleArgs a) {
     __syncthreads();
     if (t == s_chunk) s_o = O;
     __syncthreads();
-    if (wid != 0) return;
-    const int j0 = min(a.n, s_chunk * C), j1 = min(a.n, j0 + C);
+    if (wid != 0) return -1;
+    const int j0 = min(n, s_chunk * C), j1 = min(n, j0 + C);
     double r = s_o; int id = -1, last = -1;
     for (int b = j0; b < j1 && id < 0; b += 32) {
         const int i = b + lane;
-        const double e = i < j1 ? sample_weight(a, x, bits, i, m) : 0.0;
+        const double e = i < j1 ? sample_weight(dt, dp, x, bits, i, m) : 0.0;
         double q = r;                                  // r + e_b + ... + e_i, added in index order
         for (int j = 0; j < 32; j++) { const double w = __shfl_sync(0xffffffffu, e, j); if (j <= lane) q = __dadd_rn(q, w); }
         const unsigned hit = __ballot_sync(0xffffffffu, i < j1 && q > target);
@@ -2220,11 +2236,64 @@ __global__ void __launch_bounds__(1024) k_sample_rows(SampleArgs a) {
         if (pos) last = b + 31 - __clz(pos);
         r = __shfl_sync(0xffffffffu, q, 31);
     }
-    if (lane == 0) {
-        if (id < 0) id = last;
-        a.tok[k] = id; a.ids[k] = id;
-        bits[id >> 5] |= 1u << (id & 31);
+    return id < 0 ? last : id;
+}
+
+// k_sample_rows: sample_row on each of gridDim.x rows, one block per row; row k is session k of the call.
+__global__ void __launch_bounds__(1024) k_sample_rows(SampleArgs a) {
+    const int k = blockIdx.x;
+    uint32_t * bits = a.pen + (size_t) k * ((a.n + 31) >> 5);
+    const int id = sample_row(a.logits + (size_t) k * a.n, a.n, bits, a.dt, a.dp, a.seeds[k], a.draw);
+    if (threadIdx.x != 0) return;
+    a.tok[k] = id; a.ids[k] = id;
+    if (id < 0) atomicMin(a.bad, a.bad_base + k);
+    else bits[id >> 5] |= 1u << (id & 31);
+}
+
+// ---- generation streams (b200_stream_*): the sampler's state lives in per-session slots, and a step's rows name their slot
+struct StreamSlot { uint64_t seed; double dt, dp; int sampled; };   // device table, one per session
+struct StreamRow { long long draw; int slot, gather; };              // per step, in mapped pinned memory: draw index, slot,
+                                                                    // and the session's last row in the pass
+
+// A step's token rows: row r is the prompt id spec[r] when spec[r] >= 0, else the last id slot ~spec[r] drew.  spec lies in
+// mapped pinned memory.
+__global__ void k_stream_tokens(const int32_t * spec, const int32_t * last, int n, int32_t * tok) {
+    for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x) {
+        const int32_t v = spec[r];
+        tok[r] = v >= 0 ? v : last[~v];
     }
+}
+
+// Row k of out is row rows[k].gather of x: each session's last row of a mixed pass, packed for the lm_head.
+__global__ void k_gather_rows(const float * x, const StreamRow * rows, int E, float * out) {
+    __shared__ int g;
+    if (threadIdx.x == 0) g = rows[blockIdx.y].gather;
+    __syncthreads();
+    const float * src = x + (size_t) g * E;
+    float * dst = out + (size_t) blockIdx.y * E;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < E; i += gridDim.x * blockDim.x) dst[i] = src[i];
+}
+
+// One id for each of gridDim.x rows of [rows][n] logits, row k for slot rows[k].slot: the argmax rule on the raw logits for
+// a greedy slot (argmax_row), the Sampler with the slot's divisors, key and the row's draw index for a sampled one
+// (sample_row, which then marks the id in the slot's penalty bitmap).  The id becomes the slot's last id, which the next
+// step's k_stream_tokens reads, and is stored into cell k of the step's publish ring in mapped pinned memory: the host
+// sets every cell to INT32_MIN before it enqueues the step, so each cell carries its own readiness.
+__global__ void __launch_bounds__(1024) k_stream_draw(const float * logits, int n, const StreamRow * rows,
+                                                      const StreamSlot * slots, uint32_t * pen, int32_t * last, int32_t * ring) {
+    __shared__ StreamRow s_row;
+    const int k = blockIdx.x;
+    if (threadIdx.x == 0) s_row = rows[k];
+    __syncthreads();
+    const int slot = s_row.slot;
+    const StreamSlot sl = slots[slot];
+    const float * x = logits + (size_t) k * n;
+    uint32_t * bits = pen + (size_t) slot * ((n + 31) >> 5);
+    const int id = sl.sampled ? sample_row(x, n, bits, sl.dt, sl.dp, sl.seed, s_row.draw) : argmax_row(x, n);
+    if (threadIdx.x != 0) return;
+    if (sl.sampled && id >= 0) bits[id >> 5] |= 1u << (id & 31);
+    last[slot] = id;
+    *(volatile int32_t *)(ring + k) = id;
 }
 
 // The client's perplexity term (cli_api/common.py:129-139) for each of gridDim.x rows of [rows][n] logits, one block per
@@ -2381,6 +2450,7 @@ int b200_extra_load(const char * path, int device, b200_extra_t ** out) {
 
 int b200_extra_unload(b200_extra_t * e) {
     if (!e) return fail(B200_EINVAL, "null handle");
+    { std::lock_guard<std::mutex> lk(e->mu); B200_UNOWNED(&e->ctx); }
     b200_slice * s = &e->ctx;
     cudaSetDevice(s->device);
     if (s->stream) cudaStreamSynchronize(s->stream);
@@ -2402,7 +2472,7 @@ int b200_extra_dims(b200_extra_t * e, int * n_vocab, int * n_embd) {
 
 int b200_extra_embed(b200_extra_t * e, const int32_t * tokens, int n_tokens, float * out) {
     if (!e || !tokens || !out || n_tokens <= 0) return fail(B200_EINVAL, "bad argument");
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::lock_guard<std::mutex> lk(e->mu); B200_UNOWNED(&e->ctx);
     b200_slice * s = &e->ctx;
     B200_CUDA(cudaSetDevice(s->device));
     int rc = extra_reserve(e, n_tokens);
@@ -2445,7 +2515,7 @@ static int extra_logits_device(b200_extra * e, const float * emb, int n_tokens) 
 
 int b200_extra_logits(b200_extra_t * e, const float * emb, int n_tokens, int all_logits, float * out) {
     if (!e || !emb || !out || n_tokens <= 0) return fail(B200_EINVAL, "bad argument");
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::lock_guard<std::mutex> lk(e->mu); B200_UNOWNED(&e->ctx);
     b200_slice * s = &e->ctx;
     B200_CUDA(cudaSetDevice(s->device));
     int rc = extra_logits_device(e, emb, n_tokens);
@@ -2459,7 +2529,7 @@ int b200_extra_logits(b200_extra_t * e, const float * emb, int n_tokens, int all
 
 int b200_extra_next_token(b200_extra_t * e, const float * emb, int n_tokens, int32_t * token) {
     if (!e || !emb || !token || n_tokens <= 0) return fail(B200_EINVAL, "bad argument");
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::lock_guard<std::mutex> lk(e->mu); B200_UNOWNED(&e->ctx);
     b200_slice * s = &e->ctx;
     B200_CUDA(cudaSetDevice(s->device));
     // only the LAST token's logits decide (get_llm_output + sample_next_token, tensor_processor.cpp:1787-1908); rows of
@@ -2655,9 +2725,10 @@ extern "C" {
 
 namespace b200 {
 
-// Every handle's mutex of a device loop, in address order, so that two loops that share handles cannot deadlock.
+// Every handle's mutex of a device loop, in address order, so that two loops that share handles cannot deadlock.  A handle
+// that belongs to a generation stream other than `self` is refused.
 static int lock_handles(b200_slice_t * const * slices, int n_slices, b200_extra_t * e,
-                        std::vector<std::unique_lock<std::mutex>> & locks) {
+                        std::vector<std::unique_lock<std::mutex>> & locks, const b200_stream * self = nullptr) {
     std::vector<std::mutex *> mus{&e->mu};
     for (int i = 0; i < n_slices; i++) {
         if (!slices[i]) return fail(B200_EINVAL, "slice %d is a null handle", i);
@@ -2666,6 +2737,9 @@ static int lock_handles(b200_slice_t * const * slices, int n_slices, b200_extra_
     std::sort(mus.begin(), mus.end());
     if (std::adjacent_find(mus.begin(), mus.end()) != mus.end()) return fail(B200_EINVAL, "a slice handle is listed twice");
     for (std::mutex * m : mus) locks.emplace_back(*m);
+    if (e->ctx.owner != self) return refuse_owned(&e->ctx);
+    for (int i = 0; i < n_slices; i++)
+        if (slices[i]->owner != self) return refuse_owned(slices[i]);
     return 0;
 }
 
@@ -2801,7 +2875,7 @@ int b200_generate_sample(b200_slice_t * const * slices, int n_slices, b200_extra
 
 int b200_extra_sample(b200_extra_t * e, const float * logits, int n_rows, const b200_sampling_t * sp, int32_t * ids) {
     if (!e || !logits || n_rows < 1 || !ids) return fail(B200_EINVAL, "b200_extra_sample: null argument or no rows");
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::lock_guard<std::mutex> lk(e->mu); B200_UNOWNED(&e->ctx);
     if (int rc = sample_check(sp, n_rows, e->n_vocab)) return rc;
     const size_t V = (size_t) e->n_vocab;
     for (size_t i = 0; i < (size_t) n_rows * V; i++)
@@ -2831,7 +2905,7 @@ int b200_score(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, co
 
 int b200_extra_nll(b200_extra_t * e, const float * logits, int n_rows, const int32_t * targets, double * nll) {
     if (!e || !logits || n_rows < 1 || !targets || !nll) return fail(B200_EINVAL, "b200_extra_nll: null argument or no rows");
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::lock_guard<std::mutex> lk(e->mu); B200_UNOWNED(&e->ctx);
     if (int rc = check_tokens(targets, n_rows, e->n_vocab, "target")) return rc;
     b200_slice * s = &e->ctx;
     B200_CUDA(cudaSetDevice(s->device));
@@ -2861,6 +2935,306 @@ const char * b200_extra_token_text(b200_extra_t * e, int32_t id, int * len) {
     if (!e || id < 0 || id >= (int32_t) e->vocab.size()) { if (len) *len = 0; return nullptr; }
     if (len) *len = (int) e->vocab[id].first.size();
     return e->vocab[id].first.data();
+}
+
+}  // extern "C"
+
+// ============================================================================ generation streams (b200_stream_*)
+// The generation loop, open-ended: the host schedules one step at a time (who decodes, which queued prompts join), keeps
+// up to `lookahead` steps enqueued beyond the oldest one the caller has not read, and learns the ids from a publish ring in
+// mapped pinned memory instead of synchronising.  The slices' streams are lent to the extra layers' stream from open to
+// close (StreamLoan), so every step is ordered on one stream, as in generate_locked.
+#include <deque>
+
+struct b200_stream {
+    std::vector<b200_slice *> slices; b200_extra * e = nullptr;
+    std::unique_ptr<b200::StreamLoan> loan;
+    int max_rows = 0, lookahead = 0, n_sess = 0, rows_cap = 0, nw = 0;   // rows_cap: sessions one step can hold
+    // device: per-session sampler slots, penalty bitmaps [n_sess][nw], last ids
+    b200::StreamSlot * d_slots = nullptr; uint32_t * d_pen = nullptr; int32_t * d_last = nullptr;
+    // mapped pinned, one region per step in flight (lookahead + 1): token specs [max_rows], rows [rows_cap], ids [rows_cap]
+    int32_t * h_spec = nullptr; b200::StreamRow * h_rows = nullptr; int32_t * h_ring = nullptr;
+    struct Sess {
+        int state = 0;                    // 0 not in the stream, 1 queued, 2 admitted (its prompt is enqueued)
+        unsigned gen = 0;                 // bumped when the session leaves: rows of steps enqueued before are dropped
+        std::vector<int32_t> prompt, stops;
+        std::vector<int> old;             // n_past on each slice when it was added
+        int max_tokens = 0, enq = 0, delivered = 0;   // ids enqueued / returned by b200_stream_read
+        long long first_draw = 0;
+    };
+    std::vector<Sess> sess;
+    std::deque<int> queue;                // added, not admitted yet, in add order
+    struct Step { int region; std::vector<std::pair<int, unsigned>> rows; size_t next = 0; };   // row k: (session, gen)
+    std::deque<Step> pending;             // enqueued steps whose ids have not all been read
+    long long n_steps = 0;
+};
+
+namespace b200 {
+
+constexpr int kStreamLookahead = 4;
+
+// The session leaves the stream: n_past = old + n_prompt + delivered - 1 (old when nothing was delivered) on every slice,
+// host copy now and device copy in stream order, behind any step the device still runs for it.  Those steps' rows are at
+// or above the new n_past, so they are unreachable.
+static int stream_finish(b200_stream * st, int k) {
+    b200_stream::Sess & z = st->sess[k];
+    if (z.state == 1) st->queue.erase(std::find(st->queue.begin(), st->queue.end(), k));
+    if (z.state == 2) {
+        for (size_t i = 0; i < st->slices.size(); i++) {
+            b200_slice * s = st->slices[i];
+            const int p = z.delivered ? z.old[i] + (int) z.prompt.size() + z.delivered - 1 : z.old[i];
+            if (s->past[k] == p) continue;
+            s->past[k] = p;
+            B200_CUDA(cudaMemcpyAsync(s->d_npast + k, &p, 4, cudaMemcpyHostToDevice, st->e->ctx.stream));   // staged at once
+        }
+    }
+    z.state = 0; z.gen++;
+    return 0;
+}
+
+// Schedules and enqueues one step (*did = false when no session has anything to run): every admitted session that still
+// owes ids decodes one row; queued prompts join in add order while the rows fit in max_rows.
+static int stream_step(b200_stream * st, bool * did) {
+    *did = false;
+    std::vector<int> ses, cnt;
+    int N = 0;
+    for (int k = 0; k < st->n_sess; k++) {
+        const b200_stream::Sess & z = st->sess[k];
+        if (z.state == 2 && z.enq < z.max_tokens) { ses.push_back(k); cnt.push_back(1); N++; }
+    }
+    const int n_decode = (int) ses.size();
+    while (!st->queue.empty() && N + (int) st->sess[st->queue.front()].prompt.size() <= st->max_rows) {
+        const int k = st->queue.front();
+        st->queue.pop_front();
+        ses.push_back(k); cnt.push_back((int) st->sess[k].prompt.size()); N += cnt.back();
+    }
+    const int n = (int) ses.size();
+    if (n == 0) return 0;
+    const int q = (int)(st->n_steps % (st->lookahead + 1));
+    int32_t * spec = st->h_spec + (size_t) q * st->max_rows;
+    StreamRow * rows = st->h_rows + (size_t) q * st->rows_cap;
+    volatile int32_t * ring = st->h_ring + (size_t) q * st->rows_cap;
+    b200_stream::Step step{q, {}, 0};
+    for (int j = 0, r = 0; j < n; j++) {
+        b200_stream::Sess & z = st->sess[ses[j]];
+        if (j < n_decode) spec[r++] = ~ses[j];
+        else for (int32_t t : z.prompt) spec[r++] = t;
+        rows[j] = {z.first_draw + z.enq, ses[j], r - 1};
+        ring[j] = INT32_MIN;
+        step.rows.emplace_back(ses[j], z.gen);
+    }
+    b200_extra * e = st->e;
+    b200_slice * x = &e->ctx;
+    k_stream_tokens<<<(N + 255) / 256, 256, 0, x->stream>>>(spec, st->d_last, N, e->d_tok);
+    k_embed_rows<<<dim3((e->E + 255) / 256, N), 256, 0, x->stream>>>(e->emb_raw, e->emb_type, e->E, e->d_tok, e->n_vocab, e->d_x);
+    B200_CUDA(cudaGetLastError());
+    x->launches += 2;
+    // a single session decoding alone replays the slice's captured decode graph; anything else is one pass (all-1 counts:
+    // the batched step).  Both are exact mode, as b200_mixed_forward.
+    const float * cur = e->d_x;
+    int rc;
+    for (b200_slice * s : st->slices) {
+        if (N == 1 && n_decode == 1) rc = forward_locked(s, cur, 1, s->d_out, false, ses[0]);
+        else                         rc = pass_locked(s, ses.data(), cnt.data(), n, cur, s->d_out, false);
+        if (rc) return rc;
+        cur = s->d_out;
+    }
+    if (N > n) {                                    // each session's last row, packed for the lm_head
+        k_gather_rows<<<dim3((e->E + 255) / 256, n), 256, 0, x->stream>>>(cur, rows, e->E, e->d_x);
+        B200_CUDA(cudaGetLastError());
+        x->launches++;
+        cur = e->d_x;
+    }
+    if ((rc = extra_lmhead(e, cur, n))) return rc;
+    k_stream_draw<<<n, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, rows, st->d_slots, st->d_pen, st->d_last, st->h_ring + (size_t) q * st->rows_cap);
+    B200_CUDA(cudaGetLastError());
+    x->launches++;
+    for (int j = 0; j < n; j++) {
+        b200_stream::Sess & z = st->sess[ses[j]];
+        z.state = 2; z.enq++;
+    }
+    st->pending.push_back(std::move(step));
+    st->n_steps++;
+    *did = true;
+    return 0;
+}
+
+static void stream_free(b200_stream * st) {
+    st->loan.reset();                              // waits for the stream, gives the slices their streams back
+    for (b200_slice * s : st->slices) s->owner = nullptr;
+    if (st->e) st->e->ctx.owner = nullptr;
+    cudaFree(st->d_slots); cudaFree(st->d_pen); cudaFree(st->d_last);
+    cudaFreeHost(st->h_spec); cudaFreeHost(st->h_rows); cudaFreeHost(st->h_ring);
+    delete st;
+}
+
+// Every stream call holds the handles' mutexes, so a call from another thread on one of them is refused at once.
+static int stream_lock(b200_stream * st, std::vector<std::unique_lock<std::mutex>> & locks) {
+    if (!st) return fail(B200_EINVAL, "null stream");
+    if (int rc = lock_handles(st->slices.data(), (int) st->slices.size(), st->e, locks, st)) return rc;
+    B200_CUDA(cudaSetDevice(st->e->ctx.device));
+    return 0;
+}
+
+}  // namespace b200
+
+extern "C" {
+
+int b200_stream_open(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int max_rows, int lookahead,
+                     b200_stream_t ** out) {
+    if (!slices || n_slices < 1 || !e || !out) return fail(B200_EINVAL, "b200_stream_open: null argument or no slices");
+    *out = nullptr;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(B200_ENODEV, "no CUDA device visible: no CPU fallback");
+    std::vector<std::unique_lock<std::mutex>> locks;
+    if (int rc = lock_handles(slices, n_slices, e, locks)) return rc;
+    if (int rc = chain_check(slices, n_slices, e)) return rc;
+    int n_ctx = INT_MAX, n_sess = INT_MAX;
+    for (int i = 0; i < n_slices; i++) { n_ctx = std::min(n_ctx, slices[i]->n_ctx); n_sess = std::min(n_sess, slices[i]->n_sessions); }
+    if (max_rows <= 0) max_rows = n_ctx;
+    if (max_rows > n_ctx) return fail(B200_EINVAL, "max_rows %d exceeds the smallest n_ctx %d", max_rows, n_ctx);
+    if (lookahead <= 0) lookahead = kStreamLookahead;
+    if (lookahead > 1024) return fail(B200_EINVAL, "lookahead %d exceeds 1024", lookahead);
+    B200_CUDA(cudaSetDevice(e->ctx.device));
+    b200_stream * st = new b200_stream();
+    st->slices.assign(slices, slices + n_slices); st->e = e;
+    st->max_rows = max_rows; st->lookahead = lookahead; st->n_sess = n_sess;
+    st->rows_cap = std::min(n_sess, max_rows); st->nw = (e->n_vocab + 31) / 32;
+    st->sess.resize(n_sess);
+    const size_t regions = (size_t) lookahead + 1;
+    auto fail_free = [&](int rc) { delete st; return rc; };
+    cudaError_t ce = cudaSuccess;
+    if ((ce = cudaMalloc(&st->d_slots, sizeof(StreamSlot) * n_sess)) != cudaSuccess ||
+        (ce = cudaMalloc(&st->d_pen, (size_t) 4 * st->nw * n_sess)) != cudaSuccess ||
+        (ce = cudaMalloc(&st->d_last, (size_t) 4 * n_sess)) != cudaSuccess ||
+        (ce = cudaHostAlloc(&st->h_spec, 4 * regions * max_rows, cudaHostAllocMapped)) != cudaSuccess ||
+        (ce = cudaHostAlloc(&st->h_rows, sizeof(StreamRow) * regions * st->rows_cap, cudaHostAllocMapped)) != cudaSuccess ||
+        (ce = cudaHostAlloc(&st->h_ring, 4 * regions * st->rows_cap, cudaHostAllocMapped)) != cudaSuccess) {
+        cudaFree(st->d_slots); cudaFree(st->d_pen); cudaFree(st->d_last);
+        cudaFreeHost(st->h_spec); cudaFreeHost(st->h_rows); cudaFreeHost(st->h_ring);
+        return fail_free(fail(B200_ECUDA, "stream buffers: %s", cudaGetErrorString(ce)));
+    }
+    if (int rc = extra_reserve(e, max_rows)) { stream_free(st); return rc; }
+    for (int i = 0; i < n_slices; i++)
+        if (cudaStreamSynchronize(slices[i]->stream) != cudaSuccess) { stream_free(st); return fail(B200_ECUDA, "slice %d: stream failed", i); }
+    st->loan.reset(new StreamLoan(slices, n_slices, e->ctx.stream));
+    for (int i = 0; i < n_slices; i++) slices[i]->owner = st;
+    e->ctx.owner = st;
+    *out = st;
+    return 0;
+}
+
+int b200_stream_add(b200_stream_t * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
+                    const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop) {
+    std::vector<std::unique_lock<std::mutex>> locks;
+    if (int rc = stream_lock(st, locks)) return rc;
+    if (session < 0 || session >= st->n_sess) return fail(B200_EINVAL, "session %d outside [0, %d)", session, st->n_sess);
+    b200_stream::Sess & z = st->sess[session];
+    if (z.state) return fail(B200_EINVAL, "session %d is already in the stream", session);
+    if (!prompt || n_prompt < 1) return fail(B200_EINVAL, "session %d: the prompt needs at least one id", session);
+    if (max_tokens < 1) return fail(B200_EINVAL, "session %d: max_tokens must be positive (got %d)", session, max_tokens);
+    if (n_stop < 0 || (n_stop > 0 && !stop_ids)) return fail(B200_EINVAL, "session %d: bad stop list", session);
+    const int V = st->e->n_vocab;
+    if (int rc = check_tokens(prompt, n_prompt, V, "prompt token")) return rc;
+    if (int rc = check_tokens(stop_ids, n_stop, V, "stop id")) return rc;
+    if (sp)
+        if (int rc = sample_check(sp, 1, V)) return rc;
+    for (size_t i = 0; i < st->slices.size(); i++) {
+        const b200_slice * s = st->slices[i];
+        if ((long long) s->past[session] + n_prompt + max_tokens - 1 > s->n_ctx)
+            return fail(B200_ECONTEXT, "context overflow: slice %zu session %d n_past %d + %d prompt tokens + %d steps > n_ctx %d",
+                        i, session, s->past[session], n_prompt, max_tokens - 1, s->n_ctx);
+    }
+    if (n_prompt > st->max_rows)
+        return fail(B200_EINVAL, "session %d: a prompt of %d ids exceeds max_rows %d (a prompt is never split)", session, n_prompt, st->max_rows);
+    // the slot's sampler state, in stream order behind any step still running for an earlier stay of the session
+    const double dt = sp ? sp->temperature + 1e-5 : 1.0;
+    const StreamSlot slot{sp ? sp->seeds[0] : 0, dt, sp ? sp->repeat_penalty * dt : 1.0, sp ? 1 : 0};
+    cudaStream_t cs = st->e->ctx.stream;
+    B200_CUDA(cudaMemcpyAsync(st->d_slots + session, &slot, sizeof slot, cudaMemcpyHostToDevice, cs));
+    if (sp) {
+        std::vector<uint32_t> pen(st->nw, 0u);
+        if (sp->history)
+            for (int j = 0; j < sp->history_counts[0]; j++) pen[sp->history[j] >> 5] |= 1u << (sp->history[j] & 31);
+        B200_CUDA(cudaMemcpyAsync(st->d_pen + (size_t) session * st->nw, pen.data(), pen.size() * 4, cudaMemcpyHostToDevice, cs));
+    }
+    z.prompt.assign(prompt, prompt + n_prompt);
+    z.stops.assign(stop_ids, stop_ids + n_stop);
+    z.old.clear();
+    for (const b200_slice * s : st->slices) z.old.push_back(s->past[session]);
+    z.max_tokens = max_tokens; z.enq = 0; z.delivered = 0;
+    z.first_draw = sp ? sp->first_draw : 0;
+    z.state = 1;
+    st->queue.push_back(session);
+    return 0;
+}
+
+int b200_stream_read(b200_stream_t * st, int32_t * sessions, int32_t * ids, int cap, int * n_out) {
+    if (!sessions || !ids || !n_out || cap < 1) return fail(B200_EINVAL, "b200_stream_read: null argument or cap < 1");
+    *n_out = 0;
+    std::vector<std::unique_lock<std::mutex>> locks;
+    if (int rc = stream_lock(st, locks)) return rc;
+    int got = 0;
+    long long spins = 0;
+    for (;;) {
+        while ((int) st->pending.size() <= st->lookahead) {
+            bool did = false;
+            if (int rc = stream_step(st, &did)) return rc;
+            if (!did) break;
+        }
+        if (got == cap || st->pending.empty()) break;
+        b200_stream::Step & f = st->pending.front();
+        const volatile int32_t * ring = st->h_ring + (size_t) f.region * st->rows_cap;
+        while (f.next < f.rows.size() && got < cap) {
+            const int32_t id = ring[f.next];
+            if (id == INT32_MIN) break;
+            const int k = f.rows[f.next].first;
+            const unsigned gen = f.rows[f.next].second;
+            f.next++;
+            b200_stream::Sess & z = st->sess[k];
+            if (z.state != 2 || z.gen != gen) continue;      // a step the device ran past the session's end
+            sessions[got] = k; ids[got] = id; got++;
+            z.delivered++;
+            if (id < 0 || z.delivered == z.max_tokens || std::find(z.stops.begin(), z.stops.end(), id) != z.stops.end())
+                if (int rc = stream_finish(st, k)) return rc;
+        }
+        if (f.next == f.rows.size()) { st->pending.pop_front(); spins = 0; continue; }
+        if (got > 0) break;
+        // nothing published yet: poll; now and then make sure the device is still running the steps
+        if (++spins % 4096 == 0) {
+            const cudaError_t q = cudaStreamQuery(st->e->ctx.stream);
+            if (q != cudaSuccess && q != cudaErrorNotReady) return fail(B200_ECUDA, "generation stream: %s", cudaGetErrorString(q));
+            if (q == cudaSuccess && ring[f.next] == INT32_MIN)
+                return fail(B200_ECUDA, "generation stream: the device finished a step without publishing its id");
+        }
+        std::this_thread::yield();
+    }
+    *n_out = got;
+    return 0;
+}
+
+int b200_stream_cancel(b200_stream_t * st, int session) {
+    std::vector<std::unique_lock<std::mutex>> locks;
+    if (int rc = stream_lock(st, locks)) return rc;
+    if (session < 0 || session >= st->n_sess || st->sess[session].state == 0)
+        return fail(B200_EINVAL, "session %d is not in the stream", session);
+    return stream_finish(st, session);
+}
+
+int b200_stream_close(b200_stream_t * st) {
+    int rc;
+    {
+        std::vector<std::unique_lock<std::mutex>> locks;
+        if ((rc = stream_lock(st, locks))) return rc;
+        for (int k = 0; k < st->n_sess && !rc; k++)
+            if (st->sess[k].state) rc = stream_finish(st, k);
+        if (!rc && cudaStreamSynchronize(st->e->ctx.stream) != cudaSuccess) rc = fail(B200_ECUDA, "generation stream failed");
+        st->loan.reset();
+        for (b200_slice * s : st->slices) s->owner = nullptr;
+        st->e->ctx.owner = nullptr;
+    }
+    stream_free(st);
+    return rc;
 }
 
 }  // extern "C"

@@ -291,6 +291,45 @@ int b200_score(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, co
 /* k_nll_rows on host logits [n_rows][n_vocab]: the kernel's test door, as b200_extra_sample is k_sample_rows'.
  * nll[k] as b200_score computes it for row k and target targets[k]; a target outside [0, n_vocab) is B200_EINVAL. */
 int b200_extra_nll(b200_extra_t * e, const float * logits, int n_rows, const int32_t * targets, double * nll);
+
+/* ---- generation streams: sessions join and leave between steps, ids reach the caller as they are drawn ----------------
+ * A stream runs the generation loop of b200_generate_greedy / b200_generate_sample over a chain of slices on one GPU (the
+ * same handle checks: contiguous layers, one device, no pipeline, the extra layers' n_embd), but open-ended:
+ *   - b200_stream_add queues a session.  Its whole prompt is one segment of one mixed pass at the next step with room for
+ *     it (never split: a segment's rows depend on its length); decode rows of other sessions may share that pass.  Every
+ *     later step feeds the session the id it drew last.  sp NULL: greedy (the argmax of the raw logits, first maximum
+ *     wins); else sampled with sp's temperature and penalty, key seeds[0], history (history_counts[0] ids) and draw
+ *     first_draw + j for its j-th id.  Greedy and sampled sessions with any settings share a stream.
+ *   - A session ends after its max_tokens-th id, after the first id in stop_ids (delivered), or with id -1 when its logits
+ *     have no distribution (see b200_generate_sample); the others go on.
+ *   - b200_stream_read returns (session, id) pairs in production order: it blocks until at least one is available and
+ *     writes at most cap; *n_out = 0 only when no session is active or queued.  The device runs up to `lookahead` steps
+ *     ahead of the oldest step not yet read; ids of steps past a session's end are dropped.  Nothing synchronises per
+ *     step: the draw kernel stores each id into a ring in mapped pinned memory that the host polls.
+ *   - Each session's ids equal b200_generate_greedy / b200_generate_sample of that session alone, with the same prompt,
+ *     settings and n_steps = its delivered count, whatever joined, ran beside it or left, at whichever step it joined.
+ *   - Positions: when a session ends, is cancelled, or the stream closes, its n_past on every slice is
+ *     old + n_prompt + delivered - 1 (old when nothing was delivered); delivered counts the ids b200_stream_read returned.
+ *     So a later call with prompt = [last id], history = the delivered ids and first_draw = their count continues the run.
+ *   - While a stream is open its handles belong to it: every other entry point on them (b200_session_n_past returns -1)
+ *     fails with B200_EINVAL naming the stream, except b200_slice_launch_count, b200_session_count, b200_extra_dims,
+ *     b200_extra_tokenize and b200_extra_token_text, which only read.  b200_stream_close gives them back.
+ *   - One stream is driven from one thread.
+ * b200_stream_open: max_rows = rows per step (<= the smallest n_ctx; <= 0: that n_ctx); lookahead <= 0: 4.  Sizes every
+ *   buffer once.  B200_EINVAL for bad handles or sizes, B200_ENODEV without a device.
+ * b200_stream_add: all-or-nothing.  B200_EINVAL: a session out of range or already in the stream, n_prompt < 1 or
+ *   > max_rows, max_tokens < 1, an id outside [0, n_vocab) in prompt, history or stop_ids, bad sampling settings (as
+ *   b200_generate_sample); B200_ECONTEXT: n_past + n_prompt + max_tokens - 1 > n_ctx on some slice.
+ * b200_stream_cancel: ends a queued or active session now (B200_EINVAL if it is neither); ids not yet read are dropped.
+ * b200_stream_close: ends every session, waits for the device and frees the stream. */
+typedef struct b200_stream b200_stream_t;
+int b200_stream_open(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int max_rows, int lookahead,
+                     b200_stream_t ** out);
+int b200_stream_add(b200_stream_t * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
+                    const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop);
+int b200_stream_read(b200_stream_t * st, int32_t * sessions, int32_t * ids, int cap, int * n_out);
+int b200_stream_cancel(b200_stream_t * st, int session);
+int b200_stream_close(b200_stream_t * st);
 /* llm.tokenize_prompt(path, prompt): BOS + sentencepiece-style merge (tensor_processor.cpp:1596-1714).
  * Returns the token count (may exceed cap; only cap are written) or a negative error. */
 int b200_extra_tokenize(b200_extra_t * e, const char * prompt, int32_t * out, int cap);
