@@ -161,12 +161,19 @@ float orc_dot_q8_0_q8_0(const uint8_t * w, const int8_t * aq, const uint16_t * a
     return hsum8(acc);
 }
 
+/* h2f of every fp16 bit pattern, for the inner loop below: the same values without the branches, which keeps the
+ * attention over contexts of tens of thousands of positions affordable */
+static float T_H2F[65536];
+__attribute__((constructor)) static void init_h2f_table(void) {
+    for (int i = 0; i < 65536; i++) T_H2F[i] = h2f((uint16_t) i);
+}
+
 /* x, y: fp16 bit patterns; y may be strided (V rows are walked over positions) */
 float orc_dot_f16(const uint16_t * x, long xs, const uint16_t * y, long ys, int n) {
     const int np = n & ~31;
     float acc[32] = {0};
     for (int i = 0; i < np; i += 32)
-        for (int s = 0; s < 32; s++) acc[s] = fmaf(h2f(x[(long)(i + s) * xs]), h2f(y[(long)(i + s) * ys]), acc[s]);
+        for (int s = 0; s < 32; s++) acc[s] = fmaf(T_H2F[x[(long)(i + s) * xs]], T_H2F[y[(long)(i + s) * ys]], acc[s]);
     float v[8];
     for (int l = 0; l < 8; l++) {                 /* x0+=x2; x1+=x3; x0+=x1 (GGML_F32x8_REDUCE, ARR=4) */
         float a0 = acc[l] + acc[16 + l], a1 = acc[8 + l] + acc[24 + l];
@@ -331,7 +338,8 @@ int orc_forward(orc_slice * s, const float * in, int N, float * out) {
         }
         #pragma omp parallel for schedule(static) collapse(2)
         for (int n = 0; n < N; n++) for (int h = 0; h < H; h++) {
-            uint16_t qh[512]; float sc[8192]; uint16_t ph[8192];
+            /* score rows on the heap: n_ctx is a load parameter and reaches tens of thousands of positions */
+            uint16_t qh[512]; float * sc = malloc((size_t) T * 4); uint16_t * ph = malloc((size_t) T * 2);
             for (int d = 0; d < D; d++) qh[d] = f2h(q[(size_t) n * E + h * D + d]);
             for (int t = 0; t < T; t++) {
                 float kq = orc_dot_f16(Kc + (size_t) t * E + h * D, 1, qh, 1, D) * kq_scale;
@@ -340,6 +348,7 @@ int orc_forward(orc_slice * s, const float * in, int N, float * out) {
             orc_softmax_row(sc, T);
             for (int t = 0; t < T; t++) ph[t] = f2h(sc[t]);
             for (int c = 0; c < D; c++) att[(size_t) n * E + h * D + c] = orc_dot_f16(Vc + h * D + c, E, ph, 1, T);
+            free(sc); free(ph);
         }
         matmul(s, L->wo, E, E, att, N, cur);
         for (size_t i = 0; i < (size_t) N * E; i++) ffin[i] = cur[i] + x[i];

@@ -162,7 +162,7 @@ int kq_forward(orc_slice * s, const int * types, const float * in, int N, float 
         }
         #pragma omp parallel for schedule(static) collapse(2)
         for (int n = 0; n < N; n++) for (int h = 0; h < H; h++) {
-            uint16_t qh[512]; float sc[8192]; uint16_t ph[8192];
+            uint16_t qh[512]; float * sc = malloc((size_t) T * 4); uint16_t * ph = malloc((size_t) T * 2);
             for (int d = 0; d < D; d++) qh[d] = f2h(q[(size_t) n * E + h * D + d]);
             for (int tt = 0; tt < T; tt++) {
                 float kq = orc_dot_f16(Kc + (size_t) tt * E + h * D, 1, qh, 1, D) * kq_scale;
@@ -171,6 +171,7 @@ int kq_forward(orc_slice * s, const int * types, const float * in, int N, float 
             orc_softmax_row(sc, T);
             for (int tt = 0; tt < T; tt++) ph[tt] = f2h(sc[tt]);
             for (int c = 0; c < D; c++) att[(size_t) n * E + h * D + c] = orc_dot_f16(Vc + h * D + c, E, ph, 1, T);
+            free(sc); free(ph);
         }
         kq_matmul(t[3], L->wo, E, E, att, N, cur);
         for (size_t i = 0; i < (size_t) N * E; i++) ffin[i] = cur[i] + x[i];

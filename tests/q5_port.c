@@ -107,7 +107,7 @@ int q5_forward(orc_slice * s, const float * in, int N, float * out) {
         }
         #pragma omp parallel for schedule(static) collapse(2)
         for (int n = 0; n < N; n++) for (int h = 0; h < H; h++) {
-            uint16_t qh[512]; float sc[8192]; uint16_t ph[8192];
+            uint16_t qh[512]; float * sc = malloc((size_t) T * 4); uint16_t * ph = malloc((size_t) T * 2);
             for (int d = 0; d < D; d++) qh[d] = f2h(q[(size_t) n * E + h * D + d]);
             for (int t = 0; t < T; t++) {
                 float kq = orc_dot_f16(Kc + (size_t) t * E + h * D, 1, qh, 1, D) * kq_scale;
@@ -116,6 +116,7 @@ int q5_forward(orc_slice * s, const float * in, int N, float * out) {
             orc_softmax_row(sc, T);
             for (int t = 0; t < T; t++) ph[t] = f2h(sc[t]);
             for (int c = 0; c < D; c++) att[(size_t) n * E + h * D + c] = orc_dot_f16(Vc + h * D + c, E, ph, 1, T);
+            free(sc); free(ph);
         }
         q5_matmul(s, L->wo, E, E, att, N, cur);
         for (size_t i = 0; i < (size_t) N * E; i++) ffin[i] = cur[i] + x[i];
