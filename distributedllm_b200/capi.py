@@ -29,7 +29,8 @@ class SliceInfo(C.Structure):
 class Sampling(C.Structure):
     """b200_sampling_t."""
     _fields_ = [("temperature", C.c_double), ("repeat_penalty", C.c_double), ("seeds", C.c_void_p),
-                ("first_draw", C.c_int64), ("history", C.c_void_p), ("history_counts", C.c_void_p)]
+                ("first_draw", C.c_int64), ("history", C.c_void_p), ("history_counts", C.c_void_p),
+                ("top_k", C.c_int32), ("top_p", C.c_double)]
 
 
 _lib: Optional[C.CDLL] = None
@@ -344,11 +345,12 @@ class Extra:
         return C.string_at(p, n.value).decode("utf-8", "replace")
 
     def sample(self, logits: np.ndarray, temperature: float, repeat_penalty: float, seeds, first_draw: int = 0,
-               history=None) -> np.ndarray:
+               history=None, top_k: int = 0, top_p: float = 0.0) -> np.ndarray:
         """The client's Sampler on the device (b200_extra_sample): row k of [n][n_vocab] logits takes draw first_draw of
-        the Philox stream keyed seeds[k], with history[k] (ids already sampled) penalised.  -> [n] ids."""
+        the Philox stream keyed seeds[k], with history[k] (ids already sampled) penalised, truncated to top_k / top_p
+        (0: off).  -> [n] ids."""
         x = np.ascontiguousarray(logits, dtype=np.float32).reshape(-1, self.n_vocab)
-        sp, keep = _sampling(len(x), temperature, repeat_penalty, seeds, first_draw, history)
+        sp, keep = _sampling(len(x), temperature, repeat_penalty, seeds, first_draw, history, top_k, top_p)
         out = np.zeros(len(x), np.int32)
         check(lib().b200_extra_sample(self._h, _ptr(x), len(x), C.byref(sp), _ptr(out)))
         return out
@@ -392,12 +394,24 @@ def generate_greedy(slices, extra: Extra, sessions, prompts, n_steps: int) -> np
     return out
 
 
-def _sampling(n: int, temperature: float, repeat_penalty: float, seeds, first_draw: int, history):
+def _truncation(top_k, top_p):
+    """top_k as an int in [0, 2^31), top_p as a float >= 0 (inf allowed: no cut), or ValueError / TypeError."""
+    top_k = _int("top_k", top_k, 0, 2 ** 31 - 1)
+    if isinstance(top_p, (bool, np.bool_)) or not isinstance(top_p, (int, float, np.integer, np.floating)):
+        raise TypeError("top_p must be a number, got %r" % (top_p,))
+    top_p = float(top_p)
+    if not top_p >= 0:
+        raise ValueError("top_p must be >= 0 and not NaN, got %r" % top_p)
+    return top_k, top_p
+
+
+def _sampling(n: int, temperature: float, repeat_penalty: float, seeds, first_draw: int, history, top_k=0, top_p=0.0):
     """-> (b200_sampling_t, the arrays it points into)."""
+    top_k, top_p = _truncation(top_k, top_p)
     keys = np.ascontiguousarray([int(k) for k in seeds], dtype=np.uint64)
     if len(keys) != n:
         raise ValueError("need one seed per session (%d), got %d" % (n, len(keys)))
-    sp = Sampling(float(temperature), float(repeat_penalty), keys.ctypes.data, int(first_draw), None, None)
+    sp = Sampling(float(temperature), float(repeat_penalty), keys.ctypes.data, int(first_draw), None, None, top_k, top_p)
     keep = [keys]
     if history is not None:
         if len(history) != n:
@@ -410,14 +424,15 @@ def _sampling(n: int, temperature: float, repeat_penalty: float, seeds, first_dr
 
 
 def generate_sample(slices, extra: Extra, sessions, prompts, n_steps: int, temperature: float, repeat_penalty: float,
-                    seeds, first_draw: int = 0, history=None) -> np.ndarray:
+                    seeds, first_draw: int = 0, history=None, top_k: int = 0, top_p: float = 0.0) -> np.ndarray:
     """Sampled generation on the device (b200_generate_sample): generate_greedy's loop with the client's Sampler in place
     of the argmax.  Session sessions[k] draws from numpy.random.Philox(key=seeds[k]) starting at draw first_draw, with
-    history[k] (ids it sampled before) penalised.  -> [n_steps][n_seq] ids."""
+    history[k] (ids it sampled before) penalised and every row truncated to top_k / top_p (0: off).
+    -> [n_steps][n_seq] ids."""
     ids = np.ascontiguousarray(sessions, dtype=np.int32)
     if len(prompts) != len(ids):
         raise ValueError("need one prompt per listed session")
-    sp, keep = _sampling(len(ids), temperature, repeat_penalty, seeds, first_draw, history)
+    sp, keep = _sampling(len(ids), temperature, repeat_penalty, seeds, first_draw, history, top_k, top_p)
     counts = np.array([len(p) for p in prompts], np.int32)
     toks = np.ascontiguousarray(np.concatenate([np.asarray(p, np.int64) for p in prompts]) if len(prompts) else [],
                                 dtype=np.int32)
@@ -491,10 +506,11 @@ class Stream:
         return self._h
 
     def add(self, session: int, prompt, max_tokens: int, temperature: Optional[float] = None, repeat_penalty: float = 1.1,
-            seed: int = 0, first_draw: int = 0, history=None, stop_ids=()) -> None:
+            seed: int = 0, first_draw: int = 0, history=None, stop_ids=(), top_k: int = 0, top_p: float = 0.0) -> None:
         """Queue `session` with `prompt` (token ids) for at most max_tokens ids.  temperature None: greedy (the argmax of
         the raw logits); else the client's Sampler with repeat_penalty on numpy.random.Philox(key=seed), starting at draw
-        first_draw, with history (ids sampled before) penalised.  The session ends after the first id in stop_ids."""
+        first_draw, with history (ids sampled before) penalised, truncated to top_k / top_p (0: off).  The session ends
+        after the first id in stop_ids."""
         session = _int("session", session, 0, 2 ** 31 - 1)
         p = _ids("prompt", prompt, self.n_vocab, 1)
         max_tokens = _int("max_tokens", max_tokens, 1, 2 ** 31 - 1)
@@ -510,9 +526,9 @@ class Stream:
             first_draw = _int("first_draw", first_draw, 0, 2 ** 63 - 1)
             if history is not None:
                 history = [_ids("history", history, self.n_vocab, 0)[:len(history)].tolist()]
-            sp, keep = _sampling(1, t, rp, [seed], first_draw, history)
-        elif history is not None or first_draw:
-            raise ValueError("history and first_draw apply to sampled sessions (give a temperature)")
+            sp, keep = _sampling(1, t, rp, [seed], first_draw, history, top_k, top_p)
+        elif history is not None or first_draw or _truncation(top_k, top_p) != (0, 0.0):
+            raise ValueError("history, first_draw, top_k and top_p apply to sampled sessions (give a temperature)")
         check(lib().b200_stream_add(self._handle(), session, _ptr(p), len(prompt), max_tokens,
                                     None if sp is None else C.byref(sp), _ptr(stops), len(stop_ids)))
 

@@ -56,19 +56,40 @@ def _softmax(x: np.ndarray, axis=-1) -> np.ndarray:
 
 
 class Sampler:
-    def __init__(self, temperature=0.7, repeat_penalty=1.1, rng=None):
+    """The reference's sampler, plus llama.cpp's top-k and top-p truncation (off when both are None, which runs the
+    reference's arithmetic unchanged).  Truncation ranks the ids by the scaled logits y descending (equal y: lower id
+    first), keeps the first top_k of them (0 or None: all), then within those keeps an id iff the probability ranked
+    strictly before it is < top_p times their total (0, None or >= 1: no cut; the top id is always kept), and draws from
+    the kept probabilities with the same single random() and the same id-order rule."""
+
+    def __init__(self, temperature=0.7, repeat_penalty=1.1, rng=None, top_k=None, top_p=None):
         self.T = temperature
         self.penalty = repeat_penalty
         self.previous_ids: List[int] = []
         self.eps = 10 ** (-5)
         self.rng = rng or np.random
+        self.top_k = top_k
+        self.top_p = top_p
 
     def __call__(self, logits) -> int:
         logits = np.array(logits)
         ids = np.arange(len(logits))
         seen = np.isin(ids, self.previous_ids)
         logits = logits / ((seen * self.penalty + ~seen) * (self.T + self.eps))
-        token_id = int(self.rng.choice(ids, p=_softmax(logits)))
+        if self.top_k is None and self.top_p is None:
+            token_id = int(self.rng.choice(ids, p=_softmax(logits)))
+        else:
+            p = _softmax(logits)
+            order = np.lexsort((ids, -logits))                  # y descending, lower id first
+            K = order[:self.top_k] if self.top_k else order
+            keep = np.zeros(len(ids), bool)
+            keep[K] = True
+            if self.top_p and self.top_p < 1:
+                pk = p[K]
+                before = np.concatenate(([0.0], np.cumsum(pk)[:-1]))
+                keep[K[before >= self.top_p * pk.sum()]] = False
+            p = np.where(keep, p, 0.0)
+            token_id = int(self.rng.choice(ids, p=p / p.sum()))
         self.previous_ids.append(token_id)
         return token_id
 
@@ -85,13 +106,14 @@ class DistributedLLM:
         self.wire = wire
         self.llm = import_llm()
 
-    def generate(self, prompt, max_steps=200, temperature=0.0, repeat_penalty=1.1, rng=None):
+    def generate(self, prompt, max_steps=200, temperature=0.0, repeat_penalty=1.1, rng=None, top_k=None, top_p=None):
         """rng: the Sampler's random generator (default numpy's global one, as the reference);
-        numpy.random.Generator(numpy.random.Philox(key=seed)) gives LocalPipeline.generate's ids for that seed."""
+        numpy.random.Generator(numpy.random.Philox(key=seed)) gives LocalPipeline.generate's ids for that seed.
+        top_k / top_p: the Sampler's truncation (None: off)."""
         self.clear_context()
         extra = self.extra_layers_path
         tokens = self.llm.tokenize_prompt(extra, prompt)
-        sampler = Sampler(temperature, repeat_penalty, rng=rng)
+        sampler = Sampler(temperature, repeat_penalty, rng=rng, top_k=top_k, top_p=top_p)
         for _ in range(max_steps):
             emb = self.propagate_tensor(self.llm.prepare_embeddings(extra, tokens))
             token_id = sampler(self.llm.get_logits(extra, emb, False))
@@ -180,7 +202,8 @@ class LocalPipeline:
         return self.capi.generate_greedy(self.slices, extra, [0], [tokens], max_steps)[:, 0].tolist()
 
     def generate(self, extra_path: str, prompt: str, max_steps: int = 200, temperature: float = 0.0,
-                 repeat_penalty: float = 1.1, seed: int = None, stop_at_eos: bool = False):
+                 repeat_penalty: float = 1.1, seed: int = None, stop_at_eos: bool = False, top_k: int = None,
+                 top_p: float = None):
         """DistributedLLM.generate on this box: clear the contexts, tokenize, then up to max_steps steps of the client's
         Sampler, all on the GPU with no host round trip between tokens (a one-session capi.Stream).  Yields each token
         string as soon as its id is drawn; leaving the loop early cancels the steps that remain, and the slices' n_past
@@ -188,7 +211,8 @@ class LocalPipeline:
         DistributedLLM.generate(..., rng=numpy.random.Generator(numpy.random.Philox(key=seed))) yields the same strings.
         seed=None draws a key from numpy's global generator, so unseeded runs vary as the reference's do.
         stop_at_eos=True ends the run after the end-of-sequence id (EOS_ID, yielded); the default runs max_steps steps,
-        as the reference does.  Needs every slice on one device."""
+        as the reference does.  top_k / top_p truncate each draw as client.Sampler does (None: off).  Needs every slice
+        on one device."""
         extra = self._device_extra(extra_path, "sampled generation")
         if seed is None:
             seed = int(np.random.randint(0, 2 ** 64, dtype=np.uint64))
@@ -197,7 +221,8 @@ class LocalPipeline:
         if max_steps < 1:
             return
         with self.capi.Stream(self.slices, extra) as st:
-            st.add(0, tokens, max_steps, temperature, repeat_penalty, seed, stop_ids=[EOS_ID] if stop_at_eos else ())
+            st.add(0, tokens, max_steps, temperature, repeat_penalty, seed, stop_ids=[EOS_ID] if stop_at_eos else (),
+                   top_k=top_k or 0, top_p=top_p or 0.0)
             for j, (_, token_id) in enumerate(st):
                 if token_id < 0:
                     raise self.capi.B200Error(1, "step %d: the logits hold a NaN or +inf, are all -inf or overflow "

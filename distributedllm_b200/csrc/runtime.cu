@@ -2154,11 +2154,181 @@ struct SampleArgs {
     uint32_t * pen;                  // [rows][(n + 31) / 32]: bit i of row k = id i is in session k's prev
     int32_t * tok, * ids;            // the chosen id -> tok[k] (the next step's embedding reads it) and ids[k]
     int * bad; int bad_base;         // a row without a distribution: id -1, atomicMin(bad, bad_base + k)
+    int top_k; double top_p;         // truncation; 0 = off
 };
 
 __device__ __forceinline__ double sample_weight(double dt, double dp, const float * x, const uint32_t * bits, int i, double m) {
     const double d = (bits[i >> 5] >> (i & 31)) & 1u ? dp : dt;
     return exp(__dsub_rn(__ddiv_rn((double) x[i], d), m));
+}
+
+// ---- sample_row's truncation stage (top-k / top-p): the kept ids are a prefix of the ranking (y descending, equal y lower
+// id first), so one threshold per row describes them: id i is kept iff key_i > tau, or key_i == tau and i <= c.
+
+__device__ __forceinline__ double sample_y(double dt, double dp, const float * x, const uint32_t * bits, int i) {
+    const double d = (bits[i >> 5] >> (i & 31)) & 1u ? dp : dt;
+    return __ddiv_rn((double) x[i], d);
+}
+
+// y as an unsigned integer in the order of y; -0 is folded onto +0, so equal y give equal keys.  (NaN rows never get here.)
+__device__ __forceinline__ unsigned long long order_key(double y) {
+    const unsigned long long b = (unsigned long long) __double_as_longlong(__dadd_rn(y, 0.0));
+    return (b >> 63) ? ~b : b | 0x8000000000000000ull;
+}
+
+// sample_weight for a truncated row: the same arithmetic for a kept id, 0 for a dropped one.
+__device__ __forceinline__ double kept_weight(double dt, double dp, const float * x, const uint32_t * bits, int i, double m,
+                                              unsigned long long tau, int c) {
+    const double y = sample_y(dt, dp, x, bits, i);
+    const unsigned long long key = order_key(y);
+    return key > tau || (key == tau && i <= c) ? exp(__dsub_rn(y, m)) : 0.0;
+}
+
+// Exclusive prefix of v over the block in thread order; *total = the block's sum.
+__device__ __forceinline__ int block_scan_excl(int v, int * total) {
+    __shared__ int s_w[33];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
+    int in = v;
+    for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, in, o); if (lane >= o) in += u; }
+    if (lane == 31) s_w[wid] = in;
+    __syncthreads();
+    if (wid == 0) {
+        const int w = lane < nwarp ? s_w[lane] : 0;
+        int wi = w;
+        for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, wi, o); if (lane >= o) wi += u; }
+        s_w[lane] = wi - w;
+        if (lane == 31) s_w[32] = wi;
+    }
+    __syncthreads();
+    const int r = s_w[wid] + in - v;
+    *total = s_w[32];
+    __syncthreads();                                    // s_w is free for the next call
+    return r;
+}
+
+constexpr int kTruncCap = 1024;                         // candidates held on chip: one per thread of the 1024-thread block
+struct TruncShared {
+    unsigned long long key[kTruncCap], w[kTruncCap];    // the compacted candidates, in id order
+    int id[kTruncCap];
+    unsigned cnt[256]; unsigned long long mass[256];    // one level's histograms
+    unsigned long long target, above_w, tau;            // block-uniform state of trunc_cut
+    unsigned above_n, bin_n; int bin, ncand, c;
+};
+
+// One cut of a row's ranking -> (S.tau, S.c): the ranked id at which the running count reaches k (top-k), or at which the
+// running weight within K first reaches ceil(p * S_K) (top-p; K = the ids kept by the cut (tk, ck) when kon).  Weights
+// are fixed point, W_i = round(w_i * scale) with scale = 2^(63 - floor(log2 n)), so no sum can overflow 64 bits and any
+// sum of them is exact whatever the order: counts and weights are shared-memory integer atomics.  The rounding error of a
+// sum is at most n / (2 * scale), which relative to S_K >= 1 (the top id's weight is 1) is <= n * 2^(floor(log2 n) - 64).
+// An MSB-first radix descent over the 64-bit keys, 8 bits a level: each level histograms the ids whose key matches the
+// digits found so far, and warp 0 walks the bins from the top to the one where the running total reaches the target.
+// Once the matching ids fit kTruncCap they are compacted on chip in id order (an ordered block scan) and the remaining
+// levels read them there instead of the row.  After the last level the cut lies in a run of equal keys tau (equal y, so
+// equal W): it takes the lowest j ids of the run, found with the ordered scan again.
+__device__ __forceinline__ void trunc_cut(const float * x, int n, const uint32_t * bits, double dt, double dp, double m,
+                                          double scale, bool by_mass, unsigned long long k, double p, bool kon,
+                                          unsigned long long tk, int ck, TruncShared & S) {
+    const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
+    const int C = (n + blockDim.x - 1) / blockDim.x, i0 = min(n, t * C), i1 = min(n, i0 + C);
+    if (t == 0) { S.target = k; S.above_w = 0; S.above_n = 0; }
+    bool onchip = false;
+    unsigned long long prefix = 0;
+    for (int shift = 56; shift >= 0; shift -= 8) {
+        const int hs = shift + 8;                       // the bits above this digit must equal prefix's
+        for (int b = t; b < 256; b += blockDim.x) { S.cnt[b] = 0; S.mass[b] = 0; }
+        __syncthreads();
+        if (onchip) {
+            if (t < S.ncand) {
+                const unsigned long long key = S.key[t];
+                if (hs == 64 || (key >> hs) == (prefix >> hs)) {
+                    const int dig = (int)(key >> shift) & 255;
+                    atomicAdd(&S.cnt[dig], 1u);
+                    if (by_mass) atomicAdd(&S.mass[dig], S.w[t]);
+                }
+            }
+        } else {
+            for (int i = i0; i < i1; i++) {
+                const double y = sample_y(dt, dp, x, bits, i);
+                const unsigned long long key = order_key(y);
+                if ((hs < 64 && (key >> hs) != (prefix >> hs)) || (kon && (key < tk || (key == tk && i > ck)))) continue;
+                const int dig = (int)(key >> shift) & 255;
+                atomicAdd(&S.cnt[dig], 1u);
+                if (by_mass) atomicAdd(&S.mass[dig], __double2ull_rn(__dmul_rn(exp(__dsub_rn(y, m)), scale)));
+            }
+        }
+        __syncthreads();
+        if (wid == 0) {                                 // lane l sums bins 255 - 8l .. 248 - 8l, then a scan from the top
+            unsigned cn = 0; unsigned long long ms = 0;
+            for (int j = 0; j < 8; j++) { cn += S.cnt[255 - 8 * lane - j]; ms += S.mass[255 - 8 * lane - j]; }
+            unsigned ci = cn; unsigned long long mi = ms;
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned a = __shfl_up_sync(0xffffffffu, ci, o);
+                const unsigned long long b = __shfl_up_sync(0xffffffffu, mi, o);
+                if (lane >= o) { ci += a; mi += b; }
+            }
+            unsigned long long target = S.target;
+            if (by_mass && shift == 56) {               // the first level holds all of K: S_K, and the target ceil(p S_K)
+                const unsigned long long SK = __shfl_sync(0xffffffffu, mi, 31);
+                target = min(max(__double2ull_ru(__dmul_rn(p, (double) SK)), 1ull), SK);
+            }
+            const unsigned long long aw = S.above_w; const unsigned an = S.above_n;
+            const unsigned hit = __ballot_sync(0xffffffffu, by_mass ? aw + mi >= target : an + ci >= target);
+            const int L = hit ? __ffs(hit) - 1 : 31;
+            if (lane == L) {
+                unsigned long long w = aw + mi - ms; unsigned c = an + ci - cn;
+                int b = 255 - 8 * lane;
+                for (int j = 0; j < 7; j++, b--) {
+                    if (by_mass ? w + S.mass[b] >= target : c + S.cnt[b] >= target) break;
+                    w += S.mass[b]; c += S.cnt[b];
+                }
+                S.bin = b; S.above_w = w; S.above_n = c; S.bin_n = S.cnt[b]; S.target = target;
+            }
+        }
+        __syncthreads();
+        prefix |= (unsigned long long) S.bin << shift;
+        if (!onchip && shift > 0 && S.bin_n <= (unsigned) kTruncCap) {   // compact the candidates on chip, in id order
+            int mine = 0;
+            for (int i = i0; i < i1; i++) {
+                const unsigned long long key = order_key(sample_y(dt, dp, x, bits, i));
+                mine += (key >> shift) == (prefix >> shift) && !(kon && (key < tk || (key == tk && i > ck)));
+            }
+            int total;
+            int at = block_scan_excl(mine, &total);
+            for (int i = i0; i < i1 && mine; i++) {
+                const double y = sample_y(dt, dp, x, bits, i);
+                const unsigned long long key = order_key(y);
+                if ((key >> shift) != (prefix >> shift) || (kon && (key < tk || (key == tk && i > ck)))) continue;
+                S.key[at] = key; S.id[at] = i;
+                S.w[at] = by_mass ? __double2ull_rn(__dmul_rn(exp(__dsub_rn(y, m)), scale)) : 0ull;
+                at++; mine--;
+            }
+            if (t == 0) S.ncand = total;
+            __syncthreads();
+            onchip = true;
+        }
+    }
+    // the run of keys == prefix holds the cut: the lowest j of its ids are kept
+    unsigned long long j;
+    if (by_mass) {
+        const unsigned long long W = S.mass[S.bin] / S.bin_n, d = S.target - S.above_w;
+        j = W ? d / W + (d % W != 0) : 1;
+    } else {
+        j = S.target - S.above_n;
+    }
+    if (t == 0) { S.tau = prefix; S.c = n - 1; }
+    int mine = 0;
+    if (onchip) mine = t < S.ncand && S.key[t] == prefix;
+    else
+        for (int i = i0; i < i1; i++) mine += order_key(sample_y(dt, dp, x, bits, i)) == prefix;
+    int total;
+    const int at = block_scan_excl(mine, &total);
+    if ((unsigned long long) at < j && j <= (unsigned long long)(at + mine)) {
+        if (onchip) S.c = S.id[t];
+        else
+            for (int i = i0, r = at; i < i1; i++)
+                if (order_key(sample_y(dt, dp, x, bits, i)) == prefix && ++r == (int) j) { S.c = i; break; }
+    }
+    __syncthreads();
 }
 
 // The client's Sampler (cli_api/common.py:64-86) on one row x of n logits, for a whole block: divisors dt / dp, penalty
@@ -2173,11 +2343,16 @@ __device__ __forceinline__ double sample_weight(double dt, double dp, const floa
 //      the draw; warp 0 re-walks that chunk in order from O_t and picks the first id whose running sum passes u*S,
 //      falling back to the chunk's last id of positive weight.  An id of weight 0 never moves the sum, so it is never
 //      picked.  The row's logits are read from L2 in each pass.
+// With truncation on (0 < top_k < n, or 0 < top_p < 1: a block-uniform branch), a stage between 1 and 2 finds the row's
+// threshold (tau, c) with trunc_cut -- top-k first, then top-p within K -- and steps 2 and 3 use weight 0 for every id
+// it drops, in the same chunks and order.  So dropping ids whose weight is already 0 changes no bit.  With truncation
+// off, steps 2 and 3 are the untruncated arithmetic.
 __device__ __forceinline__ int sample_row(const float * x, int n, const uint32_t * bits, double dt, double dp, uint64_t seed,
-                                          long long draw) {
+                                          long long draw, int top_k, double top_p) {
     __shared__ float smf[32], smp[32];
     __shared__ double swt[32], swo[32], s_m, s_u, s_total, s_target, s_o;
     __shared__ int s_chunk;
+    __shared__ TruncShared s_trunc;
     const int t = threadIdx.x, lane = t & 31, wid = t >> 5, nwarp = blockDim.x >> 5;
     const int C = (n + blockDim.x - 1) / blockDim.x, i0 = min(n, t * C), i1 = min(n, i0 + C);
     float mf = -INFINITY, mp = -INFINITY; bool nan = false;
@@ -2205,8 +2380,23 @@ __device__ __forceinline__ int sample_row(const float * x, int n, const uint32_t
     __syncthreads();
     const double m = s_m;
     if (any_nan || !isfinite(m)) return -1;
+    const bool trunc = (top_k > 0 && top_k < n) || (top_p > 0.0 && top_p < 1.0);
+    unsigned long long tau = 0; int cut = 0;
+    if (trunc) {
+        const double scale = ldexp(1.0, 63 - (31 - __clz(n)));
+        bool kon = false;
+        if (top_k > 0 && top_k < n) {
+            trunc_cut(x, n, bits, dt, dp, m, scale, false, (unsigned long long) top_k, 0.0, false, 0, 0, s_trunc);
+            kon = true; tau = s_trunc.tau; cut = s_trunc.c;
+        }
+        if (top_p > 0.0 && top_p < 1.0) {
+            trunc_cut(x, n, bits, dt, dp, m, scale, true, 0, top_p, kon, tau, cut, s_trunc);
+            tau = s_trunc.tau; cut = s_trunc.c;
+        }
+    }
     double tot = 0.0;
-    for (int i = i0; i < i1; i++) tot = __dadd_rn(tot, sample_weight(dt, dp, x, bits, i, m));
+    if (trunc) for (int i = i0; i < i1; i++) tot = __dadd_rn(tot, kept_weight(dt, dp, x, bits, i, m, tau, cut));
+    else       for (int i = i0; i < i1; i++) tot = __dadd_rn(tot, sample_weight(dt, dp, x, bits, i, m));
     const double P = warp_prefix_ordered(tot), Pin = __dadd_rn(P, tot);
     if (lane == 31) swt[wid] = Pin;
     __syncthreads();
@@ -2227,7 +2417,7 @@ __device__ __forceinline__ int sample_row(const float * x, int n, const uint32_t
     double r = s_o; int id = -1, last = -1;
     for (int b = j0; b < j1 && id < 0; b += 32) {
         const int i = b + lane;
-        const double e = i < j1 ? sample_weight(dt, dp, x, bits, i, m) : 0.0;
+        const double e = i >= j1 ? 0.0 : trunc ? kept_weight(dt, dp, x, bits, i, m, tau, cut) : sample_weight(dt, dp, x, bits, i, m);
         double q = r;                                  // r + e_b + ... + e_i, added in index order
         for (int j = 0; j < 32; j++) { const double w = __shfl_sync(0xffffffffu, e, j); if (j <= lane) q = __dadd_rn(q, w); }
         const unsigned hit = __ballot_sync(0xffffffffu, i < j1 && q > target);
@@ -2243,7 +2433,7 @@ __device__ __forceinline__ int sample_row(const float * x, int n, const uint32_t
 __global__ void __launch_bounds__(1024) k_sample_rows(SampleArgs a) {
     const int k = blockIdx.x;
     uint32_t * bits = a.pen + (size_t) k * ((a.n + 31) >> 5);
-    const int id = sample_row(a.logits + (size_t) k * a.n, a.n, bits, a.dt, a.dp, a.seeds[k], a.draw);
+    const int id = sample_row(a.logits + (size_t) k * a.n, a.n, bits, a.dt, a.dp, a.seeds[k], a.draw, a.top_k, a.top_p);
     if (threadIdx.x != 0) return;
     a.tok[k] = id; a.ids[k] = id;
     if (id < 0) atomicMin(a.bad, a.bad_base + k);
@@ -2251,7 +2441,7 @@ __global__ void __launch_bounds__(1024) k_sample_rows(SampleArgs a) {
 }
 
 // ---- generation streams (b200_stream_*): the sampler's state lives in per-session slots, and a step's rows name their slot
-struct StreamSlot { uint64_t seed; double dt, dp; int sampled; };   // device table, one per session
+struct StreamSlot { uint64_t seed; double dt, dp; int sampled, top_k; double top_p; };   // device table, one per session
 struct StreamRow { long long draw; int slot, gather; };              // per step, in mapped pinned memory: draw index, slot,
                                                                     // and the session's last row in the pass
 
@@ -2289,7 +2479,7 @@ __global__ void __launch_bounds__(1024) k_stream_draw(const float * logits, int 
     const StreamSlot sl = slots[slot];
     const float * x = logits + (size_t) k * n;
     uint32_t * bits = pen + (size_t) slot * ((n + 31) >> 5);
-    const int id = sl.sampled ? sample_row(x, n, bits, sl.dt, sl.dp, sl.seed, s_row.draw) : argmax_row(x, n);
+    const int id = sl.sampled ? sample_row(x, n, bits, sl.dt, sl.dp, sl.seed, s_row.draw, sl.top_k, sl.top_p) : argmax_row(x, n);
     if (threadIdx.x != 0) return;
     if (sl.sampled && id >= 0) bits[id >> 5] |= 1u << (id & 31);
     last[slot] = id;
@@ -2611,6 +2801,8 @@ static int sample_check(const b200_sampling_t * sp, int n_seq, int n_vocab) {
     if (!(sp->repeat_penalty > 0) || !std::isfinite(sp->repeat_penalty))
         return fail(B200_EINVAL, "repeat penalty must be finite and > 0 (got %g)", sp->repeat_penalty);
     if (sp->first_draw < 0) return fail(B200_EINVAL, "first_draw must be >= 0 (got %lld)", (long long) sp->first_draw);
+    if (sp->top_k < 0) return fail(B200_EINVAL, "top_k must be >= 0 (got %d)", (int) sp->top_k);
+    if (!(sp->top_p >= 0)) return fail(B200_EINVAL, "top_p must be >= 0 and not NaN (got %g)", sp->top_p);
     if (!sp->history) return 0;
     if (!sp->history_counts) return fail(B200_EINVAL, "a history needs history_counts");
     for (int k = 0, at = 0; k < n_seq; k++) {
@@ -2644,7 +2836,7 @@ static int sample_start(b200_extra * e, const b200_sampling_t * sp, int n_seq) {
 static int sample_launch(b200_extra * e, const b200_sampling_t * sp, int rows, int step, int32_t * ids) {
     const double dt = sp->temperature + 1e-5;
     SampleArgs a{e->d_logits, e->n_vocab, dt, sp->repeat_penalty * dt, e->d_seeds, (long long) sp->first_draw + step,
-                 e->d_pen, e->d_tok, ids, e->d_bad, step * rows};
+                 e->d_pen, e->d_tok, ids, e->d_bad, step * rows, sp->top_k, sp->top_p};
     k_sample_rows<<<rows, 1024, 0, e->ctx.stream>>>(a);
     B200_CUDA(cudaGetLastError());
     e->ctx.launches++;
@@ -3149,7 +3341,8 @@ int b200_stream_add(b200_stream_t * st, int session, const int32_t * prompt, int
         return fail(B200_EINVAL, "session %d: a prompt of %d ids exceeds max_rows %d (a prompt is never split)", session, n_prompt, st->max_rows);
     // the slot's sampler state, in stream order behind any step still running for an earlier stay of the session
     const double dt = sp ? sp->temperature + 1e-5 : 1.0;
-    const StreamSlot slot{sp ? sp->seeds[0] : 0, dt, sp ? sp->repeat_penalty * dt : 1.0, sp ? 1 : 0};
+    const StreamSlot slot{sp ? sp->seeds[0] : 0, dt, sp ? sp->repeat_penalty * dt : 1.0, sp ? 1 : 0, sp ? (int) sp->top_k : 0,
+                          sp ? sp->top_p : 0.0};
     cudaStream_t cs = st->e->ctx.stream;
     B200_CUDA(cudaMemcpyAsync(st->d_slots + session, &slot, sizeof slot, cudaMemcpyHostToDevice, cs));
     if (sp) {

@@ -250,6 +250,8 @@ typedef struct b200_sampling {
     int64_t first_draw;          /* draws each stream has already given (0 = fresh generator) */
     const int32_t * history;     /* NULL, or ids already sampled, grouped by session: history_counts[k] for session k */
     const int * history_counts;
+    int32_t top_k;               /* >= 0; 0 (or >= n_vocab): no top-k cut */
+    double top_p;                /* >= 0, not NaN; 0 (or >= 1): no top-p cut */
 } b200_sampling_t;
 /* Sampled generation on the device: b200_generate_greedy's loop with the client's Sampler in place of the argmax.
  * For each row of logits x, with prev = the session's history plus the ids this call has drawn for it so far:
@@ -260,10 +262,24 @@ typedef struct b200_sampling {
  * draw; ids can differ from it only where u lies within ~1e-12 of a CDF boundary (the last ulp of exp and the summation
  * order).  On the device there is no such freedom: a session's ids are the same alone, in a batch, or split across calls
  * (a call with the earlier ids as history, first_draw = their count and the last id as prompt continues another).
- * An id whose probability is exactly 0 is never chosen.  Everything else, including the error codes, is as
- * b200_generate_greedy; B200_EINVAL also covers a null sp or seeds, temperature < 0 or not finite, repeat_penalty <= 0
- * or not finite, first_draw < 0, history without history_counts, a history count < 0 and a history id outside
- * [0, n_vocab), and those leave every position unchanged.
+ * An id whose probability is exactly 0 is never chosen.
+ * Truncation (top_k, top_p; llama.cpp's order and rule), applied per row before the draw:
+ *   1. rank the ids by y descending, equal y lower id first (y, not x: the penalty can reorder ids);
+ *   2. top-k: K = the first top_k ranked ids (all ids when top_k is 0 or >= n_vocab);
+ *   3. top-p: with w_i = exp(y_i - max y) and S_K = sum of w over K, an id of K is kept iff the weight ranked strictly
+ *      before it within K is < top_p * S_K; so the top-ranked id is always kept (no cut when top_p is 0 or >= 1);
+ *   4. the draw above, unchanged (same u, same id order), on the weights w_i * [i kept].
+ * The kept set is a prefix of the ranking, so on the device it is one threshold per row: a key tau (an order-preserving
+ * transform of y) and an id cut c; i is kept iff key_i > tau or key_i == tau and i <= c.  The top-p masses are sums of
+ * w in fixed point (exact integers, so they do not depend on the order of summation) with an error of at most
+ * n_vocab * 2^(floor(log2 n_vocab) - 64) * S_K (2.8e-11 S_K at 32000 ids).  With both off the call runs the untruncated
+ * arithmetic; exclusions of ids whose weight is already 0 change no bit.  client.Sampler(T, rp, rng, top_k, top_p) is
+ * the host twin; beyond the draw's own ~1e-12, its ids may differ only where its mass before the last kept id or the
+ * first dropped one lies within ~1e-10 S_K of top_p * S_K.
+ * Everything else, including the error codes, is as b200_generate_greedy; B200_EINVAL also covers a null sp or seeds,
+ * temperature < 0 or not finite, repeat_penalty <= 0 or not finite, first_draw < 0, history without history_counts, a
+ * history count < 0, a history id outside [0, n_vocab), top_k < 0 and top_p NaN or < 0, and those leave every position
+ * unchanged.
  * A row whose logits hold a NaN or +inf, are all -inf, or scale past the float64 range has no distribution (numpy
  * raises "probabilities contain NaN"): its id is -1, the rest of the loop still runs, and the call returns B200_EINVAL
  * naming the first such step and session.  The positions HAVE moved by then, as after a successful call. */
@@ -298,8 +314,8 @@ int b200_extra_nll(b200_extra_t * e, const float * logits, int n_rows, const int
  *   - b200_stream_add queues a session.  Its whole prompt is one segment of one mixed pass at the next step with room for
  *     it (never split: a segment's rows depend on its length); decode rows of other sessions may share that pass.  Every
  *     later step feeds the session the id it drew last.  sp NULL: greedy (the argmax of the raw logits, first maximum
- *     wins); else sampled with sp's temperature and penalty, key seeds[0], history (history_counts[0] ids) and draw
- *     first_draw + j for its j-th id.  Greedy and sampled sessions with any settings share a stream.
+ *     wins); else sampled with sp's temperature, penalty, top_k and top_p, key seeds[0], history (history_counts[0] ids)
+ *     and draw first_draw + j for its j-th id.  Greedy and sampled sessions with any settings share a stream.
  *   - A session ends after its max_tokens-th id, after the first id in stop_ids (delivered), or with id -1 when its logits
  *     have no distribution (see b200_generate_sample); the others go on.
  *   - b200_stream_read returns (session, id) pairs in production order: it blocks until at least one is available and
