@@ -241,28 +241,26 @@ def dequant_rows(f: ggjt.GGJTFile, name: str, rows) -> np.ndarray:
     return _DEQUANT[t.ttype](w)
 
 
+PORT_OUTPUT_TYPES = (ggjt.T_Q4_0, ggjt.T_Q4_1, ggjt.T_Q5_0, ggjt.T_Q5_1, ggjt.T_Q8_0, ggjt.T_F16, ggjt.T_Q6_K)
+
+
 def port_logits(path: str, x: np.ndarray) -> np.ndarray:
-    """Logits of every row of x on the C restatement: RMSNorm * norm.weight, then the Q6_K lm_head of kq_port, or the
-    Q4_0 one from slice_oracle.c's Q8_0 quantiser and Q4_0 dot."""
+    """Logits of every row of x on the C restatement: RMSNorm * norm.weight, then the Q6_K lm_head of kq_port, or for
+    Q4_0, Q4_1, Q8_0 and F16 slice_oracle.c's activation quantisers and dots (F16: fp16 activations), for Q5_0 and Q5_1
+    q5_port's."""
     f = ggjt.read_file(path, sliced=True)
-    if f.tensors["output.weight"].ttype == ggjt.T_Q6_K:
+    wt = f.tensors["output.weight"].ttype
+    if wt == ggjt.T_Q6_K:
         from kq_port import KQPortExtra
         return KQPortExtra(path).logits(x)
-    from oracle import oracle
-    assert f.tensors["output.weight"].ttype == ggjt.T_Q4_0
-    L = oracle.port_lib()
+    import q5_port
+    assert wt in PORT_OUTPUT_TYPES, ggjt.TYPE_NAME.get(wt, wt)
     k, nv = f.hparams.n_embd, f.hparams.n_vocab
     w = np.frombuffer(f.read_raw("output.weight"), np.uint8).copy()
     nw = np.frombuffer(f.read_raw("norm.weight"), np.float32).copy()
     x = np.ascontiguousarray(x, np.float32).reshape(-1, k)
     y = np.empty((len(x), nv), np.float32)
-    row = k // 32 * 18
-    for r in range(len(x)):
-        v, q, d = np.empty(k, np.float32), np.empty(k, np.int8), np.empty(k // 32, np.uint16)
-        L.orc_rmsnorm(ptr(x[r]), ptr(nw), k, ptr(v))
-        L.orc_quant_q8_0(ptr(v), k, ptr(q), ptr(d))
-        for j in range(nv):
-            y[r, j] = L.orc_dot_q4_0_q8_0(ptr(w[j * row:(j + 1) * row]), ptr(q), ptr(d), k)
+    q5_port.lib().q5_logits(wt, ptr(w), nv, k, ptr(nw), ptr(x), len(x), ptr(y))
     return y
 
 

@@ -11,6 +11,7 @@
  * orc_dot_q5_0_q8_0   ggml_vec_dot_q5_0_q8_0, AVX2 branch (ggml.c:2914-2936): Q4_0's chain with a fifth bit per weight
  * orc_dot_q5_1_q8_1   ggml_vec_dot_q5_1_q8_1, AVX2 branch (ggml.c:3164-3189): Q4_1's chain with a fifth bit per weight
  * q5_forward          orc_forward (tensor_processor.cpp:537-766) with the Q5 matmul dispatch (vec_dot_type, ggml.c:1674-1681)
+ * q5_logits           get_llm_output's RMSNorm + lm_head (tensor_processor.cpp:1850-1863) for any type q5_matmul takes
  */
 #include "slice_oracle.c"
 
@@ -79,6 +80,17 @@ static void q5_matmul(const orc_slice * s, const uint8_t * W, int rows, int k, c
     } else {
         matmul(s, W, rows, k, x, N, y);
     }
+}
+
+/* lm_head of an extra-layers file whose output.weight is Q4_0, Q4_1, Q5_0, Q5_1, Q8_0 or F16 (wtype): RMSNorm * norm
+ * weight, then y[N][n_vocab] = W . x as the layers' matmuls compute it */
+void q5_logits(int wtype, const uint8_t * W, int n_vocab, int E, const float * norm_w, const float * x, int N, float * y) {
+    init_tables();
+    orc_slice s; memset(&s, 0, sizeof s); s.wtype = wtype;
+    float * cur = malloc((size_t) N * E * 4);
+    for (int n = 0; n < N; n++) orc_rmsnorm(x + (size_t) n * E, norm_w, E, cur + (size_t) n * E);
+    q5_matmul(&s, W, n_vocab, E, cur, N, y);
+    free(cur);
 }
 
 /* orc_forward with q5_matmul.  in/out: [N][n_embd] f32.  Returns 0, or 1 when the context would overflow. */

@@ -1,7 +1,8 @@
 """The Q5_0 / Q5_1 C restatement (tests/q5_port.c on top of oracle/slice_oracle.c), TEST INFRASTRUCTURE.
 
-`Q5PortSlice` mirrors oracle.oracle.PortSlice on a slice file of any type the restatement covers; the library is
-compiled on first use into a per-source directory under the system temporary directory (the tree may be read-only).
+`Q5PortSlice` mirrors oracle.oracle.PortSlice on a slice file of any type the restatement covers; `q5_logits` is the
+lm_head of an extra-layers file with any of those output types (edge_cases.port_logits).  The library is compiled on
+first use into a per-source directory under the system temporary directory (the tree may be read-only).
 """
 from __future__ import annotations
 
@@ -59,6 +60,7 @@ def lib() -> C.CDLL:
         L.orc_dot_q5_1_q8_1.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         L.orc_quant_q8_0.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         L.orc_quant_q8_1.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.q5_logits.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         _lib = L
     return _lib
 
