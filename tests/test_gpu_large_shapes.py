@@ -91,16 +91,17 @@ def layer_file(tmp_path_factory):
         os.remove(p)
 
 
-def _checker(path, n_ctx):
-    """The CPU computation a mismatch is counted against: the compiled reference where it was built, else the C port."""
-    return oracle.RefSlice(path, min(16, os.cpu_count() or 4), n_ctx) if HAVE_REF else oracle.PortSlice(path, n_ctx)
+def _checker(path, n_ctx, port=oracle.PortSlice):
+    """The CPU computation a mismatch is counted against: the compiled reference where it was built, else the C port
+    `port` (a class with PortSlice's forward / clear_context / close)."""
+    return oracle.RefSlice(path, min(16, os.cpu_count() or 4), n_ctx) if HAVE_REF else port(path, n_ctx)
 
 
-def _checker_name():
-    return "RefSlice" if HAVE_REF else "PortSlice"
+def _checker_name(port=oracle.PortSlice):
+    return "RefSlice" if HAVE_REF else port.__name__
 
 
-def _replay_schedule(path, case):
+def _replay_schedule(path, case, port=oracle.PortSlice):
     from distributedllm_b200 import capi
     xs = large.case_inputs(case)
     gpu = capi.Slice(path, 0, case["n_ctx"])
@@ -112,7 +113,7 @@ def _replay_schedule(path, case):
     for i, y in enumerate(ys):
         assert np.isfinite(y).all(), "call %d (N=%d): non-finite output" % (i, len(xs[i]))
     if wrong:
-        cpu = _checker(path, case["n_ctx"])
+        cpu = _checker(path, case["n_ctx"], port)
         try:
             want = [cpu.forward(x) for x in xs[:wrong[-1] + 1]]
         finally:
@@ -120,10 +121,10 @@ def _replay_schedule(path, case):
         report = ["call %d (N=%d): %d of %d floats differ" % (i, len(xs[i]), int((_bits(ys[i]) != _bits(want[i])).sum()),
                                                               ys[i].size) for i in wrong]
         pytest.fail("%d of %d calls differ from the reference (recomputed with %s): %s" % (
-            len(wrong), len(xs), _checker_name(), "; ".join(report)))
+            len(wrong), len(xs), _checker_name(port), "; ".join(report)))
 
 
-def _replay_batch(path, case):
+def _replay_batch(path, case, port=oracle.PortSlice):
     from distributedllm_b200 import capi
     prompts, steps = large.batch_inputs(case)
     sessions = case["sessions"]
@@ -138,7 +139,7 @@ def _replay_batch(path, case):
               if large.digest(got_s[i][b]) != case["step_digests"][i][b]]
     assert all(np.isfinite(y).all() for y in got_p + got_s)
     if wrong:
-        cpu = _checker(path, case["n_ctx"])
+        cpu = _checker(path, case["n_ctx"], port)
         want_p, want_s = [], [[None] * len(sessions) for _ in steps]
         try:
             for b in range(len(sessions)):
@@ -154,7 +155,7 @@ def _replay_batch(path, case):
             report.append("%s, column %d (session %d): %d of %d floats differ" % (
                 what, b, sessions[b], int((_bits(g) != _bits(w)).sum()), g.size))
         pytest.fail("%d outputs differ from the reference (recomputed with %s): %s" % (
-            len(wrong), _checker_name(), "; ".join(report)))
+            len(wrong), _checker_name(port), "; ".join(report)))
 
 
 @pytest.mark.parametrize("name,env", [pytest.param(n, e, id=_run_id(n, e)) for n, e in RUNS])
