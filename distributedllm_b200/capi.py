@@ -99,6 +99,9 @@ def lib() -> C.CDLL:
                            ("b200_extra_tokenize", [vp, C.c_char_p, vp, ci]),
                            ("b200_generate_greedy", [vp, ci, vp, vp, vp, ci, vp, ci, vp]),
                            ("b200_generate_sample", [vp, ci, vp, vp, vp, ci, vp, ci, vp, vp]),
+                           ("b200_generate_speculative", [vp, ci, vp, ci, vp, ci, vp, ci, vp, ci, ci, ci, vp, vp, vp]),
+                           ("b200_session_forward_steps", [vp, ci, vp, ci, vp]),
+                           ("b200_session_forward_steps_device", [vp, ci, vp, ci, vp, ci]),
                            ("b200_extra_sample", [vp, vp, ci, vp, vp]),
                            ("b200_score", [vp, ci, vp, vp, vp, ci, vp, vp]), ("b200_extra_nll", [vp, vp, ci, vp, vp]),
                            ("b200_stream_open", [vp, ci, vp, ci, ci, C.POINTER(vp)]),
@@ -137,6 +140,14 @@ class Slice:
         x = np.ascontiguousarray(x, dtype=np.float32).reshape(-1, self.n_embd)
         out = np.empty_like(x)
         check(lib().b200_session_forward(self._h, session, _ptr(x), x.shape[0], _ptr(out)))
+        return out
+
+    def forward_steps(self, session: int, x: np.ndarray) -> np.ndarray:
+        """Decode rows (b200_session_forward_steps): the rows of x as single-token steps of `session`, in one pass;
+        bit-identical to one session_forward call per row."""
+        x = np.ascontiguousarray(x, dtype=np.float32).reshape(-1, self.n_embd)
+        out = np.empty_like(x)
+        check(lib().b200_session_forward_steps(self._h, session, _ptr(x), x.shape[0], _ptr(out)))
         return out
 
     def batch_forward(self, sessions, x: np.ndarray) -> np.ndarray:
@@ -441,6 +452,35 @@ def generate_sample(slices, extra: Extra, sessions, prompts, n_steps: int, tempe
     check(lib().b200_generate_sample(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks),
                                      n_steps, C.byref(sp), _ptr(out)))
     return out
+
+
+class SpecStats(C.Structure):
+    _fields_ = [("passes", C.c_int32), ("drafted", C.c_int32), ("accepted", C.c_int32)]
+
+
+def generate_speculative(slices, extra: Extra, session: int, draft_slices, draft_extra: Extra, draft_session: int, prompt,
+                         n_steps: int, n_draft: int, temperature: Optional[float] = None, repeat_penalty: float = 1.1,
+                         seed: Optional[int] = None, first_draw: int = 0, history=None, top_k: int = 0, top_p: float = 0.0):
+    """Speculative decoding on the device (b200_generate_speculative): the draft chain proposes n_draft ids per
+    iteration, one pass of the target checks them.  temperature None: greedy, the ids of generate_greedy; else the ids of
+    generate_sample with the same settings (seed: the session's Philox key; history: the ids it sampled before).
+    -> (ids [n_steps] int32, {"passes", "drafted", "accepted"})."""
+    toks = np.ascontiguousarray([int(t) for t in prompt], dtype=np.int32)
+    handles = (C.c_void_p * max(len(slices), 1))(*[s.handle for s in slices])
+    dhandles = (C.c_void_p * max(len(draft_slices), 1))(*[s.handle for s in draft_slices])
+    sp, keep = None, []
+    if temperature is not None:
+        if seed is None:
+            raise ValueError("sampled speculative generation needs a seed")
+        sp, keep = _sampling(1, temperature, repeat_penalty, [seed], first_draw, None if history is None else [history],
+                             top_k, top_p)
+    out = np.zeros(max(n_steps, 0), np.int32)
+    stats = SpecStats()
+    check(lib().b200_generate_speculative(handles, len(slices), extra.handle, session, dhandles, len(draft_slices),
+                                          draft_extra.handle, draft_session, _ptr(toks), len(toks), n_steps, n_draft,
+                                          C.byref(sp) if sp is not None else None, _ptr(out), C.byref(stats)))
+    del keep
+    return out, {"passes": stats.passes, "drafted": stats.drafted, "accepted": stats.accepted}
 
 
 def score(slices, extra: Extra, sessions, token_lists) -> list:

@@ -229,6 +229,28 @@ class LocalPipeline:
                                                  "float64 once scaled, so they have no distribution" % j)
                 yield extra.token_text(token_id)
 
+    def generate_speculative(self, extra_path: str, prompt: str, draft: "LocalPipeline", draft_extra_path: str,
+                             max_steps: int = 200, n_draft: int = 4, temperature: float = 0.0, repeat_penalty: float = 1.1,
+                             seed: int = None, top_k: int = None, top_p: float = None) -> List[int]:
+        """Speculative decoding on this box (capi.generate_speculative): clear both pipelines' contexts, tokenize with the
+        target's extra layers, then max_steps ids, the draft pipeline proposing n_draft ids per target pass.  The ids do
+        not depend on the draft: at temperature 0 they are generate_greedy's; otherwise the ids behind the strings
+        generate(..., seed=seed, stop_at_eos=False) yields.  Needs every slice of both pipelines on one device."""
+        extra = self._device_extra(extra_path, "speculative generation")
+        dextra = draft._device_extra(draft_extra_path, "speculative generation")
+        if temperature and seed is None:
+            seed = int(np.random.randint(0, 2 ** 64, dtype=np.uint64))
+        self.clear_context()
+        draft.clear_context()
+        tokens = extra.tokenize(prompt)
+        if max_steps < 1:
+            return []
+        ids, _ = self.capi.generate_speculative(self.slices, extra, 0, draft.slices, dextra, 0, tokens, max_steps, n_draft,
+                                                temperature=temperature if temperature else None,
+                                                repeat_penalty=repeat_penalty, seed=seed, top_k=top_k or 0,
+                                                top_p=top_p or 0.0)
+        return ids.tolist()
+
     def perplexity(self, extra_path: str, text: str) -> float:
         """DistributedLLM.perplexity on this box: clear the contexts, tokenize, then score the text on the GPU
         (capi.score: one pass, lm_head and softmax on the device, only the per-token NLLs come back).  The NLLs are

@@ -1895,6 +1895,20 @@ __global__ void k_advance_segs(int * n_past, const int2 * segs, int n) {
     grid_dep_wait();
     for (int i = threadIdx.x; i < n; i += blockDim.x) n_past[segs[i].x] += segs[i].y;
 }
+// Decode rows (b200_session_forward_steps): the pass table of N single-token steps of one session, from its device-side
+// position p = n_past[session]: column j = (session, p + j) with row length T = p + j + 1, one segment (session, N).  So a
+// pass needs no host-known position.  Positions are clamped to n_ctx - 1 so that a pass never writes outside the cache;
+// every caller checks p + N <= n_ctx on the host, so the clamp changes no row of a valid call.
+// Layout as begin_pass: cols [N] int2, segs [1] int2, col_T [N].
+__global__ void k_steps_table(const int * n_past, int session, int N, int n_ctx, int * tab) {
+    grid_dep_wait();
+    const int p = n_past[session];
+    for (int j = threadIdx.x; j < N; j += blockDim.x) {
+        const int pos = min(p + j, n_ctx - 1);
+        tab[2 * j] = session; tab[2 * j + 1] = pos; tab[2 * N + 2 + j] = pos + 1;
+    }
+    if (threadIdx.x == 0) { tab[2 * N] = session; tab[2 * N + 1] = N; }
+}
 
 }  // namespace b200
 

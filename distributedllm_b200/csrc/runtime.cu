@@ -62,6 +62,9 @@ struct b200_slice {
     std::vector<Seg> segs; std::vector<int> h_pass;
     int * d_pass = nullptr; const int2 * cols = nullptr; const int * col_T = nullptr; const int2 * d_segs = nullptr;
     const AttnTile * d_tiles = nullptr; int n_tiles = 0, tile_rows = 0;
+    // decode rows (begin_steps): the pass is N single-token steps of one session, its table built on the device, and every
+    // column attends with its own row length T = position + 1
+    bool steps = false;
     std::vector<LayerW> layers;
     std::vector<void *> allocs;
     uint16_t * kc = nullptr, * vc = nullptr, * q16 = nullptr;
@@ -481,6 +484,21 @@ static int attention(b200_slice * s, int il, int N, bool preq) {
         }
         return 0;
     };
+    if (s->steps) {
+        // decode rows: every row's K / V is appended first, then each row attends with T = its position + 1, the arithmetic
+        // of its own single-token step.  Not the fused kernel: its columns would race on each other's K / V rows; not the
+        // query-tiled one: it takes one T per chunk.
+        s->cur_class = 1;
+        RopeArgs ra{s->qkv, E, H, D, N, d_npast, s->cs, s->q16, kc, vc, s->cols, s->sess_stride};
+        if ((rc = launch(s, k_rope_append, dim3((E / 2 + 255) / 256, N, 1), dim3(256, 1, 1), 0, ra))) return rc;
+        s->cur_class = 2;
+        aa.col_T = s->col_T;
+        for (int n0 = 0; n0 < N; n0 += kChunk) {
+            aa.n0 = n0;
+            if ((rc = launch(s, k_attn128<false>, dim3(4 * H, std::min(N - n0, kChunk), 1), dim3(256, 1, 1), am.plain, aa))) return rc;
+        }
+        return 0;
+    }
     if (s->cols && !s->col_T) {
         // batched step: every column is a single-token step
         s->cur_class = 2;
@@ -836,7 +854,46 @@ static int begin_pass(b200_slice * s, const int * sessions, const int * counts, 
     return 0;
 }
 
-static void end_pass(b200_slice * s) { s->cols = nullptr; s->col_T = nullptr; s->d_segs = nullptr; s->d_tiles = nullptr; s->n_tiles = 0; }
+static void end_pass(b200_slice * s) {
+    s->cols = nullptr; s->col_T = nullptr; s->d_segs = nullptr; s->d_tiles = nullptr; s->n_tiles = 0; s->steps = false;
+}
+
+// Decode rows: N single-token steps of `session` in one pass, at the positions its DEVICE counter holds (k_steps_table), so
+// the pass can follow device-side position updates without the host knowing them.  From here until end_pass,
+// enqueue_layers runs the pass; its k_advance_segs moves the session N positions.  Fast prefill never applies (cols mode).
+static int begin_steps(b200_slice * s, int session, int N) {
+    if (int rc = launch(s, k_steps_table, dim3(1), dim3(256), 0, (const int *) s->d_npast, session, N, s->n_ctx, s->d_pass)) return rc;
+    s->segs.assign(1, b200_slice::Seg{session, 0, N, 0});
+    s->n_tiles = 0; s->tile_rows = 0; s->cur = 0; s->steps = true;
+    s->cols = (const int2 *) s->d_pass;
+    s->d_segs = (const int2 *)(s->d_pass + 2 * N);
+    s->col_T = s->d_pass + 2 * N + 2;
+    return 0;
+}
+
+// b200_session_forward_steps: decode rows with the host checks of b200_session_forward
+static int steps_locked(b200_slice * s, int session, const float * in, int N, float * out, bool host) {
+    if (N <= 0) return fail(B200_EINVAL, "n_tokens must be positive (got %d)", N);
+    if (session < 0 || session >= s->n_sessions) return fail(B200_EINVAL, "session %d outside [0, %d)", session, s->n_sessions);
+    if (s->past[session] + N > s->n_ctx)
+        return fail(B200_ECONTEXT, "context overflow: n_past %d + n_tokens %d > n_ctx %d", s->past[session], N, s->n_ctx);
+    B200_CUDA(cudaSetDevice(s->device));
+    B200_CUDA(cudaEventRecord(s->ev0, s->stream));
+    int rc;
+    if ((rc = begin_steps(s, session, N))) { end_pass(s); return rc; }
+    if (host) B200_CUDA(cudaMemcpyAsync(s->d_in, in, (size_t) N * s->E * 4, cudaMemcpyHostToDevice, s->stream));
+    rc = enqueue_layers(s, host ? s->d_in : in, N, host ? s->d_out : out);
+    end_pass(s);
+    if (rc) return rc;
+    B200_CUDA(cudaEventRecord(s->ev1, s->stream));
+    if (host) {
+        B200_CUDA(cudaMemcpyAsync(out, s->d_out, (size_t) N * s->E * 4, cudaMemcpyDeviceToHost, s->stream));
+        B200_CUDA(cudaStreamSynchronize(s->stream));
+    }
+    s->timed = true;
+    s->past[session] += N;
+    return 0;
+}
 
 static void advance_pass(b200_slice * s, const int * sessions, const int * counts, int n_seq) {
     for (int k = 0; k < n_seq; k++) s->past[sessions[k]] += counts ? counts[k] : 1;
@@ -1391,6 +1448,21 @@ int b200_session_forward_device(b200_slice_t * s, int session, const float * d_i
     if (!s || !d_in || !d_out) return fail(B200_EINVAL, "null argument");
     std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     int rc = forward_locked(s, d_in, n_tokens, d_out, false, session);
+    if (rc) return rc;
+    if (sync) B200_CUDA(cudaStreamSynchronize(s->stream));
+    return 0;
+}
+
+int b200_session_forward_steps(b200_slice_t * s, int session, const float * in, int n_tokens, float * out) {
+    if (!s || !in || !out) return fail(B200_EINVAL, "null argument");
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
+    return steps_locked(s, session, in, n_tokens, out, true);
+}
+
+int b200_session_forward_steps_device(b200_slice_t * s, int session, const float * d_in, int n_tokens, float * d_out, int sync) {
+    if (!s || !d_in || !d_out) return fail(B200_EINVAL, "null argument");
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
+    int rc = steps_locked(s, session, d_in, n_tokens, d_out, false);
     if (rc) return rc;
     if (sync) B200_CUDA(cudaStreamSynchronize(s->stream));
     return 0;
@@ -3048,6 +3120,325 @@ static int score_locked(b200_slice * const * slices, int n_slices, b200_extra * 
     return 0;
 }
 
+// ---------------------------------------------------------------- speculative decoding (b200_generate_speculative)
+// One iteration, with t the last emitted id, m the ids emitted so far and p the target's position (where t goes):
+//   draft  a two-row decode pass [token at p - 1, t], then k - 1 replays of its decode step, each followed by its lm_head
+//          and a proposal d_i (k_spec_draft_pick);
+//   check  the target's decode rows [t, d_1 .. d_k] at p .. p + k, its lm_head over the k + 1 rows and its choice g_j after
+//          each row (k_spec_check_pick);
+//   accept k_spec_accept keeps g_0 .. g_n, n the longest run with d_i == g_(i-1), and moves both chains' positions.
+// The two-row draft pass rewrites the draft's row p - 1 with the token it already holds there (or fills it when the
+// previous iteration kept all k proposals, so the draft never ran d_k): every iteration has the same shape.  Everything an
+// iteration reads (tokens, positions, draw indices) is on the device, so the host only enqueues.
+constexpr int kSpecMaxDraft = 15;
+constexpr int kSpecLookahead = 2;           // iterations enqueued beyond the last one the host has seen finish
+
+struct SpecState {
+    int m, p, iters, passes, drafted, accepted;
+    int32_t ctok[kSpecMaxDraft + 1];        // the checking pass's tokens: t, d_1 .. d_k
+    int32_t g[kSpecMaxDraft + 1];           // the target's id after each checking row
+    int32_t dtok[2];                        // the draft's two-row pass: the token at p - 1, t
+    int32_t dcur;                           // the draft's last proposal, its next single step's token
+};
+
+// The sampling settings of one speculative call (sampled == 0: greedy, the argmax of the raw logits)
+struct SpecSample { uint64_t seed; double dt, dp; long long first_draw; int top_k; double top_p; int sampled; };
+
+__global__ void k_spec_init(SpecState * st, const int32_t * id0, int32_t prev, int p, int * const * npast_d, int n_d) {
+    if (threadIdx.x) return;
+    st->m = 1; st->p = p; st->iters = 0; st->passes = 0; st->drafted = 0; st->accepted = 0;
+    const int32_t t = *id0;
+    st->ctok[0] = t; st->dtok[0] = prev; st->dtok[1] = t;
+    for (int i = 0; i < n_d; i++) *npast_d[i] = p - 1;
+}
+
+// The draft's proposal d_i: the argmax, or the Sampler with the draw the target takes for the id d_i guesses
+// (first_draw + m + i - 1) and the penalty set history + ids[0, m) + d_1 .. d_(i-1): `work` starts each iteration as a copy
+// of the emitted ids' bitmap `base` and collects the proposals.
+__global__ void __launch_bounds__(1024) k_spec_draft_pick(const float * logits, int n, SpecState * st, int i, SpecSample sp,
+                                                          const uint32_t * base, uint32_t * work, int nw) {
+    if (sp.sampled && i == 1) {
+        for (int w = threadIdx.x; w < nw; w += blockDim.x) work[w] = base[w];
+        __syncthreads();
+    }
+    const int id = sp.sampled ? sample_row(logits, n, work, sp.dt, sp.dp, sp.seed, sp.first_draw + st->m + i - 1, sp.top_k, sp.top_p)
+                              : argmax_row(logits, n);
+    if (threadIdx.x) return;
+    st->dcur = id; st->ctok[i] = id;
+    if (sp.sampled && id >= 0) work[id >> 5] |= 1u << (id & 31);
+}
+
+// The target's id g_j after checking row j (one block per row): the argmax, or the Sampler with draw first_draw + m + j and
+// the penalty set history + ids[0, m) + d_1 .. d_j, which is the plain loop's set for ids[m + j] whenever g_j is kept.
+// Row j's bitmap is its own copy of `base` with d_1 .. d_j added, so the sampler's arithmetic is k_sample_rows'.
+__global__ void __launch_bounds__(1024) k_spec_check_pick(const float * logits, int n, SpecState * st, SpecSample sp,
+                                                          const uint32_t * base, uint32_t * rows, int nw) {
+    const int j = blockIdx.x;
+    const float * x = logits + (size_t) j * n;
+    int id;
+    if (sp.sampled) {
+        uint32_t * bits = rows + (size_t) j * nw;
+        for (int w = threadIdx.x; w < nw; w += blockDim.x) bits[w] = base[w];
+        __syncthreads();
+        if (threadIdx.x == 0)
+            for (int i = 1; i <= j; i++) { const int d = st->ctok[i]; if (d >= 0) bits[d >> 5] |= 1u << (d & 31); }
+        __syncthreads();
+        id = sample_row(x, n, bits, sp.dt, sp.dp, sp.seed, sp.first_draw + st->m + j, sp.top_k, sp.top_p);
+    } else {
+        id = argmax_row(x, n);
+    }
+    if (threadIdx.x == 0) st->g[j] = id;
+}
+
+// Keeps g_0 .. g_n (n the largest j <= k with d_i == g_(i-1) for every i <= j), cut at the budget of n_steps ids, and moves
+// every target slice to p + (ids emitted) and every draft slice one row before it.  The host never enqueues an iteration
+// the ones in flight could leave without budget; should one start with the budget spent, it emits nothing and puts the
+// positions back where it found them.  Then it publishes (iterations done, ids emitted) to the host through mapped memory.
+__global__ void k_spec_accept(SpecState * st, int k, int n_steps, int32_t * ids, uint32_t * base, int * bad,
+                              int * const * npast_t, int n_t, int * const * npast_d, int n_d, volatile int * progress) {
+    if (threadIdx.x) return;
+    const int m = st->m;
+    if (m < n_steps) {
+        int n = 0;
+        while (n < k && st->ctok[n + 1] == st->g[n]) n++;
+        const int c = min(n + 1, n_steps - m);
+        for (int j = 0; j < c; j++) {
+            const int id = st->g[j];
+            ids[m + j] = id;
+            if (id < 0) { if (bad) atomicMin(bad, m + j); }
+            else if (base) base[id >> 5] |= 1u << (id & 31);
+        }
+        st->passes++; st->drafted += k; st->accepted += n;
+        const int32_t t = st->g[c - 1];
+        st->dtok[0] = st->ctok[c - 1]; st->dtok[1] = t; st->ctok[0] = t;
+        st->m = m + c; st->p += c;
+    }
+    for (int i = 0; i < n_t; i++) *npast_t[i] = st->p;
+    for (int i = 0; i < n_d; i++) *npast_d[i] = st->p - 1;
+    st->iters++;
+    __threadfence_system();
+    progress[0] = st->iters; progress[1] = st->m;
+}
+
+// One single-token step of slice s for `session`: the decode graph when it is used, as forward_locked runs it.
+static int decode_step(b200_slice * s, int session, const float * in, float * out) {
+    s->cur = session; s->cols = nullptr;
+    if (s->use_graph && !s->profiling) return run_decode_graph(s, in, out, false);
+    return enqueue_layers(s, in, 1, out);
+}
+
+// decode rows of one session over a chain: -> the last slice's output
+static int chain_steps(b200_slice * const * sl, int n, int session, const float * in, int N, const float ** out) {
+    for (int i = 0; i < n; i++) {
+        b200_slice * s = sl[i];
+        int rc = begin_steps(s, session, N);
+        if (!rc) rc = enqueue_layers(s, in, N, s->d_out);
+        end_pass(s);
+        if (rc) return rc;
+        in = s->d_out;
+    }
+    *out = in;
+    return 0;
+}
+
+static int embed_launch(b200_extra * e, const int32_t * tok, int N, float * out) {
+    k_embed_rows<<<dim3((e->E + 255) / 256, N), 256, 0, e->ctx.stream>>>(e->emb_raw, e->emb_type, e->E, tok, e->n_vocab, out);
+    B200_CUDA(cudaGetLastError());
+    e->ctx.launches++;
+    return 0;
+}
+
+// Everything b200_generate_speculative checks before it enqueues anything (every mutex is held).
+static int spec_check(b200_slice * const * t, int nt, const b200_extra * e, int session, b200_slice * const * d, int nd,
+                      const b200_extra * de, int dsession, const int32_t * prompt, int n_prompt, int n_steps, int k,
+                      const b200_sampling_t * sp) {
+    if (int rc = chain_check(t, nt, e)) return rc;
+    if (int rc = chain_check(d, nd, de)) return rc;
+    if (de->ctx.device != e->ctx.device)
+        return fail(B200_EINVAL, "the draft is on device %d, the target on device %d: the loop runs on one GPU", de->ctx.device, e->ctx.device);
+    if (de->n_vocab != e->n_vocab) return fail(B200_EINVAL, "the draft has %d ids, the target %d", de->n_vocab, e->n_vocab);
+    if (n_steps < 1) return fail(B200_EINVAL, "n_steps must be positive (got %d)", n_steps);
+    if (k < 1 || k > kSpecMaxDraft) return fail(B200_EINVAL, "n_draft %d outside [1, %d]", k, kSpecMaxDraft);
+    int total = 0;
+    for (int i = 0; i < nt; i++) if (int rc = check_pass(t[i], &session, &n_prompt, 1, &total)) return rc;
+    for (int i = 0; i < nd; i++) if (int rc = check_pass(d[i], &dsession, &n_prompt, 1, &total)) return rc;
+    if (int rc = check_tokens(prompt, n_prompt, e->n_vocab, "prompt token")) return rc;
+    const int past = t[0]->past[session];
+    for (int c = 0; c < 2; c++)
+        for (int i = 0; i < (c ? nd : nt); i++) {
+            const b200_slice * s = c ? d[i] : t[i];
+            const int q = s->past[c ? dsession : session];
+            if (q != past)
+                return fail(B200_EINVAL, "%s slice %d is at n_past %d, target slice 0 at %d: both chains must start at one position",
+                            c ? "draft" : "target", i, q, past);
+            if ((long long) q + n_prompt + n_steps - 1 + k > s->n_ctx)
+                return fail(B200_ECONTEXT, "context overflow: %s slice %d n_past %d + %d prompt tokens + %d steps + %d draft rows > n_ctx %d",
+                            c ? "draft" : "target", i, q, n_prompt, n_steps - 1, k, s->n_ctx);
+        }
+    if (sp) return sample_check(sp, 1, e->n_vocab);
+    return 0;
+}
+
+static int spec_locked(b200_slice * const * t, int nt, b200_extra * e, int session, b200_slice * const * d, int nd,
+                       b200_extra * de, int dsession, const int32_t * prompt, int n_prompt, int n_steps, int k,
+                       const b200_sampling_t * sp, int32_t * ids, b200_spec_stats_t * stats) {
+    b200_slice * x = &e->ctx;
+    B200_CUDA(cudaSetDevice(x->device));
+    const int V = e->n_vocab, nw = (V + 31) / 32, p0 = t[0]->past[session] + n_prompt, p_final = p0 + n_steps - 1;
+    int rc;
+    if ((rc = extra_reserve(e, std::max(n_prompt, k + 1))) || (rc = extra_reserve_ids(e, n_steps)) ||
+        (rc = extra_reserve(de, std::max(n_prompt, 2))))
+        return rc;
+    for (int i = 0; i < nt; i++) B200_CUDA(cudaStreamSynchronize(t[i]->stream));
+    for (int i = 0; i < nd; i++) B200_CUDA(cudaStreamSynchronize(d[i]->stream));
+    B200_CUDA(cudaStreamSynchronize(de->ctx.stream));
+    if (sp && (rc = sample_start(e, sp, 1))) return rc;
+    // device scratch: the state, the slices' position counters, the draft's and the checking rows' penalty bitmaps
+    const size_t off_ptr = (sizeof(SpecState) + 15) & ~(size_t) 15, off_bits = off_ptr + ((sizeof(int *) * (nt + nd) + 15) & ~(size_t) 15);
+    const size_t bytes = off_bits + (sp ? (size_t)(k + 2) * nw * 4 : 0);
+    uint8_t * blob = nullptr; int * h_prog = nullptr; int * d_prog = nullptr;
+    B200_CUDA(cudaMalloc(&blob, bytes));
+    if (cudaHostAlloc(&h_prog, 2 * sizeof(int), cudaHostAllocMapped) != cudaSuccess || cudaHostGetDevicePointer(&d_prog, h_prog, 0) != cudaSuccess) {
+        if (h_prog) cudaFreeHost(h_prog);
+        cudaFree(blob);
+        return fail(B200_ECUDA, "cudaHostAlloc of the speculative loop's progress words failed");
+    }
+    struct Release { uint8_t * b; int * h; ~Release() { cudaFree(b); cudaFreeHost(h); } } release{blob, h_prog};
+    SpecState * st = (SpecState *) blob;
+    int ** npast = (int **)(blob + off_ptr);
+    uint32_t * work = sp ? (uint32_t *)(blob + off_bits) : nullptr, * rows = sp ? work + nw : nullptr;
+    uint32_t * base = sp ? e->d_pen : nullptr;       // sample_start's row: the history, then every emitted id
+    std::vector<int *> h_npast;
+    for (int i = 0; i < nt; i++) h_npast.push_back(t[i]->d_npast + session);
+    for (int i = 0; i < nd; i++) h_npast.push_back(d[i]->d_npast + dsession);
+    h_prog[0] = 0; h_prog[1] = 1;
+    SpecSample ss{};
+    if (sp) {
+        ss.sampled = 1; ss.seed = sp->seeds[0]; ss.dt = sp->temperature + 1e-5; ss.dp = sp->repeat_penalty * ss.dt;
+        ss.first_draw = sp->first_draw; ss.top_k = sp->top_k; ss.top_p = sp->top_p;
+    }
+    B200_CUDA(cudaMemcpyAsync(npast, h_npast.data(), h_npast.size() * sizeof(int *), cudaMemcpyHostToDevice, x->stream));
+    B200_CUDA(cudaMemcpyAsync(e->d_tok, prompt, (size_t) n_prompt * 4, cudaMemcpyHostToDevice, x->stream));
+    B200_CUDA(cudaMemcpyAsync(de->d_tok, prompt, (size_t) n_prompt * 4, cudaMemcpyHostToDevice, x->stream));
+    int issued = 0;
+    {
+        std::vector<b200_slice *> all(t, t + nt);
+        all.insert(all.end(), d, d + nd);
+        all.push_back(&de->ctx);
+        StreamLoan loan(all.data(), (int) all.size(), x->stream);
+        // step 0: the prompt, one mixed pass on each chain, as b200_generate_greedy's step 0
+        const float * cur = e->d_x;
+        if ((rc = embed_launch(e, e->d_tok, n_prompt, e->d_x))) return rc;
+        for (int i = 0; i < nt; i++) {
+            if ((rc = pass_locked(t[i], &session, &n_prompt, 1, cur, t[i]->d_out, false))) return rc;
+            cur = t[i]->d_out;
+        }
+        if ((rc = extra_lmhead(e, cur + (size_t)(n_prompt - 1) * e->E, 1))) return rc;
+        if (sp) { if ((rc = sample_launch(e, sp, 1, 0, e->d_ids))) return rc; }
+        else {
+            k_argmax_rows<<<1, 1024, 0, x->stream>>>(e->d_logits, V, e->d_tok, e->d_ids);
+            B200_CUDA(cudaGetLastError());
+            x->launches++;
+        }
+        cur = de->d_x;
+        if ((rc = embed_launch(de, de->d_tok, n_prompt, de->d_x))) return rc;
+        for (int i = 0; i < nd; i++) {
+            if ((rc = pass_locked(d[i], &dsession, &n_prompt, 1, cur, d[i]->d_out, false))) return rc;
+            cur = d[i]->d_out;
+        }
+        k_spec_init<<<1, 32, 0, x->stream>>>(st, e->d_ids, prompt[n_prompt - 1], p0, npast + nt, nd);
+        B200_CUDA(cudaGetLastError());
+        x->launches++;
+        // the iterations: each emits at least one id, so n_steps - 1 of them always suffice.  One more is enqueued only while
+        // fewer than kSpecLookahead are in flight and those cannot finish the budget (each emits at most k + 1 ids), so no
+        // iteration runs after the last id.
+        for (long spins = 0; issued < n_steps - 1;) {
+            const int done = ((volatile int *) h_prog)[0], m = ((volatile int *) h_prog)[1];
+            if (m >= n_steps) break;
+            const int flying = issued - done;
+            if (flying >= kSpecLookahead || (long long) m + (long long) flying * (k + 1) >= n_steps) {
+                // now and then make sure the device is still running the iterations (b200_stream_read's guard)
+                if (++spins % 4096 == 0) {
+                    const cudaError_t q = cudaStreamQuery(x->stream);
+                    if (q != cudaSuccess && q != cudaErrorNotReady)
+                        return fail(B200_ECUDA, "speculative loop: %s", cudaGetErrorString(q));
+                    if (q == cudaSuccess && ((volatile int *) h_prog)[0] < issued)
+                        return fail(B200_ECUDA, "speculative loop: the device finished an iteration without publishing it");
+                }
+                std::this_thread::yield();
+                continue;
+            }
+            spins = 0;
+            if ((rc = embed_launch(de, st->dtok, 2, de->d_x)) || (rc = chain_steps(d, nd, dsession, de->d_x, 2, &cur)) ||
+                (rc = extra_lmhead(de, cur + de->E, 1)))
+                return rc;
+            k_spec_draft_pick<<<1, 1024, 0, x->stream>>>(de->d_logits, V, st, 1, ss, base, work, nw);
+            B200_CUDA(cudaGetLastError());
+            x->launches++;
+            for (int i = 2; i <= k; i++) {
+                if ((rc = embed_launch(de, &st->dcur, 1, de->d_x))) return rc;
+                cur = de->d_x;
+                for (int j = 0; j < nd; j++) {
+                    if ((rc = decode_step(d[j], dsession, cur, d[j]->d_out))) return rc;
+                    cur = d[j]->d_out;
+                }
+                if ((rc = extra_lmhead(de, cur, 1))) return rc;
+                k_spec_draft_pick<<<1, 1024, 0, x->stream>>>(de->d_logits, V, st, i, ss, base, work, nw);
+                B200_CUDA(cudaGetLastError());
+                x->launches++;
+            }
+            if ((rc = embed_launch(e, st->ctok, k + 1, e->d_x)) || (rc = chain_steps(t, nt, session, e->d_x, k + 1, &cur)) ||
+                (rc = extra_lmhead(e, cur, k + 1)))
+                return rc;
+            k_spec_check_pick<<<k + 1, 1024, 0, x->stream>>>(e->d_logits, V, st, ss, base, rows, nw);
+            B200_CUDA(cudaGetLastError());
+            k_spec_accept<<<1, 32, 0, x->stream>>>(st, k, n_steps, e->d_ids, base, sp ? e->d_bad : nullptr, npast, nt,
+                                                   npast + nt, nd, d_prog);
+            B200_CUDA(cudaGetLastError());
+            x->launches += 2;
+            issued++;
+        }
+    }
+    SpecState h{};
+    B200_CUDA(cudaMemcpyAsync(ids, e->d_ids, (size_t) n_steps * 4, cudaMemcpyDeviceToHost, x->stream));
+    B200_CUDA(cudaMemcpyAsync(&h, st, sizeof(SpecState), cudaMemcpyDeviceToHost, x->stream));
+    for (int * q : h_npast) B200_CUDA(cudaMemcpyAsync(q, &p_final, 4, cudaMemcpyHostToDevice, x->stream));
+    B200_CUDA(cudaStreamSynchronize(x->stream));
+    for (int i = 0; i < nt; i++) t[i]->past[session] = p_final;
+    for (int i = 0; i < nd; i++) d[i]->past[dsession] = p_final;
+    if (stats) { stats->passes = h.passes; stats->drafted = h.drafted; stats->accepted = h.accepted; }
+    return sp ? sample_finish(e, 1, &session) : 0;
+}
+
+// b200_generate_speculative: the checks, every handle's mutex of both chains in address order, then the loop.
+static int speculative(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int session, b200_slice_t * const * draft,
+                       int n_draft_slices, b200_extra_t * draft_e, int draft_session, const int32_t * prompt, int n_prompt,
+                       int n_steps, int n_draft, const b200_sampling_t * sp, int32_t * ids, b200_spec_stats_t * stats) {
+    if (!slices || n_slices < 1 || !e || !draft || n_draft_slices < 1 || !draft_e || !prompt || n_prompt < 1 || !ids)
+        return fail(B200_EINVAL, "b200_generate_speculative: null argument or empty list");
+    std::vector<std::mutex *> mus{&e->mu, &draft_e->mu};
+    for (int c = 0; c < 2; c++)
+        for (int i = 0; i < (c ? n_draft_slices : n_slices); i++) {
+            b200_slice * s = c ? draft[i] : slices[i];
+            if (!s) return fail(B200_EINVAL, "%s slice %d is a null handle", c ? "draft" : "target", i);
+            mus.push_back(&s->mu);
+        }
+    std::sort(mus.begin(), mus.end());
+    if (std::adjacent_find(mus.begin(), mus.end()) != mus.end())
+        return fail(B200_EINVAL, "a handle is listed twice (every slice and extra-layers handle of both chains must be distinct)");
+    std::vector<std::unique_lock<std::mutex>> locks;
+    for (std::mutex * m : mus) locks.emplace_back(*m);
+    if (e->ctx.owner) return refuse_owned(&e->ctx);
+    if (draft_e->ctx.owner) return refuse_owned(&draft_e->ctx);
+    for (int i = 0; i < n_slices; i++) if (slices[i]->owner) return refuse_owned(slices[i]);
+    for (int i = 0; i < n_draft_slices; i++) if (draft[i]->owner) return refuse_owned(draft[i]);
+    if (int rc = spec_check(slices, n_slices, e, session, draft, n_draft_slices, draft_e, draft_session, prompt, n_prompt,
+                            n_steps, n_draft, sp))
+        return rc;
+    return spec_locked(slices, n_slices, e, session, draft, n_draft_slices, draft_e, draft_session, prompt, n_prompt, n_steps,
+                       n_draft, sp, ids, stats);
+}
+
 }  // namespace b200
 
 extern "C" {
@@ -3063,6 +3454,14 @@ int b200_generate_sample(b200_slice_t * const * slices, int n_slices, b200_extra
                          const b200_sampling_t * sp, int32_t * ids) {
     return generate(true, slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps,
                     sp, ids);
+}
+
+int b200_generate_speculative(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int session,
+                              b200_slice_t * const * draft, int n_draft_slices, b200_extra_t * draft_e, int draft_session,
+                              const int32_t * prompt, int n_prompt, int n_steps, int n_draft, const b200_sampling_t * sp,
+                              int32_t * ids, b200_spec_stats_t * stats) {
+    return speculative(slices, n_slices, e, session, draft, n_draft_slices, draft_e, draft_session, prompt, n_prompt, n_steps,
+                       n_draft, sp, ids, stats);
 }
 
 int b200_extra_sample(b200_extra_t * e, const float * logits, int n_rows, const b200_sampling_t * sp, int32_t * ids) {

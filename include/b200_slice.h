@@ -95,6 +95,14 @@ int b200_session_rewind(b200_slice_t * s, int session, int n_past);
 int b200_session_forward(b200_slice_t * s, int session, const float * in, int n_tokens, float * out);          /* host buffers */
 int b200_session_forward_device(b200_slice_t * s, int session, const float * d_in, int n_tokens, float * d_out, int sync);
 
+/* Decode rows: n_tokens single-token steps of one session in ONE pass, at positions n_past .. n_past + n_tokens - 1.  Row j
+ * runs with row length T = n_past + j + 1, as if it were its own step, so the output is bit-identical to n_tokens calls of
+ * b200_session_forward with one token each (a prompt chunk's rows are not: their attention follows the chunk's length).
+ * The weights stream once for all rows.  The pass table is built on the device from the session's device-side position.
+ * Afterwards n_past has advanced by n_tokens.  Fast prefill never applies.  Errors as b200_session_forward. */
+int b200_session_forward_steps(b200_slice_t * s, int session, const float * in, int n_tokens, float * out);       /* host buffers */
+int b200_session_forward_steps_device(b200_slice_t * s, int session, const float * d_in, int n_tokens, float * d_out, int sync);
+
 /* Throughput mode: ONE token for each of n_seq DISTINCT sessions in a single pass.  in / out are [n_seq][n_embd]; row b
  * belongs to sessions[b] and is processed at that session's own position.  The weights are streamed once for the whole
  * batch; every row's arithmetic is that of its own single-token step, so the result is bit-identical to calling
@@ -286,6 +294,37 @@ typedef struct b200_sampling {
 int b200_generate_sample(b200_slice_t * const * slices, int n_slices, b200_extra_t * e,
                          const int * sessions, const int * prompt_counts, int n_seq,
                          const int32_t * prompt_tokens, int n_steps, const b200_sampling_t * sp, int32_t * ids);
+/* Speculative decoding on the device, for one session: a draft model proposes n_draft ids, one pass of decode rows of the
+ * target (b200_session_forward_steps) checks them, and the longest agreeing prefix is kept.
+ *   - Ids: ids[0, n_steps) equal what b200_generate_greedy (sp NULL) or b200_generate_sample (same sp; seeds[0] and
+ *     history_counts[0] for this session) writes for this session alone with the same prompt and n_steps, bit for bit,
+ *     whatever the draft is.  The draft only decides how many target passes it takes.
+ *   - Each iteration: the draft runs n_draft single-token steps from the last emitted id t (greedy: the argmax; sampled:
+ *     proposal d_i guesses ids[m + i - 1] and takes that id's draw, first_draw + m + i - 1, with the penalty set history +
+ *     ids[0, m) + d_1 .. d_(i-1)); the target runs rows [t, d_1 .. d_k] and chooses g_j after row j with draw
+ *     first_draw + m + j and penalty set history + ids[0, m) + d_1 .. d_j; g_0 .. g_n are emitted, n the largest j with
+ *     d_i == g_(i-1) for every i <= j.  Step 0 is the prompt: one mixed pass on each chain, as b200_generate_greedy.
+ *   - Positions: every slice of both chains must start at one n_past (else B200_EINVAL); afterwards all are at
+ *     old + n_prompt + n_steps - 1, as after b200_generate_greedy.  So a second call with prompt = [last id] (sampled: with
+ *     the earlier ids as history and first_draw = their count) continues the run exactly.
+ *   - Draft chain: its own slices and extra layers on the target's GPU; its n_embd may differ, its n_vocab must equal the
+ *     target's.  Every handle of both chains must be distinct.
+ *   - The host enqueues iterations without a round trip (positions, tokens and draw indices live on the device), at most 2
+ *     beyond the last one it has seen finish (a counter in mapped memory) and none that the iterations in flight could leave
+ *     without budget, and synchronises once at the end.  A device error while it waits is B200_ECUDA.
+ *   - Locking, chain checks, stream ownership and all-or-nothing errors are as b200_generate_greedy.  Also B200_EINVAL for
+ *     n_draft outside [1, 15], a null draft or draft_e, a vocabulary mismatch or unequal starting positions, and
+ *     B200_ECONTEXT when n_past + n_prompt + n_steps - 1 + n_draft > n_ctx on any slice of either chain: a check can write
+ *     up to n_draft rows past the last kept one (rows nothing reads afterwards).
+ *   - stats (may be NULL): passes = target checking passes, drafted = proposals made (passes * n_draft), accepted =
+ *     proposals that matched the target's choice (including matches past the budget's end).
+ *   - A row with no distribution behaves as in b200_generate_sample: the same ids including -1, and B200_EINVAL naming
+ *     the first such step. */
+typedef struct b200_spec_stats { int32_t passes, drafted, accepted; } b200_spec_stats_t;
+int b200_generate_speculative(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int session,
+                              b200_slice_t * const * draft, int n_draft_slices, b200_extra_t * draft_e, int draft_session,
+                              const int32_t * prompt, int n_prompt, int n_steps, int n_draft,
+                              const b200_sampling_t * sp /* NULL: greedy */, int32_t * ids, b200_spec_stats_t * stats);
 /* The sampling rule alone on host logits [n_rows][n_vocab]: row k is session k (seeds[k], history of row k) and takes
  * draw first_draw of its stream.  A non-finite logit (NaN or +inf) is B200_EINVAL before anything runs. */
 int b200_extra_sample(b200_extra_t * e, const float * logits, int n_rows, const b200_sampling_t * sp, int32_t * ids);
