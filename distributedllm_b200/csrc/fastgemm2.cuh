@@ -36,6 +36,8 @@ __global__ void __launch_bounds__(256) k_prep_q8_f16(const PrepArgs a) {
     const float * x = a.x + (size_t) n * a.ldx;
     float scale = 1.f;
     if (NORM) {
+        // fast mode is checked against a tolerance, not bit for bit: the tree sum's scale is used as it is (exact mode
+        // certifies it, see rms_scale)
         double s = 0.0;
         for (int i = tid; i < a.K; i += 256) s += (double) fmul(x[i], x[i]);
         for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);

@@ -292,6 +292,35 @@ __device__ __forceinline__ double widen_nonneg(float f) {
     if (u - 0x00800000u < 0x7F000000u) return __hiloint2double((int)((u >> 3) + 0x38000000u), (int)(u << 29));
     return (double) f;
 }
+// ---- RMSNorm scale, the reference's bit for bit (ggml_compute_forward_rms_norm_f32, ggml.c:10334-10348): the reference
+// adds the terms (double)(x_i * x_i) in index order, mean = (float)(sum / K), scale = 1 / sqrtf(mean + 1e-6f).  The norm
+// sites add the same terms as a tree, and the two sums can differ in their last bits; where sum / K lies within that
+// distance of a float rounding boundary, the float mean and the scale differ by one ulp.  Such rows are easy to build
+// (a few large terms whose sum / K is a float tie, then tiny terms that the sequential sum absorbs one by one), so the
+// tree sum is certified instead of trusted:
+//   every term is >= 0, so any order of adding K of them returns T(1 + e), |e| <= g = (K-1)u / (1 - (K-1)u), u = 2^-53,
+//   T the exact sum (Higham, Accuracy and Stability of Numerical Algorithms, 2nd ed., eq. 4.4; additions of an exact 0
+//   are exact, so zero padding does not count).  Hence |S_seq - S| <= 2gT with T <= S / (1 - g), i.e.
+//   |S_seq - S| <= 2(K-1)u / (1 - 2(K-1)u) * S <= 2.001 K u S for K <= 2^41.  B = RU(S * K * 0x1.01p-52) >= 2.0078 K u S.
+//   S -> (float)(S / K) is monotone (two round-to-nearest steps), so when RD(S - B) and RU(S + B) map to one float, that
+//   float is the reference's mean whatever the order of S was.
+// Otherwise the row is summed again in index order.  Every thread that needs the scale calls this with the same S and
+// runs the same branch, so no barrier is needed; in the fallback the threads of a warp load the same addresses.  The
+// fallback loop is not inlined, so it adds no registers to the hot kernels (the check itself does add a few).
+__device__ __noinline__ double rms_seq_sum(const float * x, int K) {
+    double s = 0.0;
+    for (int i = 0; i < K; i++) { const float v = __ldcg(x + i); s = __dadd_rn(s, (double) __fmul_rn(v, v)); }
+    return s;
+}
+
+// scale of the row x[0..K) (global memory; the fallback reads it through L2) whose terms some tree summed to S
+__device__ __forceinline__ float rms_scale(double S, const float * x, int K) {
+    const double k = (double) K, B = __dmul_ru(S, k * 0x1.01p-52);
+    float mean = __double2float_rn(__ddiv_rn(__dsub_rd(S, B), k));
+    if (mean != __double2float_rn(__ddiv_rn(__dadd_ru(S, B), k))) mean = __double2float_rn(__ddiv_rn(rms_seq_sum(x, K), k));
+    return __fdiv_rn(1.0f, __fsqrt_rn(fadd(mean, 1e-6f)));
+}
+
 // rint() of |x| <= 2^22 through the FMA pipe (round-half-even, as F2I.RN / _mm256_round_ps(NEAREST)) instead of XU
 __device__ __forceinline__ int rint_small(float x) { return __float_as_int(fadd(x, kMagic)) - kMagicI; }
 
@@ -512,7 +541,7 @@ __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
                 named_bar_sync(1, kConsumers);
                 const double tot = (red[0] + red[1]) + (red[2] + red[3]);
                 named_bar_sync(1, kConsumers);
-                const float scale = __fdiv_rn(1.0f, __fsqrt_rn(fadd((float)(tot / (double) K), 1e-6f)));
+                const float scale = rms_scale(tot, x, K);
                 if (tid == 0) B200_TRACE(a.trace, 6);
                 if (own) {
                     #pragma unroll
@@ -533,7 +562,7 @@ __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
                     named_bar_sync(1, kConsumers);
                     const double tot = (red[0] + red[1]) + (red[2] + red[3]);
                     named_bar_sync(1, kConsumers);
-                    scale = __fdiv_rn(1.0f, __fsqrt_rn(fadd((float)(tot / (double) K), 1e-6f)));
+                    scale = rms_scale(tot, x, K);
                 }
                 for (int b = tid; b < nb; b += kConsumers) {
                     float v[32];
@@ -716,7 +745,9 @@ __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
         // traffic), THIS kernel finishes the job while the values are still on chip:
         //   every CTA owns exactly one 32-row tile = one Q8_0 block (the host guarantees gridDim.x == n_tiles);
         //   1. partial sum of squares of its block -> global;  2. grid-wide arrive + spin on a counter;
-        //   3. every CTA adds the n_tiles partials in the same fixed order -> identical RMS scale everywhere;
+        //   3. every CTA adds the n_tiles partials in the same fixed order -> identical RMS scale everywhere (rms_scale:
+        //      where the sum is not certified, every CTA re-sums the whole output row from global memory; the row's stores
+        //      of every CTA precede its named barrier, and that barrier precedes lane 0's fence and arrive);
         //   4. normalise, multiply by the norm weight, Q8_0-quantise its own block into the consumer's word layout.
         // All CTAs are co-resident (grid <= SM count x CTAs/SM, and dependents are launched only after every CTA of
         // this grid has started), so the spin cannot deadlock.
@@ -744,7 +775,7 @@ __global__ void __launch_bounds__(kConsumers + 32) k_gemv(const GemvArgs a) {
                 double s = 0.0;
                 for (int i = lane; i < nt; i += 32) s += __ldcg(part + i);
                 for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-                const float scale = __fdiv_rn(1.0f, __fsqrt_rn(fadd((float)(s / (double) a.out_rows), 1e-6f)));
+                const float scale = rms_scale(s, a.y + (size_t)(col0 + n) * a.ldy, a.out_rows);
                 const float val = gq[n * 32 + lane];
                 const float wv = row < a.out_rows ? a.nq_norm_w[row] : 0.f;
                 warp_quant_block(fmul(fmul(val, scale), wv), lane, a.aq_out + (size_t)(col0 + n) * a.out_nbq * 32,
@@ -797,7 +828,7 @@ __global__ void __launch_bounds__(256) k_norm_quant(const NormQuantArgs a) {
     double tot = 0.0;
     #pragma unroll
     for (int i = 0; i < 8; i++) tot += red[i];
-    const float scale = __fdiv_rn(1.0f, __fsqrt_rn(fadd((float)(tot / (double) a.K), 1e-6f)));
+    const float scale = rms_scale(tot, x, a.K);
     int * an = a.aq + (size_t) n * a.nbq * 32;
     float * dn = a.da + (size_t) n * a.nbq * 4;
     for (int b = tid; b < nb; b += 256) {
@@ -848,7 +879,7 @@ __global__ void __launch_bounds__(256) k_gemv_f16(const GemvF16Args a) {
         __syncthreads();
         double tot = 0.0;
         for (int i = 0; i < 8; i++) tot += red[i];
-        scale = __fdiv_rn(1.0f, __fsqrt_rn(fadd((float)(tot / (double) K), 1e-6f)));
+        scale = rms_scale(tot, x, K);
     }
     for (int i = tid; i < K; i += 256) {
         float v = x[i];
@@ -931,7 +962,7 @@ __global__ void __launch_bounds__(256) k_gemv_f16_mc(const GemvF16Args a) {
             __syncthreads();
             double tot = 0.0;
             for (int i = 0; i < 8; i++) tot += red[i];
-            scale = __fdiv_rn(1.0f, __fsqrt_rn(fadd((float)(tot / (double) K), 1e-6f)));
+            scale = rms_scale(tot, x, K);
         }
         for (int i = tid; i < K; i += 256) {
             float v = x[i];
@@ -1107,7 +1138,7 @@ __global__ void __launch_bounds__(kF16Warps * 32 + 32) k_gemv_f16_ring(const Gem
         named_bar_sync(1, kF16Warps * 32);
         double tot = 0.0;
         for (int i = 0; i < kF16Warps; i++) tot += red[i];
-        scale = __fdiv_rn(1.0f, __fsqrt_rn(fadd((float)(tot / (double) K), 1e-6f)));
+        scale = rms_scale(tot, x, K);
     }
     for (int i = tid; i < nc8 * 256; i += kF16Warps * 32) {
         // chunk c = 8 * c8 + j of slot l (element x[c * 32 + l]) -> plane j >> 2, [c8][l][j & 3]

@@ -169,7 +169,7 @@ __global__ void __launch_bounds__(256) k_quant_q8k(const QuantKArgs a) {
         if (lane == 0) red[warp] = s;
         __syncthreads();
         const double tot = ((red[0] + red[1]) + (red[2] + red[3])) + ((red[4] + red[5]) + (red[6] + red[7]));
-        scale = __fdiv_rn(1.0f, __fsqrt_rn(fadd((float)(tot / (double) a.K), 1e-6f)));
+        scale = rms_scale(tot, x, a.K);
     }
     int * aq = a.aq + (size_t) n * a.nbq * 64;
     int * as = a.aq + a.soff + (size_t) n * a.nbq * 8;

@@ -182,6 +182,11 @@ def rewrite(src: str, dst: str, recipe: str) -> str:
                 w = _scale_matrix(t.ttype, w, K_SCALE)
             elif recipe == "extra":
                 w = scale_edges(name, t.ttype, w, name.startswith("tok_embeddings"))
+            elif recipe in ("no_v", "pass") and name.startswith("layers.%d." % f.hparams.first_layer):
+                # the first layer's attention output is 0 (wv = 0), so its ffn norm sees the layer input exactly; with
+                # w2 = 0 as well ("pass") the layer returns its input and the next layer's attention norm sees it
+                if name.endswith("attention.wv.weight") or (recipe == "pass" and name.endswith("feed_forward.w2.weight")):
+                    _zero_rows(w, slice(None))
             yield name, t.ttype, t.ne, np.ascontiguousarray(w).tobytes()
 
     ggjt.write_file(dst, f.hparams, f.vocab, list(gen()))
