@@ -107,7 +107,12 @@ def lib() -> C.CDLL:
                            ("b200_stream_open", [vp, ci, vp, ci, ci, C.POINTER(vp)]),
                            ("b200_stream_add", [vp, ci, vp, ci, ci, vp, vp, ci]),
                            ("b200_stream_read", [vp, vp, vp, ci, C.POINTER(ci)]),
-                           ("b200_stream_cancel", [vp, ci]), ("b200_stream_close", [vp])):
+                           ("b200_stream_cancel", [vp, ci]), ("b200_stream_close", [vp]),
+                           ("b200_stream_fork", [vp, ci, ci, ci]),
+                           ("b200_session_copy", [vp, ci, vp, ci, ci]),
+                           ("b200_session_state_size", [vp, ci, C.POINTER(C.c_size_t)]),
+                           ("b200_session_save", [vp, ci, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+                           ("b200_session_restore", [vp, ci, vp, C.c_size_t])):
             if hasattr(L, name):
                 getattr(L, name).argtypes = args
         if hasattr(L, "b200_extra_token_text"):
@@ -198,6 +203,36 @@ class Slice:
 
     def session_rewind(self, session: int, n_past: int) -> None:
         check(lib().b200_session_rewind(self._h, session, n_past))
+
+    def session_copy(self, src: int, dsts, n_keep: int) -> None:
+        """Rows [0, n_keep) of session src's KV cache to every session in dsts (b200_session_copy), whose positions become
+        n_keep: each then continues bit for bit as src would from n_keep."""
+        src = _int("src", src, 0, 2 ** 31 - 1)
+        if isinstance(dsts, (str, bytes)) or not hasattr(dsts, "__len__"):
+            raise TypeError("dsts must be a sequence of sessions")
+        d = np.array([_int("dsts[%d]" % i, k, 0, 2 ** 31 - 1) for i, k in enumerate(dsts)] or [0], np.int32)
+        if len(dsts) < 1:
+            raise ValueError("dsts needs at least one session")
+        n_keep = _int("n_keep", n_keep, 0, 2 ** 31 - 1)
+        check(lib().b200_session_copy(self._h, src, _ptr(d), len(dsts), n_keep))
+
+    def session_save(self, session: int) -> bytes:
+        """The session's state (b200_session_save): a 64-byte header, then its K and V rows [0, n_past) in fp16."""
+        session = _int("session", session, 0, 2 ** 31 - 1)
+        n = C.c_size_t()
+        check(lib().b200_session_state_size(self._h, session, C.byref(n)))
+        buf = np.empty(n.value, np.uint8)
+        check(lib().b200_session_save(self._h, session, _ptr(buf), n.value, None))
+        return buf.tobytes()
+
+    def session_restore(self, session: int, blob) -> None:
+        """Set the session's rows and position from a session_save blob of a slice of the same shape
+        (b200_session_restore)."""
+        session = _int("session", session, 0, 2 ** 31 - 1)
+        if not isinstance(blob, (bytes, bytearray, memoryview)):
+            raise TypeError("blob must be bytes, bytearray or memoryview, got %s" % type(blob).__name__)
+        buf = np.frombuffer(blob, np.uint8) if len(blob) else np.zeros(1, np.uint8)
+        check(lib().b200_session_restore(self._h, session, _ptr(buf), len(blob)))
 
     def _info(self) -> SliceInfo:
         i = SliceInfo()
@@ -585,6 +620,14 @@ class Stream:
         """End a queued or active session now: its positions reflect the ids read so far."""
         session = _int("session", session, 0, 2 ** 31 - 1)
         check(lib().b200_stream_cancel(self._handle(), session))
+
+    def fork(self, src: int, dst: int, n_keep: int) -> None:
+        """Copy rows [0, n_keep) of session src to session dst on every slice, in order behind the steps in flight
+        (b200_stream_fork); neither may be queued or active.  A following add(dst, ...) continues from n_keep."""
+        src = _int("src", src, 0, 2 ** 31 - 1)
+        dst = _int("dst", dst, 0, 2 ** 31 - 1)
+        n_keep = _int("n_keep", n_keep, 0, 2 ** 31 - 1)
+        check(lib().b200_stream_fork(self._handle(), src, dst, n_keep))
 
     def close(self) -> None:
         if self._h:

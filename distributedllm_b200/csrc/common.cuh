@@ -63,6 +63,15 @@ __device__ __forceinline__ void bulk_g2s(void * dst_smem, const void * src_gmem,
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
                  :: "r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)), "l"(pol) : "memory");
 }
+// 1-D bulk async copy shared -> global, tracked by bulk groups: s2g ... s2g, bulk_commit, then bulk_wait_read<N> before the
+// shared source is overwritten (at most N newer groups may still be reading) and bulk_wait<0> before the CTA exits.
+__device__ __forceinline__ void s2g(void * dst_gmem, const void * src_smem, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+                 :: "l"(dst_gmem), "r"(smem_u32(src_smem)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" :: "n"(N) : "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" :: "n"(N) : "memory"); }
 // 16-byte load that asks L2 to keep the line (evict_last): small, hot, read-every-token data (norm weights) must
 // survive the evict_first weight stream, otherwise every token pays an HBM round trip for it under full load
 __device__ __forceinline__ float4 ldg_keep(const float * p) {

@@ -7,6 +7,7 @@
 #include "kernels.cuh"
 #include "kquant.cuh"
 #include "fastgemm2.cuh"
+#include "kvstate.cuh"
 #include "ggjt_file.hpp"
 
 #include <algorithm>
@@ -55,6 +56,7 @@ struct b200_slice {
     std::vector<int> past;                 // n_past per session
     int * d_npast = nullptr;               // [n_sessions], device copy (graph replays read it)
     size_t sess_stride = 0;                // elements between two sessions' KV caches
+    int * d_kvdst = nullptr;               // [n_sessions]: destination list of the last KV fan-out (k_kv_fanout)
     // batched and mixed passes (begin_pass): segment k runs segs[k].count tokens of session segs[k].session; the device table
     // d_pass holds, per pass, column -> (session, position), segment -> (session, count) and, when a segment has more than
     // one token, column -> row length (the end of its segment) and the tile table of the query-tiled attention
@@ -1205,7 +1207,8 @@ static int load_locked(b200_slice * s, const char * path) {
         (rc = dev_alloc(s, &s->q16, nE)) || (rc = dev_alloc(s, &s->xa, nE)) || (rc = dev_alloc(s, &s->xb, nE)) ||
         (rc = dev_alloc(s, &s->qkv, 3 * nE)) || (rc = dev_alloc(s, &s->att, nE)) || (rc = dev_alloc(s, &s->ffin, nE)) ||
         (rc = dev_alloc(s, &s->gate, (size_t) s->n_ctx * FF)) || (rc = dev_alloc(s, &s->d_in, nE)) ||
-        (rc = dev_alloc(s, &s->d_out, nE)) || (rc = dev_alloc(s, &s->d_npast, (size_t) s->n_sessions)))
+        (rc = dev_alloc(s, &s->d_out, nE)) || (rc = dev_alloc(s, &s->d_npast, (size_t) s->n_sessions)) ||
+        (rc = dev_alloc(s, &s->d_kvdst, (size_t) s->n_sessions)))
         return rc;
     if ((rc = dev_alloc(s, &s->xh, (size_t) s->n_ctx * (FF > E ? FF : E) + 64))) return rc;
     if (wt_kquant(s->wtype)) {
@@ -1280,6 +1283,29 @@ static void destroy(b200_slice * s) {
     for (int i = 0; i < 2; i++) if (s->mark[i]) cudaEventDestroy(s->mark[i]);
     if (s->stream) cudaStreamDestroy(s->stream);
     delete s;
+}
+
+// Session src's cache rows [0, n_keep) to each of dsts[0, n_dst) (distinct, none equal to src; the caller checked), and the
+// destinations' positions to n_keep: host copy now, device copy in order on cs.  A destination's rows at or above n_keep
+// keep their bytes; nothing reads them before it writes them again (attention reads rows below the session's position).
+static int kv_fork(b200_slice * s, int src, const int * dsts, int n_dst, int n_keep, cudaStream_t cs) {
+    if (n_keep > 0) {
+        B200_CUDA(cudaMemcpyAsync(s->d_kvdst, dsts, 4 * (size_t) n_dst, cudaMemcpyHostToDevice, cs));
+        if (int rc = smem_attr<k_kv_fanout>(s, kFanSmem)) return rc;
+        const uint32_t plane = (uint32_t) n_keep * s->E * 2, n_chunks = (plane + kFanChunk - 1) / kFanChunk;
+        const int planes = 2 * s->L;
+        // about three CTAs per SM (64 KB of stages each), so a few loads and every destination's stores are in flight
+        const uint32_t per_plane = std::min<uint32_t>(n_chunks, (uint32_t) std::max(1, (3 * s->n_sm + planes - 1) / planes));
+        k_kv_fanout<<<dim3(per_plane, planes), 32, kFanSmem, cs>>>(s->kc, s->vc, s->sess_stride, (size_t) s->n_ctx * s->E, src,
+                                                                    s->d_kvdst, n_dst, plane);
+        B200_CUDA(cudaGetLastError());
+        s->launches++;
+    }
+    for (int d = 0; d < n_dst; d++) {
+        B200_CUDA(cudaMemcpyAsync(s->d_npast + dsts[d], &n_keep, 4, cudaMemcpyHostToDevice, cs));
+        s->past[dsts[d]] = n_keep;
+    }
+    return 0;
 }
 
 // A handle inside an open generation stream belongs to it: a call from elsewhere fails at once instead of waiting for the
@@ -1432,6 +1458,97 @@ int b200_session_rewind(b200_slice_t * s, int session, int n_past) {
     std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
     if (n_past < 0 || n_past > s->past[session]) return fail(B200_EINVAL, "rewind target %d outside [0, %d]", n_past, s->past[session]);
     B200_CUDA(cudaSetDevice(s->device));
+    B200_CUDA(cudaMemcpyAsync(s->d_npast + session, &n_past, 4, cudaMemcpyHostToDevice, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    s->past[session] = n_past;
+    return 0;
+}
+
+int b200_session_copy(b200_slice_t * s, int src, const int * dsts, int n_dst, int n_keep) {
+    if (!s || !dsts) return fail(B200_EINVAL, "b200_session_copy: null argument");
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
+    if (n_dst < 1) return fail(B200_EINVAL, "b200_session_copy: n_dst must be positive (got %d)", n_dst);
+    if (src < 0 || src >= s->n_sessions) return fail(B200_EINVAL, "source session %d outside [0, %d)", src, s->n_sessions);
+    std::vector<char> seen(s->n_sessions, 0);
+    for (int d = 0; d < n_dst; d++) {
+        const int k = dsts[d];
+        if (k < 0 || k >= s->n_sessions) return fail(B200_EINVAL, "destination %d is session %d, outside [0, %d)", d, k, s->n_sessions);
+        if (k == src) return fail(B200_EINVAL, "destination %d is the source session %d", d, src);
+        if (seen[k]++) return fail(B200_EINVAL, "session %d is listed twice as a destination", k);
+    }
+    if (n_keep < 0 || n_keep > s->past[src])
+        return fail(B200_EINVAL, "n_keep %d outside [0, %d] (the source's position)", n_keep, s->past[src]);
+    B200_CUDA(cudaSetDevice(s->device));
+    if (int rc = kv_fork(s, src, dsts, n_dst, n_keep, s->stream)) return rc;
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    return 0;
+}
+
+/* Session state blob: a 64-byte little-endian header, then K rows [layer][n_past][n_embd] fp16, then V rows alike. */
+namespace {
+constexpr size_t kStateHeader = 64;
+constexpr uint32_t kStateVersion = 1;
+enum { kHdrMagic = 0, kHdrVersion = 4, kHdrEmbd = 8, kHdrHead = 12, kHdrLayer = 16, kHdrFirst = 20, kHdrPast = 24 };
+void put_u32(uint8_t * p, uint32_t v) { for (int i = 0; i < 4; i++) p[i] = (uint8_t) (v >> (8 * i)); }
+uint32_t get_u32(const uint8_t * p) { uint32_t v = 0; for (int i = 0; i < 4; i++) v |= (uint32_t) p[i] << (8 * i); return v; }
+size_t state_bytes(const b200_slice * s, int n_past) { return kStateHeader + (size_t) n_past * s->L * 2 * s->E * 2; }
+}  // namespace
+
+int b200_session_state_size(b200_slice_t * s, int session, size_t * bytes) {
+    if (!s || !bytes) return fail(B200_EINVAL, "b200_session_state_size: null argument");
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
+    if (session < 0 || session >= s->n_sessions) return fail(B200_EINVAL, "session %d outside [0, %d)", session, s->n_sessions);
+    *bytes = state_bytes(s, s->past[session]);
+    return 0;
+}
+
+int b200_session_save(b200_slice_t * s, int session, void * buf, size_t cap, size_t * written) {
+    if (!s || !buf) return fail(B200_EINVAL, "b200_session_save: null argument");
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
+    if (session < 0 || session >= s->n_sessions) return fail(B200_EINVAL, "session %d outside [0, %d)", session, s->n_sessions);
+    const int n_past = s->past[session];
+    const size_t need = state_bytes(s, n_past);
+    if (cap < need) return fail(B200_EINVAL, "b200_session_save: the buffer holds %zu bytes, the state needs %zu", cap, need);
+    uint8_t * h = (uint8_t *) buf;
+    memset(h, 0, kStateHeader);
+    memcpy(h + kHdrMagic, "B2KV", 4);
+    put_u32(h + kHdrVersion, kStateVersion); put_u32(h + kHdrEmbd, s->E); put_u32(h + kHdrHead, s->H);
+    put_u32(h + kHdrLayer, s->L); put_u32(h + kHdrFirst, s->first_layer); put_u32(h + kHdrPast, n_past);
+    const size_t row = (size_t) n_past * s->E * 2, pitch = (size_t) s->n_ctx * s->E * 2;
+    B200_CUDA(cudaSetDevice(s->device));
+    if (row) {
+        B200_CUDA(cudaMemcpy2DAsync(h + kStateHeader, row, s->kc + session * s->sess_stride, pitch, row, s->L, cudaMemcpyDeviceToHost, s->stream));
+        B200_CUDA(cudaMemcpy2DAsync(h + kStateHeader + row * s->L, row, s->vc + session * s->sess_stride, pitch, row, s->L,
+                                    cudaMemcpyDeviceToHost, s->stream));
+    }
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    if (written) *written = need;
+    return 0;
+}
+
+int b200_session_restore(b200_slice_t * s, int session, const void * buf, size_t n) {
+    if (!s || !buf) return fail(B200_EINVAL, "b200_session_restore: null argument");
+    std::lock_guard<std::mutex> lk(s->mu); B200_UNOWNED(s);
+    if (session < 0 || session >= s->n_sessions) return fail(B200_EINVAL, "session %d outside [0, %d)", session, s->n_sessions);
+    const uint8_t * h = (const uint8_t *) buf;
+    if (n < kStateHeader || memcmp(h + kHdrMagic, "B2KV", 4) != 0) return fail(B200_EINVAL, "b200_session_restore: not a session state");
+    if (get_u32(h + kHdrVersion) != kStateVersion)
+        return fail(B200_EINVAL, "b200_session_restore: state version %u, this library reads %u", get_u32(h + kHdrVersion), kStateVersion);
+    const int E = (int) get_u32(h + kHdrEmbd), H = (int) get_u32(h + kHdrHead), L = (int) get_u32(h + kHdrLayer),
+              first = (int) get_u32(h + kHdrFirst), n_past = (int) get_u32(h + kHdrPast);
+    if (E != s->E || H != s->H || L != s->L || first != s->first_layer)
+        return fail(B200_EINVAL, "b200_session_restore: the state is of n_embd %d, n_head %d, layers %d..%d; the slice of %d, %d, %d..%d",
+                    E, H, first, first + L - 1, s->E, s->H, s->first_layer, s->first_layer + s->L - 1);
+    if (n_past < 0 || n_past > s->n_ctx) return fail(B200_EINVAL, "b200_session_restore: n_past %d outside [0, n_ctx %d]", n_past, s->n_ctx);
+    if (n != state_bytes(s, n_past))
+        return fail(B200_EINVAL, "b200_session_restore: %zu bytes, a state of %d positions has %zu", n, n_past, state_bytes(s, n_past));
+    const size_t row = (size_t) n_past * s->E * 2, pitch = (size_t) s->n_ctx * s->E * 2;
+    B200_CUDA(cudaSetDevice(s->device));
+    if (row) {
+        B200_CUDA(cudaMemcpy2DAsync(s->kc + session * s->sess_stride, pitch, h + kStateHeader, row, row, s->L, cudaMemcpyHostToDevice, s->stream));
+        B200_CUDA(cudaMemcpy2DAsync(s->vc + session * s->sess_stride, pitch, h + kStateHeader + row * s->L, row, row, s->L,
+                                    cudaMemcpyHostToDevice, s->stream));
+    }
     B200_CUDA(cudaMemcpyAsync(s->d_npast + session, &n_past, 4, cudaMemcpyHostToDevice, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     s->past[session] = n_past;
@@ -3811,6 +3928,26 @@ int b200_stream_cancel(b200_stream_t * st, int session) {
     if (session < 0 || session >= st->n_sess || st->sess[session].state == 0)
         return fail(B200_EINVAL, "session %d is not in the stream", session);
     return stream_finish(st, session);
+}
+
+int b200_stream_fork(b200_stream_t * st, int src, int dst, int n_keep) {
+    std::vector<std::unique_lock<std::mutex>> locks;
+    if (int rc = stream_lock(st, locks)) return rc;
+    for (int k : {src, dst}) {
+        if (k < 0 || k >= st->n_sess) return fail(B200_EINVAL, "session %d outside [0, %d)", k, st->n_sess);
+        if (st->sess[k].state) return fail(B200_EINVAL, "session %d is %s", k, st->sess[k].state == 1 ? "queued" : "active");
+    }
+    if (src == dst) return fail(B200_EINVAL, "b200_stream_fork: source and destination are both session %d", src);
+    for (size_t i = 0; i < st->slices.size(); i++) {
+        const int p = st->slices[i]->past[src];
+        if (p != st->slices[0]->past[src])
+            return fail(B200_EINVAL, "session %d is at position %d on slice 0 and %d on slice %zu", src, st->slices[0]->past[src], p, i);
+        if (n_keep < 0 || n_keep > p) return fail(B200_EINVAL, "n_keep %d outside [0, %d] (session %d's position)", n_keep, p, src);
+    }
+    // in stream order, behind every step still in flight for either session
+    for (b200_slice * s : st->slices)
+        if (int rc = kv_fork(s, src, &dst, 1, n_keep, st->e->ctx.stream)) return rc;
+    return 0;
 }
 
 int b200_stream_close(b200_stream_t * st) {

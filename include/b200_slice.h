@@ -92,6 +92,28 @@ int b200_session_count(b200_slice_t * s);
 int b200_session_n_past(b200_slice_t * s, int session);                      /* -1 on a bad argument */
 int b200_session_clear(b200_slice_t * s, int session);                       /* session -1 = every session */
 int b200_session_rewind(b200_slice_t * s, int session, int n_past);
+/* Session state on the device and off it.  A session's state is its cache rows [0, n_past) and its position; two sessions
+ * with the same rows at the same position give bit-identical results (no arithmetic depends on a session's index), so a
+ * copied or restored session continues exactly as its source would have.  Each call below takes the handle's mutex, is
+ * refused while a generation stream owns the handle, is all-or-nothing (on an error no position moves and no cache byte
+ * changes) and synchronises the slice's stream before it returns.
+ * b200_session_copy: rows [0, n_keep) of every layer's K and V cache of session src to each of dsts[0, n_dst) in one
+ *   launch (each source byte is read once), and each destination's position to n_keep.  Nothing else changes: not src,
+ *   not other sessions, not a destination's rows at or above n_keep.  B200_EINVAL: a null handle or dsts, n_dst < 1, a
+ *   session outside [0, n_sessions), a destination equal to src or listed twice, n_keep outside [0, n_past of src]. */
+int b200_session_copy(b200_slice_t * s, int src, const int * dsts, int n_dst, int n_keep);
+/* Bytes b200_session_save writes for the session now: 64 + n_past * kv_bytes_per_pos. */
+int b200_session_state_size(b200_slice_t * s, int session, size_t * bytes);
+/* The session's state into buf (host memory, pageable or pinned; the copy has finished when the call returns).  Layout,
+ * little-endian: a 64-byte header (bytes 0-3 "B2KV", then uint32 version 1, n_embd, n_head, n_layer, first_layer, n_past,
+ * zero padding), then the K rows [layer][n_past][n_embd] fp16, then the V rows alike.  *written (may be NULL) = the size.
+ * B200_EINVAL: cap < the size (nothing is written), a null handle or buf, a session out of range. */
+int b200_session_save(b200_slice_t * s, int session, void * buf, size_t cap, size_t * written);
+/* Sets the session's rows [0, n_past) and its position from a blob of b200_session_save, taken from any handle of the same
+ * n_embd, n_head, n_layer and first_layer, at any n_ctx >= n_past and any n_sessions.  The blob does not identify the
+ * weights: restoring into a different model of the same shape succeeds and is the caller's mistake.  B200_EINVAL (the
+ * session untouched): a bad magic, version or shape, n_past > n_ctx, n different from the blob's exact size. */
+int b200_session_restore(b200_slice_t * s, int session, const void * buf, size_t n);
 int b200_session_forward(b200_slice_t * s, int session, const float * in, int n_tokens, float * out);          /* host buffers */
 int b200_session_forward_device(b200_slice_t * s, int session, const float * d_in, int n_tokens, float * d_out, int sync);
 
@@ -384,6 +406,14 @@ int b200_stream_add(b200_stream_t * st, int session, const int32_t * prompt, int
                     const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop);
 int b200_stream_read(b200_stream_t * st, int32_t * sessions, int32_t * ids, int cap, int * n_out);
 int b200_stream_cancel(b200_stream_t * st, int session);
+/* b200_session_copy for sessions of an open stream, with one destination, on every slice of its chain: rows [0, n_keep)
+ * of src to dst and dst's position to n_keep.  Enqueued on the stream's CUDA stream, so it runs after every step still in
+ * flight for either session (steps left over from an earlier stay write only rows at or above that session's final
+ * n_past, and the copy wins on any overlap); nothing synchronises.  dst's host position is n_keep at once, so a following
+ * b200_stream_add(dst, suffix, ...) checks its context against n_keep and continues from there.  B200_EINVAL: either
+ * session out of range, queued or active, src == dst, n_keep outside [0, n_past of src] on a slice, or slices whose
+ * n_past of src differ. */
+int b200_stream_fork(b200_stream_t * st, int src, int dst, int n_keep);
 int b200_stream_close(b200_stream_t * st);
 /* llm.tokenize_prompt(path, prompt): BOS + sentencepiece-style merge (tensor_processor.cpp:1596-1714).
  * Returns the token count (may exceed cap; only cap are written) or a negative error. */
