@@ -33,6 +33,13 @@ class Sampling(C.Structure):
                 ("top_k", C.c_int32), ("top_p", C.c_double)]
 
 
+class Logprobs(C.Structure):
+    """b200_logprobs_t."""
+    _fields_ = [("n_top", C.c_int32), ("lp", C.c_void_p), ("top_ids", C.c_void_p), ("top_lp", C.c_void_p)]
+
+
+MAX_TOP = 20            # the most alternatives a logprobs call returns per id (OpenAI's top_logprobs cap)
+
 _lib: Optional[C.CDLL] = None
 
 
@@ -108,6 +115,11 @@ def lib() -> C.CDLL:
                            ("b200_stream_add", [vp, ci, vp, ci, ci, vp, vp, ci]),
                            ("b200_stream_read", [vp, vp, vp, ci, C.POINTER(ci)]),
                            ("b200_stream_cancel", [vp, ci]), ("b200_stream_close", [vp]),
+                           ("b200_generate_lp", [vp, ci, vp, vp, vp, ci, vp, ci, vp, vp, vp]),
+                           ("b200_generate_speculative_lp", [vp, ci, vp, ci, vp, ci, vp, ci, vp, ci, ci, ci, vp, vp, vp, vp]),
+                           ("b200_extra_logprobs", [vp, vp, ci, vp, ci, vp, vp, vp]),
+                           ("b200_stream_add_lp", [vp, ci, vp, ci, ci, vp, vp, ci, ci]),
+                           ("b200_stream_read_lp", [vp, vp, vp, vp, vp, vp, ci, C.POINTER(ci)]),
                            ("b200_stream_fork", [vp, ci, ci, ci]),
                            ("b200_session_copy", [vp, ci, vp, ci, ci]),
                            ("b200_session_state_size", [vp, ci, C.POINTER(C.c_size_t)]),
@@ -412,6 +424,20 @@ class Extra:
         check(lib().b200_extra_nll(self._h, _ptr(x), len(x), _ptr(t), _ptr(out)))
         return out
 
+    def logprobs(self, logits: np.ndarray, ids, n_top: int):
+        """k_logprob_rows on the device (b200_extra_logprobs): for each row of [n][n_vocab] logits, log softmax(row)[ids[k]]
+        in float64 and the n_top ids of largest logit (equal logits: lower id first) with theirs.
+        -> (lp [n], top_ids [n][n_top], top_lp [n][n_top])."""
+        x = np.ascontiguousarray(logits, dtype=np.float32).reshape(-1, self.n_vocab)
+        t = np.ascontiguousarray(ids, dtype=np.int32)
+        if len(t) != len(x):
+            raise ValueError("need one id per row (%d), got %d" % (len(x), len(t)))
+        n_top = _n_top(n_top, self.n_vocab)
+        out = _LpOut((len(x),), n_top)
+        check(lib().b200_extra_logprobs(self._h, _ptr(x), len(x), _ptr(t), n_top, _ptr(out.lp), _ptr(out.top_ids),
+                                        _ptr(out.top_lp)))
+        return out.lp, out.top_ids, out.top_lp
+
     def close(self) -> None:
         if self._h:
             check(lib().b200_extra_unload(self._h))
@@ -424,9 +450,26 @@ class Extra:
             pass
 
 
-def generate_greedy(slices, extra: Extra, sessions, prompts, n_steps: int) -> np.ndarray:
+def _n_top(n_top, n_vocab: int) -> int:
+    return _int("logprobs", n_top, 0, min(MAX_TOP, n_vocab))
+
+
+class _LpOut:
+    """The output arrays of a logprobs call for ids of `shape`, and the b200_logprobs_t that points into them."""
+
+    def __init__(self, shape, n_top: int):
+        self.lp = np.full(shape, np.nan, np.float64)
+        self.top_ids = np.full(tuple(shape) + (n_top,), -1, np.int32)
+        self.top_lp = np.full(tuple(shape) + (n_top,), np.nan, np.float64)
+        self.c = Logprobs(n_top, self.lp.ctypes.data, self.top_ids.ctypes.data if n_top else None,
+                          self.top_lp.ctypes.data if n_top else None)
+
+
+def generate_greedy(slices, extra: Extra, sessions, prompts, n_steps: int, logprobs: Optional[int] = None):
     """Greedy decoding on the device (b200_generate_greedy): session sessions[k] is fed prompts[k] (a list of token ids),
-    then n_steps - 1 of its own ids.  `slices` are in layer order, all on the extra layers' GPU.  -> [n_steps][n_seq] ids."""
+    then n_steps - 1 of its own ids.  `slices` are in layer order, all on the extra layers' GPU.  -> [n_steps][n_seq] ids.
+    logprobs = n_top (0..20): b200_generate_lp instead, -> (ids, lp [n_steps][n_seq], top_ids and top_lp
+    [n_steps][n_seq][n_top]) in the raw distribution (include/b200_slice.h)."""
     ids = np.ascontiguousarray(sessions, dtype=np.int32)
     if len(prompts) != len(ids):
         raise ValueError("need one prompt per listed session")
@@ -435,6 +478,11 @@ def generate_greedy(slices, extra: Extra, sessions, prompts, n_steps: int) -> np
                                 dtype=np.int32)
     handles = (C.c_void_p * max(len(slices), 1))(*[s.handle for s in slices])
     out = np.zeros((max(n_steps, 0), len(ids)), np.int32)
+    if logprobs is not None:
+        lp = _LpOut(out.shape, _n_top(logprobs, extra.n_vocab))
+        check(lib().b200_generate_lp(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks),
+                                     n_steps, None, _ptr(out), C.byref(lp.c)))
+        return out, lp.lp, lp.top_ids, lp.top_lp
     check(lib().b200_generate_greedy(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks),
                                      n_steps, _ptr(out)))
     return out
@@ -470,11 +518,12 @@ def _sampling(n: int, temperature: float, repeat_penalty: float, seeds, first_dr
 
 
 def generate_sample(slices, extra: Extra, sessions, prompts, n_steps: int, temperature: float, repeat_penalty: float,
-                    seeds, first_draw: int = 0, history=None, top_k: int = 0, top_p: float = 0.0) -> np.ndarray:
+                    seeds, first_draw: int = 0, history=None, top_k: int = 0, top_p: float = 0.0,
+                    logprobs: Optional[int] = None):
     """Sampled generation on the device (b200_generate_sample): generate_greedy's loop with the client's Sampler in place
     of the argmax.  Session sessions[k] draws from numpy.random.Philox(key=seeds[k]) starting at draw first_draw, with
     history[k] (ids it sampled before) penalised and every row truncated to top_k / top_p (0: off).
-    -> [n_steps][n_seq] ids."""
+    -> [n_steps][n_seq] ids; with logprobs = n_top, (ids, lp, top_ids, top_lp) as generate_greedy."""
     ids = np.ascontiguousarray(sessions, dtype=np.int32)
     if len(prompts) != len(ids):
         raise ValueError("need one prompt per listed session")
@@ -484,6 +533,11 @@ def generate_sample(slices, extra: Extra, sessions, prompts, n_steps: int, tempe
                                 dtype=np.int32)
     handles = (C.c_void_p * max(len(slices), 1))(*[s.handle for s in slices])
     out = np.zeros((max(n_steps, 0), len(ids)), np.int32)
+    if logprobs is not None:
+        lp = _LpOut(out.shape, _n_top(logprobs, extra.n_vocab))
+        check(lib().b200_generate_lp(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks),
+                                     n_steps, C.byref(sp), _ptr(out), C.byref(lp.c)))
+        return out, lp.lp, lp.top_ids, lp.top_lp
     check(lib().b200_generate_sample(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks),
                                      n_steps, C.byref(sp), _ptr(out)))
     return out
@@ -495,11 +549,13 @@ class SpecStats(C.Structure):
 
 def generate_speculative(slices, extra: Extra, session: int, draft_slices, draft_extra: Extra, draft_session: int, prompt,
                          n_steps: int, n_draft: int, temperature: Optional[float] = None, repeat_penalty: float = 1.1,
-                         seed: Optional[int] = None, first_draw: int = 0, history=None, top_k: int = 0, top_p: float = 0.0):
+                         seed: Optional[int] = None, first_draw: int = 0, history=None, top_k: int = 0, top_p: float = 0.0,
+                         logprobs: Optional[int] = None):
     """Speculative decoding on the device (b200_generate_speculative): the draft chain proposes n_draft ids per
     iteration, one pass of the target checks them.  temperature None: greedy, the ids of generate_greedy; else the ids of
     generate_sample with the same settings (seed: the session's Philox key; history: the ids it sampled before).
-    -> (ids [n_steps] int32, {"passes", "drafted", "accepted"})."""
+    -> (ids [n_steps] int32, {"passes", "drafted", "accepted"}); with logprobs = n_top (b200_generate_speculative_lp),
+    ((ids, lp [n_steps], top_ids, top_lp [n_steps][n_top]), stats), equal to the plain loop's."""
     toks = np.ascontiguousarray([int(t) for t in prompt], dtype=np.int32)
     handles = (C.c_void_p * max(len(slices), 1))(*[s.handle for s in slices])
     dhandles = (C.c_void_p * max(len(draft_slices), 1))(*[s.handle for s in draft_slices])
@@ -511,11 +567,17 @@ def generate_speculative(slices, extra: Extra, session: int, draft_slices, draft
                              top_k, top_p)
     out = np.zeros(max(n_steps, 0), np.int32)
     stats = SpecStats()
-    check(lib().b200_generate_speculative(handles, len(slices), extra.handle, session, dhandles, len(draft_slices),
-                                          draft_extra.handle, draft_session, _ptr(toks), len(toks), n_steps, n_draft,
-                                          C.byref(sp) if sp is not None else None, _ptr(out), C.byref(stats)))
+    args = (handles, len(slices), extra.handle, session, dhandles, len(draft_slices), draft_extra.handle, draft_session,
+            _ptr(toks), len(toks), n_steps, n_draft, C.byref(sp) if sp is not None else None, _ptr(out), C.byref(stats))
+    lp = None
+    if logprobs is not None:
+        lp = _LpOut(out.shape, _n_top(logprobs, extra.n_vocab))
+        check(lib().b200_generate_speculative_lp(*args, C.byref(lp.c)))
+    else:
+        check(lib().b200_generate_speculative(*args))
     del keep
-    return out, {"passes": stats.passes, "drafted": stats.drafted, "accepted": stats.accepted}
+    st = {"passes": stats.passes, "drafted": stats.drafted, "accepted": stats.accepted}
+    return ((out, lp.lp, lp.top_ids, lp.top_lp) if lp is not None else out), st
 
 
 def score(slices, extra: Extra, sessions, token_lists) -> list:
@@ -581,11 +643,13 @@ class Stream:
         return self._h
 
     def add(self, session: int, prompt, max_tokens: int, temperature: Optional[float] = None, repeat_penalty: float = 1.1,
-            seed: int = 0, first_draw: int = 0, history=None, stop_ids=(), top_k: int = 0, top_p: float = 0.0) -> None:
+            seed: int = 0, first_draw: int = 0, history=None, stop_ids=(), top_k: int = 0, top_p: float = 0.0,
+            logprobs: Optional[int] = None) -> None:
         """Queue `session` with `prompt` (token ids) for at most max_tokens ids.  temperature None: greedy (the argmax of
         the raw logits); else the client's Sampler with repeat_penalty on numpy.random.Philox(key=seed), starting at draw
         first_draw, with history (ids sampled before) penalised, truncated to top_k / top_p (0: off).  The session ends
-        after the first id in stop_ids."""
+        after the first id in stop_ids.  logprobs = n_top (0..20): each id's record (read_logprobs) holds its
+        log-probability and n_top alternatives (b200_stream_add_lp)."""
         session = _int("session", session, 0, 2 ** 31 - 1)
         p = _ids("prompt", prompt, self.n_vocab, 1)
         max_tokens = _int("max_tokens", max_tokens, 1, 2 ** 31 - 1)
@@ -604,6 +668,11 @@ class Stream:
             sp, keep = _sampling(1, t, rp, [seed], first_draw, history, top_k, top_p)
         elif history is not None or first_draw or _truncation(top_k, top_p) != (0, 0.0):
             raise ValueError("history, first_draw, top_k and top_p apply to sampled sessions (give a temperature)")
+        if logprobs is not None:
+            n_top = _n_top(logprobs, self.n_vocab)
+            check(lib().b200_stream_add_lp(self._handle(), session, _ptr(p), len(prompt), max_tokens,
+                                           None if sp is None else C.byref(sp), _ptr(stops), len(stop_ids), n_top))
+            return
         check(lib().b200_stream_add(self._handle(), session, _ptr(p), len(prompt), max_tokens,
                                     None if sp is None else C.byref(sp), _ptr(stops), len(stop_ids)))
 
@@ -615,6 +684,18 @@ class Stream:
         sess, ids, n = np.zeros(cap, np.int32), np.zeros(cap, np.int32), C.c_int()
         check(lib().b200_stream_read(h, _ptr(sess), _ptr(ids), cap, C.byref(n)))
         return list(zip(sess[:n.value].tolist(), ids[:n.value].tolist()))
+
+    def read_logprobs(self, cap: int = 64) -> list:
+        """read() with each id's record (b200_stream_read_lp): up to cap (session, id, lp, [(id, lp), ...]) tuples, the
+        list holding the session's n_top alternatives.  A session added without logprobs gives lp NaN and no
+        alternatives."""
+        cap = _int("cap", cap, 1, 2 ** 20)
+        h = self._handle()
+        sess, ids, n = np.zeros(cap, np.int32), np.zeros(cap, np.int32), C.c_int()
+        lp = np.zeros(cap, np.float64)
+        top_ids, top_lp = np.zeros((cap, MAX_TOP), np.int32), np.zeros((cap, MAX_TOP), np.float64)
+        check(lib().b200_stream_read_lp(h, _ptr(sess), _ptr(ids), _ptr(lp), _ptr(top_ids), _ptr(top_lp), cap, C.byref(n)))
+        return unpack_records(sess[:n.value], ids[:n.value], lp[:n.value], top_ids[:n.value], top_lp[:n.value])
 
     def cancel(self, session: int) -> None:
         """End a queued or active session now: its positions reflect the ids read so far."""
@@ -652,3 +733,12 @@ class Stream:
             self.close()
         except Exception:
             pass
+
+
+def unpack_records(sessions, ids, lp, top_ids, top_lp) -> list:
+    """b200_stream_read_lp's rows (top_* of stride 20, unused entries -1) -> (session, id, lp, [(id, lp), ...])."""
+    out = []
+    for k in range(len(ids)):
+        alts = [(int(t), float(v)) for t, v in zip(top_ids[k], top_lp[k]) if t >= 0]
+        out.append((int(sessions[k]), int(ids[k]), float(lp[k]), alts))
+    return out

@@ -14,6 +14,7 @@ from typing import List, Sequence, Tuple
 
 import numpy as np
 
+from .capi import MAX_TOP, _int
 from .compute_node.slices import import_llm
 from .control_center import Connection
 
@@ -53,6 +54,28 @@ def _softmax(x: np.ndarray, axis=-1) -> np.ndarray:
     x = x - x.max(axis=axis, keepdims=True)
     e = np.exp(x)
     return e / e.sum(axis=axis, keepdims=True)
+
+
+def token_logprobs(logits, token, n_top: int):
+    """The log-probability of `token` under the raw distribution softmax(logits) in float64, and the n_top ids of largest
+    logit (equal logits: lower id first) with theirs: the host twin of the device's logprobs (include/b200_slice.h).
+    -> (lp, [(id, lp), ...]).  A row with a NaN or +inf logit, or all -inf, has no distribution: lp NaN and every
+    alternative (-1, NaN).  A token whose probability underflows gives -inf.  The sum runs in numpy's order, so values
+    agree with the device's within ~1e-15 relative, not bit for bit."""
+    x = np.asarray(logits, dtype=np.float32).reshape(-1).astype(np.float64)
+    n = len(x)
+    if n < 1:
+        raise ValueError("logits must hold at least one value")
+    token = _int("token", token, 0, n - 1)
+    n_top = _int("n_top", n_top, 0, min(MAX_TOP, n))
+    if np.isnan(x).any() or (x == np.inf).any() or (x == -np.inf).all():
+        return float("nan"), [(-1, float("nan"))] * n_top
+    with np.errstate(divide="ignore"):
+        e = np.exp(x - x.max())
+        S = e.sum()
+        lp = lambda i: float(np.log(e[i] / S))
+        top = np.lexsort((np.arange(n), -x))[:n_top]
+        return lp(token), [(int(i), lp(i)) for i in top]
 
 
 class Sampler:
@@ -106,19 +129,28 @@ class DistributedLLM:
         self.wire = wire
         self.llm = import_llm()
 
-    def generate(self, prompt, max_steps=200, temperature=0.0, repeat_penalty=1.1, rng=None, top_k=None, top_p=None):
+    def generate(self, prompt, max_steps=200, temperature=0.0, repeat_penalty=1.1, rng=None, top_k=None, top_p=None,
+                 logprobs=None):
         """rng: the Sampler's random generator (default numpy's global one, as the reference);
         numpy.random.Generator(numpy.random.Philox(key=seed)) gives LocalPipeline.generate's ids for that seed.
-        top_k / top_p: the Sampler's truncation (None: off)."""
+        top_k / top_p: the Sampler's truncation (None: off).  logprobs = n_top (0..20): yield (text, lp, [(id, lp), ...])
+        instead of text, from token_logprobs on each step's logits."""
+        if logprobs is not None:
+            logprobs = _int("logprobs", logprobs, 0, MAX_TOP)
         self.clear_context()
         extra = self.extra_layers_path
         tokens = self.llm.tokenize_prompt(extra, prompt)
         sampler = Sampler(temperature, repeat_penalty, rng=rng, top_k=top_k, top_p=top_p)
         for _ in range(max_steps):
             emb = self.propagate_tensor(self.llm.prepare_embeddings(extra, tokens))
-            token_id = sampler(self.llm.get_logits(extra, emb, False))
+            logits = self.llm.get_logits(extra, emb, False)
+            token_id = sampler(logits)
             tokens = [token_id]
-            yield self.llm.decode_token(extra, token_id)
+            text = self.llm.decode_token(extra, token_id)
+            if logprobs is None:
+                yield text
+            else:
+                yield (text, *token_logprobs(logits, token_id, logprobs))
 
     def generate_greedy(self, prompt, max_steps=200) -> List[int]:
         """Pure argmax decoding through llm.get_next_token (tensor_processor.cpp:1894-1908): the parity path."""
@@ -191,19 +223,25 @@ class LocalPipeline:
             self._extra = (extra_path, self.capi.Extra(extra_path, devices[0]))
         return self._extra[1]
 
-    def generate_greedy(self, extra_path: str, prompt: str, max_steps: int = 200) -> List[int]:
+    def generate_greedy(self, extra_path: str, prompt: str, max_steps: int = 200, logprobs: int = None) -> list:
         """DistributedLLM.generate_greedy on this box: clear the contexts, tokenize, then max_steps argmax steps, all on
-        the GPU with no host round trip between tokens (capi.generate_greedy).  Needs every slice on one device."""
+        the GPU with no host round trip between tokens (capi.generate_greedy).  Needs every slice on one device.
+        logprobs = n_top (0..20): a list of (id, lp, [(id, lp), ...]) instead of ids."""
         extra = self._device_extra(extra_path, "greedy generation")
+        if logprobs is not None:
+            logprobs = _int("logprobs", logprobs, 0, MAX_TOP)
         self.clear_context()
         tokens = extra.tokenize(prompt)
         if max_steps < 1:
             return []
-        return self.capi.generate_greedy(self.slices, extra, [0], [tokens], max_steps)[:, 0].tolist()
+        if logprobs is None:
+            return self.capi.generate_greedy(self.slices, extra, [0], [tokens], max_steps)[:, 0].tolist()
+        ids, lp, ti, tl = self.capi.generate_greedy(self.slices, extra, [0], [tokens], max_steps, logprobs=logprobs)
+        return _with_logprobs(ids[:, 0], lp[:, 0], ti[:, 0], tl[:, 0])
 
     def generate(self, extra_path: str, prompt: str, max_steps: int = 200, temperature: float = 0.0,
                  repeat_penalty: float = 1.1, seed: int = None, stop_at_eos: bool = False, top_k: int = None,
-                 top_p: float = None):
+                 top_p: float = None, logprobs: int = None):
         """DistributedLLM.generate on this box: clear the contexts, tokenize, then up to max_steps steps of the client's
         Sampler, all on the GPU with no host round trip between tokens (a one-session capi.Stream).  Yields each token
         string as soon as its id is drawn; leaving the loop early cancels the steps that remain, and the slices' n_past
@@ -211,9 +249,12 @@ class LocalPipeline:
         DistributedLLM.generate(..., rng=numpy.random.Generator(numpy.random.Philox(key=seed))) yields the same strings.
         seed=None draws a key from numpy's global generator, so unseeded runs vary as the reference's do.
         stop_at_eos=True ends the run after the end-of-sequence id (EOS_ID, yielded); the default runs max_steps steps,
-        as the reference does.  top_k / top_p truncate each draw as client.Sampler does (None: off).  Needs every slice
-        on one device."""
+        as the reference does.  top_k / top_p truncate each draw as client.Sampler does (None: off).  logprobs = n_top
+        (0..20): yield (text, lp, [(id, lp), ...]) as DistributedLLM.generate does, from the stream's records.  Needs
+        every slice on one device."""
         extra = self._device_extra(extra_path, "sampled generation")
+        if logprobs is not None:
+            logprobs = _int("logprobs", logprobs, 0, MAX_TOP)
         if seed is None:
             seed = int(np.random.randint(0, 2 ** 64, dtype=np.uint64))
         self.clear_context()
@@ -222,21 +263,29 @@ class LocalPipeline:
             return
         with self.capi.Stream(self.slices, extra) as st:
             st.add(0, tokens, max_steps, temperature, repeat_penalty, seed, stop_ids=[EOS_ID] if stop_at_eos else (),
-                   top_k=top_k or 0, top_p=top_p or 0.0)
-            for j, (_, token_id) in enumerate(st):
+                   top_k=top_k or 0, top_p=top_p or 0.0, logprobs=logprobs)
+            records = iter(st) if logprobs is None else _read_records(st)
+            for j, rec in enumerate(records):
+                token_id = rec[1]
                 if token_id < 0:
                     raise self.capi.B200Error(1, "step %d: the logits hold a NaN or +inf, are all -inf or overflow "
                                                  "float64 once scaled, so they have no distribution" % j)
-                yield extra.token_text(token_id)
+                if logprobs is None:
+                    yield extra.token_text(token_id)
+                else:
+                    yield extra.token_text(token_id), rec[2], rec[3]
 
     def generate_speculative(self, extra_path: str, prompt: str, draft: "LocalPipeline", draft_extra_path: str,
                              max_steps: int = 200, n_draft: int = 4, temperature: float = 0.0, repeat_penalty: float = 1.1,
-                             seed: int = None, top_k: int = None, top_p: float = None) -> List[int]:
+                             seed: int = None, top_k: int = None, top_p: float = None, logprobs: int = None) -> list:
         """Speculative decoding on this box (capi.generate_speculative): clear both pipelines' contexts, tokenize with the
         target's extra layers, then max_steps ids, the draft pipeline proposing n_draft ids per target pass.  The ids do
         not depend on the draft: at temperature 0 they are generate_greedy's; otherwise the ids behind the strings
-        generate(..., seed=seed, stop_at_eos=False) yields.  Needs every slice of both pipelines on one device."""
+        generate(..., seed=seed, stop_at_eos=False) yields.  Needs every slice of both pipelines on one device.
+        logprobs = n_top (0..20): a list of (id, lp, [(id, lp), ...]) instead of ids, equal to the plain loop's."""
         extra = self._device_extra(extra_path, "speculative generation")
+        if logprobs is not None:
+            logprobs = _int("logprobs", logprobs, 0, MAX_TOP)
         dextra = draft._device_extra(draft_extra_path, "speculative generation")
         if temperature and seed is None:
             seed = int(np.random.randint(0, 2 ** 64, dtype=np.uint64))
@@ -245,11 +294,11 @@ class LocalPipeline:
         tokens = extra.tokenize(prompt)
         if max_steps < 1:
             return []
-        ids, _ = self.capi.generate_speculative(self.slices, extra, 0, draft.slices, dextra, 0, tokens, max_steps, n_draft,
+        out, _ = self.capi.generate_speculative(self.slices, extra, 0, draft.slices, dextra, 0, tokens, max_steps, n_draft,
                                                 temperature=temperature if temperature else None,
                                                 repeat_penalty=repeat_penalty, seed=seed, top_k=top_k or 0,
-                                                top_p=top_p or 0.0)
-        return ids.tolist()
+                                                top_p=top_p or 0.0, logprobs=logprobs)
+        return out.tolist() if logprobs is None else _with_logprobs(*out)
 
     def perplexity(self, extra_path: str, text: str) -> float:
         """DistributedLLM.perplexity on this box: clear the contexts, tokenize, then score the text on the GPU
@@ -281,3 +330,17 @@ class LocalPipeline:
             self._extra = None
         for s in self.slices:
             s.close()
+
+
+def _with_logprobs(ids, lp, top_ids, top_lp) -> list:
+    """Arrays of a logprobs call for one session -> [(id, lp, [(id, lp), ...]), ...]."""
+    return [(int(t), float(v), [(int(a), float(b)) for a, b in zip(ti, tl)]) for t, v, ti, tl in zip(ids, lp, top_ids, top_lp)]
+
+
+def _read_records(st):
+    """A stream's (session, id, lp, alternatives) records, one at a time, until no session is left."""
+    while True:
+        recs = st.read_logprobs(1)
+        if not recs:
+            return
+        yield recs[0]

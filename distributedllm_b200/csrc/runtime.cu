@@ -2143,6 +2143,8 @@ struct b200_extra {
     uint32_t * d_pen = nullptr; uint64_t * d_seeds = nullptr; int * d_bad = nullptr; int cap_sample = 0;
     // scoring (b200_score): the embedded rows of one pass [rows][n_embd], and the NLL of every scored row
     float * d_sx = nullptr; int cap_sx = 0; double * d_nll = nullptr; int cap_nll = 0;
+    // log-probabilities (k_logprob_rows): lp [rows], top ids and their lp [rows][n_top]
+    double * d_lp = nullptr; int cap_lp = 0; int32_t * d_topi = nullptr; int cap_topi = 0; double * d_topl = nullptr; int cap_topl = 0;
     std::vector<std::pair<std::string, float>> vocab;
     std::unordered_map<std::string, int> token_to_id;
     std::mutex mu;
@@ -2631,8 +2633,9 @@ __global__ void __launch_bounds__(1024) k_sample_rows(SampleArgs a) {
 
 // ---- generation streams (b200_stream_*): the sampler's state lives in per-session slots, and a step's rows name their slot
 struct StreamSlot { uint64_t seed; double dt, dp; int sampled, top_k; double top_p; };   // device table, one per session
-struct StreamRow { long long draw; int slot, gather; };              // per step, in mapped pinned memory: draw index, slot,
-                                                                    // and the session's last row in the pass
+struct StreamRow { long long draw; int slot, gather, n_top; };       // per step, in mapped pinned memory: draw index, slot,
+                                                                    // the session's last row in the pass, and its top-n
+                                                                    // (-1: no log-probabilities)
 
 // A step's token rows: row r is the prompt id spec[r] when spec[r] >= 0, else the last id slot ~spec[r] drew.  spec lies in
 // mapped pinned memory.
@@ -2657,7 +2660,8 @@ __global__ void k_gather_rows(const float * x, const StreamRow * rows, int E, fl
 // a greedy slot (argmax_row), the Sampler with the slot's divisors, key and the row's draw index for a sampled one
 // (sample_row, which then marks the id in the slot's penalty bitmap).  The id becomes the slot's last id, which the next
 // step's k_stream_tokens reads, and is stored into cell k of the step's publish ring in mapped pinned memory: the host
-// sets every cell to INT32_MIN before it enqueues the step, so each cell carries its own readiness.
+// sets every cell to INT32_MIN before it enqueues the step, so each cell carries its own readiness.  A row that asked for
+// log-probabilities is published by k_stream_logprobs instead, after its record.
 __global__ void __launch_bounds__(1024) k_stream_draw(const float * logits, int n, const StreamRow * rows,
                                                       const StreamSlot * slots, uint32_t * pen, int32_t * last, int32_t * ring) {
     __shared__ StreamRow s_row;
@@ -2672,7 +2676,7 @@ __global__ void __launch_bounds__(1024) k_stream_draw(const float * logits, int 
     if (threadIdx.x != 0) return;
     if (sl.sampled && id >= 0) bits[id >> 5] |= 1u << (id & 31);
     last[slot] = id;
-    *(volatile int32_t *)(ring + k) = id;
+    if (s_row.n_top < 0) *(volatile int32_t *)(ring + k) = id;
 }
 
 // The client's perplexity term (cli_api/common.py:129-139) for each of gridDim.x rows of [rows][n] logits, one block per
@@ -2681,11 +2685,13 @@ __global__ void __launch_bounds__(1024) k_stream_draw(const float * logits, int 
 // (warp_prefix_ordered within and across warps, as in k_sample_rows), so a row's value depends only on its logits and its
 // target.  Non-finite rows follow numpy: a NaN or +inf logit, or a row that is all -inf, gives NaN; a target whose e_t
 // underflows gives +inf.
-__global__ void __launch_bounds__(1024) k_nll_rows(const float * logits, int n, const int32_t * tgt, double * nll) {
+// The softmax normaliser of that term for one row x of n logits, for a whole block: m and S, valid in every thread.  Returns
+// false (block-uniform) when the row has no distribution.  k_nll_rows and k_logprob_rows both take m and S from here, so a
+// log-probability is exactly the negated NLL of the same row and id.
+__device__ __forceinline__ bool row_softmax(const float * x, int n, double * m_out, double * s_out) {
     __shared__ float smx[32];
-    __shared__ double swt[32];
-    const int k = blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5, nwarp = blockDim.x >> 5;
-    const float * x = logits + (size_t) k * n;
+    __shared__ double swt[32], s_S;
+    const int t = threadIdx.x, lane = t & 31, wid = t >> 5, nwarp = blockDim.x >> 5;
     const int C = (n + blockDim.x - 1) / blockDim.x, i0 = min(n, t * C), i1 = min(n, i0 + C);
     float mx = -INFINITY; bool bad = false;
     for (int i = i0; i < i1; i++) { const float v = x[i]; bad |= v != v || v == INFINITY; mx = fmaxf(mx, v); }
@@ -2694,10 +2700,7 @@ __global__ void __launch_bounds__(1024) k_nll_rows(const float * logits, int n, 
     const bool any_bad = __syncthreads_or(bad);
     mx = lane < nwarp ? smx[lane] : -INFINITY;          // every warp reduces the warp maxima: m is block-uniform
     for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    if (any_bad || mx == -INFINITY) {
-        if (t == 0) nll[k] = __longlong_as_double(0x7ff8000000000000ll);
-        return;
-    }
+    if (any_bad || mx == -INFINITY) return false;
     const double m = (double) mx;
     double tot = 0.0;
 #pragma unroll 1                                         // unrolled, the float64 exp spills at 32 registers (2 CTAs / SM)
@@ -2705,12 +2708,113 @@ __global__ void __launch_bounds__(1024) k_nll_rows(const float * logits, int n, 
     const double P = warp_prefix_ordered(tot);
     if (lane == 31) swt[wid] = __dadd_rn(P, tot);
     __syncthreads();
-    if (wid != 0) return;
-    const double v = lane < nwarp ? swt[lane] : 0.0, W = warp_prefix_ordered(v);
-    if (lane == 31) {
-        const double S = __dadd_rn(W, v), et = exp(__dsub_rn((double) x[tgt[k]], m));
-        nll[k] = -log(__ddiv_rn(et, S));
+    if (wid == 0) {
+        const double v = lane < nwarp ? swt[lane] : 0.0, W = warp_prefix_ordered(v);
+        if (lane == 31) s_S = __dadd_rn(W, v);
     }
+    __syncthreads();
+    *m_out = m; *s_out = s_S;
+    return true;
+}
+
+// log(e_t / S) for a logit x_t of a row with normaliser (m, S): -inf when e_t underflows.
+__device__ __forceinline__ double row_logp(float xt, double m, double S) {
+    return log(__ddiv_rn(exp(__dsub_rn((double) xt, m)), S));
+}
+
+__global__ void __launch_bounds__(1024) k_nll_rows(const float * logits, int n, const int32_t * tgt, double * nll) {
+    const int k = blockIdx.x;
+    const float * x = logits + (size_t) k * n;
+    double m, S;
+    const bool ok = row_softmax(x, n, &m, &S);
+    if (threadIdx.x == 0) nll[k] = ok ? -row_logp(x[tgt[k]], m, S) : __longlong_as_double(0x7ff8000000000000ll);
+}
+
+// ---- log-probabilities of drawn ids (b200_generate_lp, b200_stream_read_lp, b200_extra_logprobs): the raw distribution
+// softmax(x) of row_softmax, whatever the sampler's settings, and the n_top ids of largest x beside the drawn one.
+constexpr int kMaxTop = 20;
+
+// (a, ia) ranks before (b, ib): larger x first, equal x lower id first.  (Rows with a NaN never get here.)
+__device__ __forceinline__ bool ranks_before(float a, int ia, float b, int ib) { return a > b || (a == b && ia < ib); }
+
+// The best-ranked id of x[i0, i1) that ranks strictly after (pv, pi); (-inf, INT_MAX) when there is none.
+__device__ __forceinline__ void chunk_next(const float * x, int i0, int i1, float pv, int pi, float & bv, int & bi) {
+    bv = -INFINITY; bi = 0x7fffffff;
+    for (int i = i0; i < i1; i++) {
+        const float v = x[i];
+        if (ranks_before(pv, pi, v, i) && ranks_before(v, i, bv, bi)) { bv = v; bi = i; }
+    }
+}
+
+__device__ __forceinline__ void warp_best(float & v, int & i) {
+    for (int o = 16; o > 0; o >>= 1) {
+        const float w = __shfl_xor_sync(0xffffffffu, v, o); const int j = __shfl_xor_sync(0xffffffffu, i, o);
+        if (ranks_before(w, j, v, i)) { v = w; i = j; }
+    }
+}
+
+// lp = log p(id) and the n_top best-ranked ids with theirs, for one row of n logits, for a whole block.  A row without a
+// distribution (row_softmax) gives NaN and ids -1; so does lp of an id < 0.  The top-n: each thread keeps the best-ranked
+// id of its chunk not picked yet; a round reduces those over the block to the next pick, and the thread that owned it
+// rescans its own chunk.  So a round reads C logits, and the rank order is total, so the picks are exact on ties.
+__device__ __forceinline__ void logprob_row(const float * x, int n, int id, int n_top, double * lp, int32_t * top_ids,
+                                            double * top_lp) {
+    __shared__ float s_v[32]; __shared__ int s_i[32], s_pick[kMaxTop];
+    const int t = threadIdx.x, lane = t & 31, wid = t >> 5, nwarp = blockDim.x >> 5;
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    double m, S;
+    if (!row_softmax(x, n, &m, &S)) {
+        if (t == 0) *lp = nan;
+        if (t < n_top) { top_ids[t] = -1; top_lp[t] = nan; }
+        return;
+    }
+    if (t == 0) *lp = id >= 0 ? row_logp(x[id], m, S) : nan;
+    if (n_top == 0) return;
+    const int C = (n + blockDim.x - 1) / blockDim.x, i0 = min(n, t * C), i1 = min(n, i0 + C);
+    float bv; int bi;
+    chunk_next(x, i0, i1, INFINITY, -1, bv, bi);
+    for (int r = 0; r < n_top; r++) {
+        float v = bv; int i = bi;
+        warp_best(v, i);
+        if (lane == 0) { s_v[wid] = v; s_i[wid] = i; }
+        __syncthreads();
+        v = lane < nwarp ? s_v[lane] : -INFINITY; i = lane < nwarp ? s_i[lane] : 0x7fffffff;
+        warp_best(v, i);                                // every warp reduces the warp bests: the pick is block-uniform
+        if (t == 0) s_pick[r] = i;
+        if (i >= i0 && i < i1) chunk_next(x, i0, i1, v, i, bv, bi);
+        __syncthreads();
+    }
+    if (t < n_top) { const int j = s_pick[t]; top_ids[t] = j; top_lp[t] = row_logp(x[j], m, S); }
+}
+
+// logprob_row on each of gridDim.x rows of [rows][n] logits: row k's id is ids[k], its outputs lp[k] and
+// top_ids / top_lp [k][n_top].
+__global__ void __launch_bounds__(1024) k_logprob_rows(const float * logits, int n, const int32_t * ids, int n_top, double * lp,
+                                                       int32_t * top_ids, double * top_lp) {
+    const size_t k = blockIdx.x;
+    logprob_row(logits + k * n, n, ids[k], n_top, lp + k, top_ids + k * n_top, top_lp + k * n_top);
+}
+
+// A row's log-probability record in a stream's mapped logprob ring, one cell per publish-ring cell.
+struct LpRecord { double lp; int32_t top_ids[kMaxTop]; double top_lp[kMaxTop]; };
+static_assert(sizeof(LpRecord) == 8 + kMaxTop * 12, "LpRecord layout");
+
+// The records of a step's rows that asked for log-probabilities (the others return at once), launched after k_stream_draw:
+// row k's id is its slot's last id.  Every thread's stores into the mapped record reach the system before the id enters
+// publish cell k, so a host that sees the id also sees the record.
+__global__ void __launch_bounds__(1024) k_stream_logprobs(const float * logits, int n, const StreamRow * rows,
+                                                          const int32_t * last, int32_t * ring, LpRecord * rec) {
+    __shared__ StreamRow s_row;
+    const int k = blockIdx.x;
+    if (threadIdx.x == 0) s_row = rows[k];
+    __syncthreads();
+    if (s_row.n_top < 0) return;
+    const int id = last[s_row.slot];
+    LpRecord * r = rec + k;
+    logprob_row(logits + (size_t) k * n, n, id, s_row.n_top, &r->lp, r->top_ids, r->top_lp);
+    __threadfence_system();
+    __syncthreads();
+    if (threadIdx.x == 0) *(volatile int32_t *)(ring + k) = id;
 }
 
 // sentencepiece-style greedy bigram merging, as tensor_processor.cpp:1596-1714 specifies it:
@@ -3032,6 +3136,45 @@ static int sample_launch(b200_extra * e, const b200_sampling_t * sp, int rows, i
     return 0;
 }
 
+// Everything a call that returns log-probabilities checks about its outputs before it enqueues anything.
+static int lp_check(const b200_logprobs_t * lp, int n_vocab) {
+    if (!lp || !lp->lp) return fail(B200_EINVAL, "null log-probability outputs");
+    if (lp->n_top < 0 || lp->n_top > std::min(kMaxTop, n_vocab))
+        return fail(B200_EINVAL, "n_top %d outside [0, %d]", (int) lp->n_top, std::min(kMaxTop, n_vocab));
+    if (lp->n_top > 0 && (!lp->top_ids || !lp->top_lp)) return fail(B200_EINVAL, "n_top %d needs top_ids and top_lp", (int) lp->n_top);
+    return 0;
+}
+
+// The log-probability scratch for `rows` rows of n_top alternatives.
+static int lp_reserve(b200_extra * e, int rows, int n_top) {
+    int rc;
+    if ((rc = extra_regrow(e, e->d_lp, e->cap_lp, 1, rows)) || (rc = extra_regrow(e, e->d_topi, e->cap_topi, 1, rows * n_top)) ||
+        (rc = extra_regrow(e, e->d_topl, e->cap_topl, 1, rows * n_top)))
+        return rc;
+    return 0;
+}
+
+// k_logprob_rows on the first `rows` rows of d_logits, whose ids are ids[0, rows): scratch rows r0 .. r0 + rows - 1.
+static int lp_launch(b200_extra * e, int rows, const int32_t * ids, int n_top, size_t r0) {
+    k_logprob_rows<<<rows, 1024, 0, e->ctx.stream>>>(e->d_logits, e->n_vocab, ids, n_top, e->d_lp + r0, e->d_topi + r0 * n_top,
+                                                     e->d_topl + r0 * n_top);
+    B200_CUDA(cudaGetLastError());
+    e->ctx.launches++;
+    return 0;
+}
+
+// Scratch rows [0, rows) to the caller's arrays, in stream order (the caller synchronises).
+static int lp_copy_back(b200_extra * e, const b200_logprobs_t * lp, int rows) {
+    cudaStream_t st = e->ctx.stream;
+    const size_t n = (size_t) rows * lp->n_top;
+    B200_CUDA(cudaMemcpyAsync(lp->lp, e->d_lp, (size_t) rows * 8, cudaMemcpyDeviceToHost, st));
+    if (n) {
+        B200_CUDA(cudaMemcpyAsync(lp->top_ids, e->d_topi, n * 4, cudaMemcpyDeviceToHost, st));
+        B200_CUDA(cudaMemcpyAsync(lp->top_lp, e->d_topl, n * 8, cudaMemcpyDeviceToHost, st));
+    }
+    return 0;
+}
+
 // After the call's synchronise: B200_EINVAL naming the first row that had no distribution.
 static int sample_finish(b200_extra * e, int rows, const int * sessions) {
     int bad = INT_MAX;
@@ -3044,16 +3187,18 @@ static int sample_finish(b200_extra * e, int rows, const int * sessions) {
     return fail(B200_EINVAL, "row %d: the logits are all -inf or overflow float64 once scaled, so they have no distribution", k);
 }
 
-// The loop of b200_generate_greedy (sp == NULL: argmax, k_argmax_rows) and b200_generate_sample (k_sample_rows).
+// The loop of b200_generate_greedy (sp == NULL: argmax, k_argmax_rows) and b200_generate_sample (k_sample_rows), and of
+// b200_generate_lp (lp != NULL: k_logprob_rows after each step's draw).
 static int generate_locked(b200_slice * const * slices, int n_slices, b200_extra * e, const int * sessions,
                            const int * counts, int n_seq, const int32_t * tokens, int n_steps, const b200_sampling_t * sp,
-                           int32_t * ids) {
+                           int32_t * ids, const b200_logprobs_t * lp) {
     b200_slice * x = &e->ctx;
     B200_CUDA(cudaSetDevice(x->device));
     int total = 0;
     for (int k = 0; k < n_seq; k++) total += counts[k];
     int rc;
     if ((rc = extra_reserve(e, total)) || (rc = extra_reserve_ids(e, n_steps * n_seq))) return rc;
+    if (lp && (rc = lp_reserve(e, n_steps * n_seq, lp->n_top))) return rc;
     for (int i = 0; i < n_slices; i++) B200_CUDA(cudaStreamSynchronize(slices[i]->stream));
     if (sp && (rc = sample_start(e, sp, n_seq))) return rc;
     B200_CUDA(cudaMemcpyAsync(e->d_tok, tokens, (size_t) total * 4, cudaMemcpyHostToDevice, x->stream));
@@ -3084,16 +3229,19 @@ static int generate_locked(b200_slice * const * slices, int n_slices, b200_extra
                 cur = e->d_x;
             }
             if ((rc = extra_lmhead(e, cur, n_seq))) return rc;
+            int32_t * step_ids = e->d_ids + (size_t) step * n_seq;
             if (sp) {
-                if ((rc = sample_launch(e, sp, n_seq, step, e->d_ids + (size_t) step * n_seq))) return rc;
-                continue;
+                if ((rc = sample_launch(e, sp, n_seq, step, step_ids))) return rc;
+            } else {
+                k_argmax_rows<<<n_seq, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, e->d_tok, step_ids);
+                B200_CUDA(cudaGetLastError());
+                x->launches++;
             }
-            k_argmax_rows<<<n_seq, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, e->d_tok, e->d_ids + (size_t) step * n_seq);
-            B200_CUDA(cudaGetLastError());
-            x->launches++;
+            if (lp && (rc = lp_launch(e, n_seq, step_ids, lp->n_top, (size_t) step * n_seq))) return rc;
         }
     }
     B200_CUDA(cudaMemcpyAsync(ids, e->d_ids, (size_t) n_steps * n_seq * 4, cudaMemcpyDeviceToHost, x->stream));
+    if (lp && (rc = lp_copy_back(e, lp, n_steps * n_seq))) return rc;
     B200_CUDA(cudaStreamSynchronize(x->stream));
     return sp ? sample_finish(e, n_seq, sessions) : 0;
 }
@@ -3124,18 +3272,22 @@ static int lock_handles(b200_slice_t * const * slices, int n_slices, b200_extra_
     return 0;
 }
 
-// Both generation entries: the checks, every handle's mutex, then the loop (greedy when not sampled).
-static int generate(bool sampled, b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
-                    const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps,
-                    const b200_sampling_t * sp, int32_t * ids) {
+// Every generation entry: the checks, every handle's mutex, then the loop (greedy when not sampled; log-probabilities when
+// want_lp).
+static int generate(const char * what, bool sampled, b200_slice_t * const * slices, int n_slices, b200_extra_t * e,
+                    const int * sessions, const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps,
+                    const b200_sampling_t * sp, int32_t * ids, bool want_lp, const b200_logprobs_t * lp) {
     if (!slices || n_slices < 1 || !e || !sessions || !prompt_counts || n_seq < 1 || !prompt_tokens || !ids)
-        return fail(B200_EINVAL, "%s: null argument or empty list", sampled ? "b200_generate_sample" : "b200_generate_greedy");
+        return fail(B200_EINVAL, "%s: null argument or empty list", what);
     std::vector<std::unique_lock<std::mutex>> locks;
     if (int rc = lock_handles(slices, n_slices, e, locks)) return rc;
     if (int rc = generate_check(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps)) return rc;
     if (sampled)
         if (int rc = sample_check(sp, n_seq, e->n_vocab)) return rc;
-    return generate_locked(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps, sp, ids);
+    if (want_lp)
+        if (int rc = lp_check(lp, e->n_vocab)) return rc;
+    return generate_locked(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps, sp, ids,
+                           want_lp ? lp : nullptr);
 }
 
 // Rows the scoring loop's lm_head and k_nll_rows take at a time: its logits scratch is kScoreRows x n_vocab floats
@@ -3307,6 +3459,21 @@ __global__ void __launch_bounds__(1024) k_spec_check_pick(const float * logits, 
     if (threadIdx.x == 0) st->g[j] = id;
 }
 
+// The log-probabilities of the ids k_spec_accept is about to emit (one block per checking row, launched between
+// k_spec_check_pick and it): row j < c, with c as k_spec_accept counts it, writes output row m + j for id g_j; the other
+// rows return at once.  Checking rows are decode rows, bit-identical to single-token steps, so these equal the plain
+// loop's values.
+__global__ void __launch_bounds__(1024) k_spec_logprobs(const float * logits, int n, const SpecState * st, int k, int n_steps,
+                                                        int n_top, double * lp, int32_t * top_ids, double * top_lp) {
+    const int j = blockIdx.x, m = st->m;
+    if (m >= n_steps) return;
+    int a = 0;
+    while (a < k && st->ctok[a + 1] == st->g[a]) a++;
+    if (j >= min(a + 1, n_steps - m)) return;
+    const size_t r = (size_t) m + j;
+    logprob_row(logits + (size_t) j * n, n, st->g[j], n_top, lp + r, top_ids + r * n_top, top_lp + r * n_top);
+}
+
 // Keeps g_0 .. g_n (n the largest j <= k with d_i == g_(i-1) for every i <= j), cut at the budget of n_steps ids, and moves
 // every target slice to p + (ids emitted) and every draft slice one row before it.  The host never enqueues an iteration
 // the ones in flight could leave without budget; should one start with the budget spent, it emits nothing and puts the
@@ -3398,7 +3565,7 @@ static int spec_check(b200_slice * const * t, int nt, const b200_extra * e, int 
 
 static int spec_locked(b200_slice * const * t, int nt, b200_extra * e, int session, b200_slice * const * d, int nd,
                        b200_extra * de, int dsession, const int32_t * prompt, int n_prompt, int n_steps, int k,
-                       const b200_sampling_t * sp, int32_t * ids, b200_spec_stats_t * stats) {
+                       const b200_sampling_t * sp, int32_t * ids, b200_spec_stats_t * stats, const b200_logprobs_t * lp) {
     b200_slice * x = &e->ctx;
     B200_CUDA(cudaSetDevice(x->device));
     const int V = e->n_vocab, nw = (V + 31) / 32, p0 = t[0]->past[session] + n_prompt, p_final = p0 + n_steps - 1;
@@ -3406,6 +3573,7 @@ static int spec_locked(b200_slice * const * t, int nt, b200_extra * e, int sessi
     if ((rc = extra_reserve(e, std::max(n_prompt, k + 1))) || (rc = extra_reserve_ids(e, n_steps)) ||
         (rc = extra_reserve(de, std::max(n_prompt, 2))))
         return rc;
+    if (lp && (rc = lp_reserve(e, n_steps, lp->n_top))) return rc;
     for (int i = 0; i < nt; i++) B200_CUDA(cudaStreamSynchronize(t[i]->stream));
     for (int i = 0; i < nd; i++) B200_CUDA(cudaStreamSynchronize(d[i]->stream));
     B200_CUDA(cudaStreamSynchronize(de->ctx.stream));
@@ -3457,6 +3625,7 @@ static int spec_locked(b200_slice * const * t, int nt, b200_extra * e, int sessi
             B200_CUDA(cudaGetLastError());
             x->launches++;
         }
+        if (lp && (rc = lp_launch(e, 1, e->d_ids, lp->n_top, 0))) return rc;
         cur = de->d_x;
         if ((rc = embed_launch(de, de->d_tok, n_prompt, de->d_x))) return rc;
         for (int i = 0; i < nd; i++) {
@@ -3509,6 +3678,11 @@ static int spec_locked(b200_slice * const * t, int nt, b200_extra * e, int sessi
                 return rc;
             k_spec_check_pick<<<k + 1, 1024, 0, x->stream>>>(e->d_logits, V, st, ss, base, rows, nw);
             B200_CUDA(cudaGetLastError());
+            if (lp) {
+                k_spec_logprobs<<<k + 1, 1024, 0, x->stream>>>(e->d_logits, V, st, k, n_steps, lp->n_top, e->d_lp, e->d_topi, e->d_topl);
+                B200_CUDA(cudaGetLastError());
+                x->launches++;
+            }
             k_spec_accept<<<1, 32, 0, x->stream>>>(st, k, n_steps, e->d_ids, base, sp ? e->d_bad : nullptr, npast, nt,
                                                    npast + nt, nd, d_prog);
             B200_CUDA(cudaGetLastError());
@@ -3518,6 +3692,7 @@ static int spec_locked(b200_slice * const * t, int nt, b200_extra * e, int sessi
     }
     SpecState h{};
     B200_CUDA(cudaMemcpyAsync(ids, e->d_ids, (size_t) n_steps * 4, cudaMemcpyDeviceToHost, x->stream));
+    if (lp && (rc = lp_copy_back(e, lp, n_steps))) return rc;
     B200_CUDA(cudaMemcpyAsync(&h, st, sizeof(SpecState), cudaMemcpyDeviceToHost, x->stream));
     for (int * q : h_npast) B200_CUDA(cudaMemcpyAsync(q, &p_final, 4, cudaMemcpyHostToDevice, x->stream));
     B200_CUDA(cudaStreamSynchronize(x->stream));
@@ -3530,7 +3705,8 @@ static int spec_locked(b200_slice * const * t, int nt, b200_extra * e, int sessi
 // b200_generate_speculative: the checks, every handle's mutex of both chains in address order, then the loop.
 static int speculative(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int session, b200_slice_t * const * draft,
                        int n_draft_slices, b200_extra_t * draft_e, int draft_session, const int32_t * prompt, int n_prompt,
-                       int n_steps, int n_draft, const b200_sampling_t * sp, int32_t * ids, b200_spec_stats_t * stats) {
+                       int n_steps, int n_draft, const b200_sampling_t * sp, int32_t * ids, b200_spec_stats_t * stats,
+                       bool want_lp, const b200_logprobs_t * lp) {
     if (!slices || n_slices < 1 || !e || !draft || n_draft_slices < 1 || !draft_e || !prompt || n_prompt < 1 || !ids)
         return fail(B200_EINVAL, "b200_generate_speculative: null argument or empty list");
     std::vector<std::mutex *> mus{&e->mu, &draft_e->mu};
@@ -3552,8 +3728,10 @@ static int speculative(b200_slice_t * const * slices, int n_slices, b200_extra_t
     if (int rc = spec_check(slices, n_slices, e, session, draft, n_draft_slices, draft_e, draft_session, prompt, n_prompt,
                             n_steps, n_draft, sp))
         return rc;
+    if (want_lp)
+        if (int rc = lp_check(lp, e->n_vocab)) return rc;
     return spec_locked(slices, n_slices, e, session, draft, n_draft_slices, draft_e, draft_session, prompt, n_prompt, n_steps,
-                       n_draft, sp, ids, stats);
+                       n_draft, sp, ids, stats, want_lp ? lp : nullptr);
 }
 
 }  // namespace b200
@@ -3562,15 +3740,22 @@ extern "C" {
 
 int b200_generate_greedy(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
                          const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps, int32_t * ids) {
-    return generate(false, slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps,
-                    nullptr, ids);
+    return generate("b200_generate_greedy", false, slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps,
+                    nullptr, ids, false, nullptr);
 }
 
 int b200_generate_sample(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
                          const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps,
                          const b200_sampling_t * sp, int32_t * ids) {
-    return generate(true, slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps,
-                    sp, ids);
+    return generate("b200_generate_sample", true, slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps,
+                    sp, ids, false, nullptr);
+}
+
+int b200_generate_lp(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
+                     const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps,
+                     const b200_sampling_t * sp, int32_t * ids, const b200_logprobs_t * lp) {
+    return generate("b200_generate_lp", sp != nullptr, slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens,
+                    n_steps, sp, ids, true, lp);
 }
 
 int b200_generate_speculative(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int session,
@@ -3578,7 +3763,15 @@ int b200_generate_speculative(b200_slice_t * const * slices, int n_slices, b200_
                               const int32_t * prompt, int n_prompt, int n_steps, int n_draft, const b200_sampling_t * sp,
                               int32_t * ids, b200_spec_stats_t * stats) {
     return speculative(slices, n_slices, e, session, draft, n_draft_slices, draft_e, draft_session, prompt, n_prompt, n_steps,
-                       n_draft, sp, ids, stats);
+                       n_draft, sp, ids, stats, false, nullptr);
+}
+
+int b200_generate_speculative_lp(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int session,
+                                 b200_slice_t * const * draft, int n_draft_slices, b200_extra_t * draft_e, int draft_session,
+                                 const int32_t * prompt, int n_prompt, int n_steps, int n_draft, const b200_sampling_t * sp,
+                                 int32_t * ids, b200_spec_stats_t * stats, const b200_logprobs_t * lp) {
+    return speculative(slices, n_slices, e, session, draft, n_draft_slices, draft_e, draft_session, prompt, n_prompt, n_steps,
+                       n_draft, sp, ids, stats, true, lp);
 }
 
 int b200_extra_sample(b200_extra_t * e, const float * logits, int n_rows, const b200_sampling_t * sp, int32_t * ids) {
@@ -3630,6 +3823,24 @@ int b200_extra_nll(b200_extra_t * e, const float * logits, int n_rows, const int
     return 0;
 }
 
+int b200_extra_logprobs(b200_extra_t * e, const float * logits, int n_rows, const int32_t * ids, int n_top, double * lp,
+                        int32_t * top_ids, double * top_lp) {
+    if (!e || !logits || n_rows < 1 || !ids) return fail(B200_EINVAL, "b200_extra_logprobs: null argument or no rows");
+    std::lock_guard<std::mutex> lk(e->mu); B200_UNOWNED(&e->ctx);
+    const b200_logprobs_t out{n_top, lp, top_ids, top_lp};
+    if (int rc = lp_check(&out, e->n_vocab)) return rc;
+    if (int rc = check_tokens(ids, n_rows, e->n_vocab, "id")) return rc;
+    b200_slice * s = &e->ctx;
+    B200_CUDA(cudaSetDevice(s->device));
+    int rc;
+    if ((rc = extra_reserve(e, n_rows)) || (rc = extra_reserve_ids(e, n_rows)) || (rc = lp_reserve(e, n_rows, n_top))) return rc;
+    B200_CUDA(cudaMemcpyAsync(e->d_logits, logits, (size_t) n_rows * e->n_vocab * 4, cudaMemcpyHostToDevice, s->stream));
+    B200_CUDA(cudaMemcpyAsync(e->d_ids, ids, (size_t) n_rows * 4, cudaMemcpyHostToDevice, s->stream));
+    if ((rc = lp_launch(e, n_rows, e->d_ids, n_top, 0)) || (rc = lp_copy_back(e, &out, n_rows))) return rc;
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    return 0;
+}
+
 int b200_extra_tokenize(b200_extra_t * e, const char * prompt, int32_t * out, int cap) {
     if (!e || !prompt) return -B200_EINVAL;
     const std::string text(prompt);
@@ -3662,12 +3873,14 @@ struct b200_stream {
     b200::StreamSlot * d_slots = nullptr; uint32_t * d_pen = nullptr; int32_t * d_last = nullptr;
     // mapped pinned, one region per step in flight (lookahead + 1): token specs [max_rows], rows [rows_cap], ids [rows_cap]
     int32_t * h_spec = nullptr; b200::StreamRow * h_rows = nullptr; int32_t * h_ring = nullptr;
+    b200::LpRecord * h_lp = nullptr;      // mapped pinned, [regions][rows_cap]: the logprob ring beside h_ring
     struct Sess {
         int state = 0;                    // 0 not in the stream, 1 queued, 2 admitted (its prompt is enqueued)
         unsigned gen = 0;                 // bumped when the session leaves: rows of steps enqueued before are dropped
         std::vector<int32_t> prompt, stops;
         std::vector<int> old;             // n_past on each slice when it was added
         int max_tokens = 0, enq = 0, delivered = 0;   // ids enqueued / returned by b200_stream_read
+        int n_top = -1;                   // log-probabilities with n_top alternatives; -1: none
         long long first_draw = 0;
     };
     std::vector<Sess> sess;
@@ -3723,11 +3936,13 @@ static int stream_step(b200_stream * st, bool * did) {
     StreamRow * rows = st->h_rows + (size_t) q * st->rows_cap;
     volatile int32_t * ring = st->h_ring + (size_t) q * st->rows_cap;
     b200_stream::Step step{q, {}, 0};
+    bool any_lp = false;
     for (int j = 0, r = 0; j < n; j++) {
         b200_stream::Sess & z = st->sess[ses[j]];
         if (j < n_decode) spec[r++] = ~ses[j];
         else for (int32_t t : z.prompt) spec[r++] = t;
-        rows[j] = {z.first_draw + z.enq, ses[j], r - 1};
+        rows[j] = {z.first_draw + z.enq, ses[j], r - 1, z.n_top};
+        any_lp |= z.n_top >= 0;
         ring[j] = INT32_MIN;
         step.rows.emplace_back(ses[j], z.gen);
     }
@@ -3757,6 +3972,12 @@ static int stream_step(b200_stream * st, bool * did) {
     k_stream_draw<<<n, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, rows, st->d_slots, st->d_pen, st->d_last, st->h_ring + (size_t) q * st->rows_cap);
     B200_CUDA(cudaGetLastError());
     x->launches++;
+    if (any_lp) {                                   // publishes the rows that asked, after their records
+        k_stream_logprobs<<<n, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, rows, st->d_last, st->h_ring + (size_t) q * st->rows_cap,
+                                                     st->h_lp + (size_t) q * st->rows_cap);
+        B200_CUDA(cudaGetLastError());
+        x->launches++;
+    }
     for (int j = 0; j < n; j++) {
         b200_stream::Sess & z = st->sess[ses[j]];
         z.state = 2; z.enq++;
@@ -3772,7 +3993,7 @@ static void stream_free(b200_stream * st) {
     for (b200_slice * s : st->slices) s->owner = nullptr;
     if (st->e) st->e->ctx.owner = nullptr;
     cudaFree(st->d_slots); cudaFree(st->d_pen); cudaFree(st->d_last);
-    cudaFreeHost(st->h_spec); cudaFreeHost(st->h_rows); cudaFreeHost(st->h_ring);
+    cudaFreeHost(st->h_spec); cudaFreeHost(st->h_rows); cudaFreeHost(st->h_ring); cudaFreeHost(st->h_lp);
     delete st;
 }
 
@@ -3781,6 +4002,62 @@ static int stream_lock(b200_stream * st, std::vector<std::unique_lock<std::mutex
     if (!st) return fail(B200_EINVAL, "null stream");
     if (int rc = lock_handles(st->slices.data(), (int) st->slices.size(), st->e, locks, st)) return rc;
     B200_CUDA(cudaSetDevice(st->e->ctx.device));
+    return 0;
+}
+
+// b200_stream_read, and with lp != NULL b200_stream_read_lp: record got's log-probabilities from the ring cell beside the
+// id's, or NaN and -1 for a session that asked for none.
+static int stream_read(b200_stream * st, int32_t * sessions, int32_t * ids, double * lp, int32_t * top_ids, double * top_lp,
+                       int cap, int * n_out) {
+    *n_out = 0;
+    std::vector<std::unique_lock<std::mutex>> locks;
+    if (int rc = stream_lock(st, locks)) return rc;
+    int got = 0;
+    long long spins = 0;
+    for (;;) {
+        while ((int) st->pending.size() <= st->lookahead) {
+            bool did = false;
+            if (int rc = stream_step(st, &did)) return rc;
+            if (!did) break;
+        }
+        if (got == cap || st->pending.empty()) break;
+        b200_stream::Step & f = st->pending.front();
+        const volatile int32_t * ring = st->h_ring + (size_t) f.region * st->rows_cap;
+        while (f.next < f.rows.size() && got < cap) {
+            const int32_t id = ring[f.next];
+            if (id == INT32_MIN) break;
+            const int k = f.rows[f.next].first;
+            const unsigned gen = f.rows[f.next].second;
+            f.next++;
+            b200_stream::Sess & z = st->sess[k];
+            if (z.state != 2 || z.gen != gen) continue;      // a step the device ran past the session's end
+            if (lp) {
+                std::atomic_thread_fence(std::memory_order_acquire);    // the record was complete before the id was stored
+                const LpRecord & r = st->h_lp[(size_t) f.region * st->rows_cap + f.next - 1];
+                const int nt = z.n_top;
+                lp[got] = nt >= 0 ? r.lp : std::nan("");
+                for (int j = 0; j < kMaxTop; j++) {
+                    top_ids[(size_t) got * kMaxTop + j] = j < nt ? r.top_ids[j] : -1;
+                    top_lp[(size_t) got * kMaxTop + j] = j < nt ? r.top_lp[j] : std::nan("");
+                }
+            }
+            sessions[got] = k; ids[got] = id; got++;
+            z.delivered++;
+            if (id < 0 || z.delivered == z.max_tokens || std::find(z.stops.begin(), z.stops.end(), id) != z.stops.end())
+                if (int rc = stream_finish(st, k)) return rc;
+        }
+        if (f.next == f.rows.size()) { st->pending.pop_front(); spins = 0; continue; }
+        if (got > 0) break;
+        // nothing published yet: poll; now and then make sure the device is still running the steps
+        if (++spins % 4096 == 0) {
+            const cudaError_t q = cudaStreamQuery(st->e->ctx.stream);
+            if (q != cudaSuccess && q != cudaErrorNotReady) return fail(B200_ECUDA, "generation stream: %s", cudaGetErrorString(q));
+            if (q == cudaSuccess && ring[f.next] == INT32_MIN)
+                return fail(B200_ECUDA, "generation stream: the device finished a step without publishing its id");
+        }
+        std::this_thread::yield();
+    }
+    *n_out = got;
     return 0;
 }
 
@@ -3817,9 +4094,10 @@ int b200_stream_open(b200_slice_t * const * slices, int n_slices, b200_extra_t *
         (ce = cudaMalloc(&st->d_last, (size_t) 4 * n_sess)) != cudaSuccess ||
         (ce = cudaHostAlloc(&st->h_spec, 4 * regions * max_rows, cudaHostAllocMapped)) != cudaSuccess ||
         (ce = cudaHostAlloc(&st->h_rows, sizeof(StreamRow) * regions * st->rows_cap, cudaHostAllocMapped)) != cudaSuccess ||
-        (ce = cudaHostAlloc(&st->h_ring, 4 * regions * st->rows_cap, cudaHostAllocMapped)) != cudaSuccess) {
+        (ce = cudaHostAlloc(&st->h_ring, 4 * regions * st->rows_cap, cudaHostAllocMapped)) != cudaSuccess ||
+        (ce = cudaHostAlloc(&st->h_lp, sizeof(LpRecord) * regions * st->rows_cap, cudaHostAllocMapped)) != cudaSuccess) {
         cudaFree(st->d_slots); cudaFree(st->d_pen); cudaFree(st->d_last);
-        cudaFreeHost(st->h_spec); cudaFreeHost(st->h_rows); cudaFreeHost(st->h_ring);
+        cudaFreeHost(st->h_spec); cudaFreeHost(st->h_rows); cudaFreeHost(st->h_ring); cudaFreeHost(st->h_lp);
         return fail_free(fail(B200_ECUDA, "stream buffers: %s", cudaGetErrorString(ce)));
     }
     if (int rc = extra_reserve(e, max_rows)) { stream_free(st); return rc; }
@@ -3834,6 +4112,11 @@ int b200_stream_open(b200_slice_t * const * slices, int n_slices, b200_extra_t *
 
 int b200_stream_add(b200_stream_t * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
                     const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop) {
+    return b200_stream_add_lp(st, session, prompt, n_prompt, max_tokens, sp, stop_ids, n_stop, -1);
+}
+
+int b200_stream_add_lp(b200_stream_t * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
+                       const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop, int n_top) {
     std::vector<std::unique_lock<std::mutex>> locks;
     if (int rc = stream_lock(st, locks)) return rc;
     if (session < 0 || session >= st->n_sess) return fail(B200_EINVAL, "session %d outside [0, %d)", session, st->n_sess);
@@ -3847,6 +4130,8 @@ int b200_stream_add(b200_stream_t * st, int session, const int32_t * prompt, int
     if (int rc = check_tokens(stop_ids, n_stop, V, "stop id")) return rc;
     if (sp)
         if (int rc = sample_check(sp, 1, V)) return rc;
+    if (n_top < -1 || n_top > std::min(kMaxTop, V))
+        return fail(B200_EINVAL, "session %d: n_top %d outside [-1, %d]", session, n_top, std::min(kMaxTop, V));
     for (size_t i = 0; i < st->slices.size(); i++) {
         const b200_slice * s = st->slices[i];
         if ((long long) s->past[session] + n_prompt + max_tokens - 1 > s->n_ctx)
@@ -3871,7 +4156,7 @@ int b200_stream_add(b200_stream_t * st, int session, const int32_t * prompt, int
     z.stops.assign(stop_ids, stop_ids + n_stop);
     z.old.clear();
     for (const b200_slice * s : st->slices) z.old.push_back(s->past[session]);
-    z.max_tokens = max_tokens; z.enq = 0; z.delivered = 0;
+    z.max_tokens = max_tokens; z.enq = 0; z.delivered = 0; z.n_top = n_top;
     z.first_draw = sp ? sp->first_draw : 0;
     z.state = 1;
     st->queue.push_back(session);
@@ -3880,46 +4165,14 @@ int b200_stream_add(b200_stream_t * st, int session, const int32_t * prompt, int
 
 int b200_stream_read(b200_stream_t * st, int32_t * sessions, int32_t * ids, int cap, int * n_out) {
     if (!sessions || !ids || !n_out || cap < 1) return fail(B200_EINVAL, "b200_stream_read: null argument or cap < 1");
-    *n_out = 0;
-    std::vector<std::unique_lock<std::mutex>> locks;
-    if (int rc = stream_lock(st, locks)) return rc;
-    int got = 0;
-    long long spins = 0;
-    for (;;) {
-        while ((int) st->pending.size() <= st->lookahead) {
-            bool did = false;
-            if (int rc = stream_step(st, &did)) return rc;
-            if (!did) break;
-        }
-        if (got == cap || st->pending.empty()) break;
-        b200_stream::Step & f = st->pending.front();
-        const volatile int32_t * ring = st->h_ring + (size_t) f.region * st->rows_cap;
-        while (f.next < f.rows.size() && got < cap) {
-            const int32_t id = ring[f.next];
-            if (id == INT32_MIN) break;
-            const int k = f.rows[f.next].first;
-            const unsigned gen = f.rows[f.next].second;
-            f.next++;
-            b200_stream::Sess & z = st->sess[k];
-            if (z.state != 2 || z.gen != gen) continue;      // a step the device ran past the session's end
-            sessions[got] = k; ids[got] = id; got++;
-            z.delivered++;
-            if (id < 0 || z.delivered == z.max_tokens || std::find(z.stops.begin(), z.stops.end(), id) != z.stops.end())
-                if (int rc = stream_finish(st, k)) return rc;
-        }
-        if (f.next == f.rows.size()) { st->pending.pop_front(); spins = 0; continue; }
-        if (got > 0) break;
-        // nothing published yet: poll; now and then make sure the device is still running the steps
-        if (++spins % 4096 == 0) {
-            const cudaError_t q = cudaStreamQuery(st->e->ctx.stream);
-            if (q != cudaSuccess && q != cudaErrorNotReady) return fail(B200_ECUDA, "generation stream: %s", cudaGetErrorString(q));
-            if (q == cudaSuccess && ring[f.next] == INT32_MIN)
-                return fail(B200_ECUDA, "generation stream: the device finished a step without publishing its id");
-        }
-        std::this_thread::yield();
-    }
-    *n_out = got;
-    return 0;
+    return stream_read(st, sessions, ids, nullptr, nullptr, nullptr, cap, n_out);
+}
+
+int b200_stream_read_lp(b200_stream_t * st, int32_t * sessions, int32_t * ids, double * lp, int32_t * top_ids, double * top_lp,
+                        int cap, int * n_out) {
+    if (!sessions || !ids || !lp || !top_ids || !top_lp || !n_out || cap < 1)
+        return fail(B200_EINVAL, "b200_stream_read_lp: null argument or cap < 1");
+    return stream_read(st, sessions, ids, lp, top_ids, top_lp, cap, n_out);
 }
 
 int b200_stream_cancel(b200_stream_t * st, int session) {

@@ -369,6 +369,47 @@ int b200_score(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, co
  * nll[k] as b200_score computes it for row k and target targets[k]; a target outside [0, n_vocab) is B200_EINVAL. */
 int b200_extra_nll(b200_extra_t * e, const float * logits, int n_rows, const int32_t * targets, double * nll);
 
+/* ---- log-probabilities of generated ids ("logprobs") ------------------------------------------------------------------
+ * For the logits row x (n_vocab floats) that a step drew id t from:
+ *   - the distribution is the model's raw one, softmax(x) in float64: before temperature, repeat penalty and top-k/top-p,
+ *     so the same whatever the sampler's settings (the sampling distribution's probabilities are not reported);
+ *   - lp = log(e_t / S) with m = max x, e_i = exp((double) x_i - m) and S summed in b200_score's fixed order; the device
+ *     takes m and S from the code k_nll_rows uses, so lp == -nll bit for bit, nll being b200_extra_nll of the same row and
+ *     target.  An e_t that underflows gives -inf;
+ *   - top-n: the n_top ids with the largest x, equal x lower id first (so in greedy mode top_ids[0] == t), each with its
+ *     own log(e_i / S) from the same m and S.  0 <= n_top <= min(20, n_vocab);
+ *   - a row with no distribution (a NaN or +inf logit, or all -inf) gives lp and top_lp NaN and top_ids -1; lp of an id -1
+ *     (a sampled row whose scaled logits overflow) is NaN.  The id is what the call without log-probabilities gives.
+ * Log-probabilities never feed back into the draw, so asking for them changes no id, and a call or stream session that asks
+ * for none launches nothing extra.  Each of these calls is all-or-nothing on its arguments: B200_EINVAL, with no position
+ * moved, for n_top out of range, a null lp, or a null top_ids or top_lp when n_top > 0. */
+typedef struct b200_logprobs {
+    int32_t  n_top;      /* 0..min(20, n_vocab): alternatives per id (0: only the drawn id's lp) */
+    double * lp;         /* [n_steps][n_seq], the ids' layout */
+    int32_t * top_ids;   /* [n_steps][n_seq][n_top]; may be NULL when n_top == 0 */
+    double * top_lp;     /* same shape */
+} b200_logprobs_t;
+/* b200_generate_sample (sp NULL: b200_generate_greedy) with the log-probability of every id it writes.  The ids are those
+ * calls' ids; lp row (step, k) belongs to ids[step][k].  One kernel per step after the draw, outputs on the device, copied
+ * back once at the end with the ids.  A session's values are bit-identical alone, in a batch or split across calls.  Errors
+ * as those calls, plus the refusals above. */
+int b200_generate_lp(b200_slice_t * const * slices, int n_slices, b200_extra_t * e,
+                     const int * sessions, const int * prompt_counts, int n_seq,
+                     const int32_t * prompt_tokens, int n_steps, const b200_sampling_t * sp /* NULL: greedy */,
+                     int32_t * ids, const b200_logprobs_t * lp);
+/* b200_generate_speculative with the log-probability of every emitted id ([n_steps], n_seq = 1).  Only the emitted rows of a
+ * checking pass are computed; checking rows are decode rows, bit-identical to single-token steps, so the values equal
+ * b200_generate_lp's for this session alone bit for bit, whatever the draft. */
+int b200_generate_speculative_lp(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int session,
+                                 b200_slice_t * const * draft, int n_draft_slices, b200_extra_t * draft_e, int draft_session,
+                                 const int32_t * prompt, int n_prompt, int n_steps, int n_draft,
+                                 const b200_sampling_t * sp /* NULL: greedy */, int32_t * ids, b200_spec_stats_t * stats,
+                                 const b200_logprobs_t * lp);
+/* k_logprob_rows on host logits [n_rows][n_vocab] for ids[k] (in [0, n_vocab), else B200_EINVAL): the kernel's test door.
+ * lp [n_rows], top_ids / top_lp [n_rows][n_top]. */
+int b200_extra_logprobs(b200_extra_t * e, const float * logits, int n_rows, const int32_t * ids, int n_top,
+                        double * lp, int32_t * top_ids, double * top_lp);
+
 /* ---- generation streams: sessions join and leave between steps, ids reach the caller as they are drawn ----------------
  * A stream runs the generation loop of b200_generate_greedy / b200_generate_sample over a chain of slices on one GPU (the
  * same handle checks: contiguous layers, one device, no pipeline, the extra layers' n_embd), but open-ended:
@@ -405,6 +446,18 @@ int b200_stream_open(b200_slice_t * const * slices, int n_slices, b200_extra_t *
 int b200_stream_add(b200_stream_t * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
                     const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop);
 int b200_stream_read(b200_stream_t * st, int32_t * sessions, int32_t * ids, int cap, int * n_out);
+/* b200_stream_add with log-probabilities for the session's ids: n_top in [0, min(20, n_vocab)] alternatives each, -1 for
+ * none (b200_stream_add).  Each session's (ids, lp, top) equal b200_generate_lp of it alone bit for bit.  A row that asks is
+ * published after its record: the draw leaves its publish cell to a second kernel that writes the record into a mapped
+ * logprob ring (sized once at b200_stream_open: regions x rows x (8 + 20 x 12) bytes), fences at system scope, and only then
+ * stores the id.  Rows that do not ask are published by the draw as before. */
+int b200_stream_add_lp(b200_stream_t * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
+                       const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop, int n_top);
+/* b200_stream_read with each id's record: lp [cap], top_ids / top_lp [cap][20], entry j < the session's n_top filled, the
+ * rest -1 / NaN; a session added without log-probabilities reads back lp NaN and top_ids -1.  b200_stream_read still works on
+ * any stream and drops the records. */
+int b200_stream_read_lp(b200_stream_t * st, int32_t * sessions, int32_t * ids, double * lp, int32_t * top_ids,
+                        double * top_lp, int cap, int * n_out);
 int b200_stream_cancel(b200_stream_t * st, int session);
 /* b200_session_copy for sessions of an open stream, with one destination, on every slice of its chain: rows [0, n_keep)
  * of src to dst and dst's position to n_keep.  Enqueued on the stream's CUDA stream, so it runs after every step still in
