@@ -111,6 +111,8 @@ def lib() -> C.CDLL:
                            ("b200_session_forward_steps_device", [vp, ci, vp, ci, vp, ci]),
                            ("b200_extra_sample", [vp, vp, ci, vp, vp]),
                            ("b200_score", [vp, ci, vp, vp, vp, ci, vp, vp]), ("b200_extra_nll", [vp, vp, ci, vp, vp]),
+                           ("b200_perplexity_windows", [vp, ci, vp, vp, ci, vp, ci, ci, ci, ci, vp]),
+                           ("b200_extra_ppl_terms", [vp, vp, ci, vp, vp]),
                            ("b200_stream_open", [vp, ci, vp, ci, ci, C.POINTER(vp)]),
                            ("b200_stream_add", [vp, ci, vp, ci, ci, vp, vp, ci]),
                            ("b200_stream_read", [vp, vp, vp, ci, C.POINTER(ci)]),
@@ -424,6 +426,17 @@ class Extra:
         check(lib().b200_extra_nll(self._h, _ptr(x), len(x), _ptr(t), _ptr(out)))
         return out
 
+    def ppl_terms(self, logits: np.ndarray, targets) -> np.ndarray:
+        """llama.cpp's perplexity term on the device (b200_extra_ppl_terms): -logf(softmax(row k)[targets[k]]) with the
+        float exps summed in double in index order (client.ppl_terms is the host twin).  -> [n] float32."""
+        x = np.ascontiguousarray(logits, dtype=np.float32).reshape(-1, self.n_vocab)
+        t = np.ascontiguousarray(targets, dtype=np.int32)
+        if len(t) != len(x):
+            raise ValueError("need one target per row (%d), got %d" % (len(x), len(t)))
+        out = np.zeros(len(x), np.float32)
+        check(lib().b200_extra_ppl_terms(self._h, _ptr(x), len(x), _ptr(t), _ptr(out)))
+        return out
+
     def logprobs(self, logits: np.ndarray, ids, n_top: int):
         """k_logprob_rows on the device (b200_extra_logprobs): for each row of [n][n_vocab] logits, log softmax(row)[ids[k]]
         in float64 and the n_top ids of largest logit (equal logits: lower id first) with theirs.
@@ -595,6 +608,40 @@ def score(slices, extra: Extra, sessions, token_lists) -> list:
     out = np.zeros(max(int(fed.sum()), 1), np.float64)
     check(lib().b200_score(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks), _ptr(out)))
     return np.split(out[:int(fed.sum())], np.cumsum(fed)[:-1])
+
+
+def ppl_window_rows(n_tokens: int, n_ctx: int, n_batch: int = 512):
+    """perplexity.cpp's window rules (:37, :48, :103, :130) -> (n_chunk, n_batch, first, n_scored): n_chunk windows of
+    n_ctx ids (a trailing partial window dropped), segments of n_batch = min(n_batch, n_ctx) rows, rows j in
+    [first, n_ctx - 1) scored, first = min(512, n_ctx / 2)."""
+    n_ctx = _int("n_ctx", n_ctx, 2, 2 ** 31 - 1)
+    n_batch = min(_int("n_batch", n_batch, 1, 2 ** 31 - 1), n_ctx)
+    first = min(512, n_ctx // 2)
+    return n_tokens // n_ctx, n_batch, first, n_ctx - 1 - first
+
+
+def perplexity_windows(slices, extra: Extra, sessions, tokens, n_ctx: int, n_batch: int = 512,
+                       fast: bool = False) -> np.ndarray:
+    """llama.cpp's windowed perplexity on the device (b200_perplexity_windows): tokens (the text tokenized with BOS) cut
+    into windows of n_ctx ids, each evaluated from n_past 0 with its id 0 replaced by BOS, in segments of n_batch rows,
+    len(sessions) windows per wave at most.  -> float32 [n_chunk][n_scored]: row i holds window i's terms -logf(prob)
+    for rows first .. n_ctx - 2 (ppl_window_rows).  The sessions are left at n_past 0.  fast: the tensor-core prefill
+    on Q4_0 / Q8_0 slices (other formats ignore it)."""
+    n_chunk, _, _, n_scored = ppl_window_rows(len(tokens), n_ctx, n_batch)
+    ids = np.ascontiguousarray(sessions, dtype=np.int32).reshape(-1)
+    if len(ids) < 1:
+        raise ValueError("perplexity_windows needs at least one session")
+    if len(set(ids.tolist())) != len(ids):
+        raise ValueError("session listed twice: %s" % ids.tolist())
+    toks = np.ascontiguousarray(np.asarray(tokens, np.int64).reshape(-1), dtype=np.int32)
+    if len(toks) and (toks.min() < 0 or toks.max() >= extra.n_vocab):
+        raise ValueError("token ids must lie in [0, %d)" % extra.n_vocab)
+    handles = (C.c_void_p * max(len(slices), 1))(*[s.handle for s in slices])
+    out = np.zeros(max(n_chunk * n_scored, 1), np.float32)
+    keep = toks if len(toks) else np.zeros(1, np.int32)
+    check(lib().b200_perplexity_windows(handles, len(slices), extra.handle, _ptr(ids), len(ids), _ptr(keep), len(toks),
+                                        n_ctx, n_batch, int(bool(fast)), _ptr(out)))
+    return out[:n_chunk * n_scored].reshape(n_chunk, n_scored)
 
 
 def _int(name: str, v, lo: int, hi: int) -> int:

@@ -78,6 +78,59 @@ def token_logprobs(logits, token, n_top: int):
         return lp(token), [(int(i), lp(i)) for i in top]
 
 
+def ppl_terms(logits, targets) -> np.ndarray:
+    """llama.cpp's perplexity term for each row of [n][n_vocab] logits (perplexity.cpp:12-26, 103-113), the host twin of
+    the device's (include/b200_slice.h): m = max x, e_i = expf(x_i - m) with the subtraction in float32, S = the e_i
+    summed in float64 strictly in index order (a sequential cumsum: np.sum is pairwise), prob = float32(e_t / S),
+    term = -logf(prob).  expf / logf are float64 exp / log rounded to float32, as on the device; glibc's expf / logf, which
+    perplexity.cpp calls, differ from them only near float midpoints.  A row with a NaN or +inf logit, or all -inf, gives
+    NaN; a prob that underflows to 0 gives +inf.  -> [n] float32."""
+    t = np.asarray(targets, dtype=np.int64).reshape(-1)
+    x = np.asarray(logits, dtype=np.float32).reshape(len(t), -1)
+    out = np.empty(len(t), np.float32)
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+        for k, (row, tk) in enumerate(zip(x, t)):
+            if np.isnan(row).any() or (row == np.inf).any() or (row == -np.inf).all():
+                out[k] = np.nan
+                continue
+            e = np.exp((row - row.max()).astype(np.float64)).astype(np.float32)
+            S = np.cumsum(e, dtype=np.float64)[-1]
+            prob = np.float32(np.float64(e[tk]) / S)
+            out[k] = -np.float32(np.log(np.float64(prob)))
+    return out
+
+
+def running_perplexity(terms) -> List[float]:
+    """The values perplexity.cpp prints after each window, from terms [n_chunk][n_scored]: nll (float64) adds the terms
+    window by window, row by row,
+    then exp(nll / count) (perplexity.cpp:111-115)."""
+    out, nll, count = [], 0.0, 0
+    for row in np.asarray(terms, np.float32):
+        for v in row:
+            nll += float(v)
+            count += 1
+        out.append(float(np.exp(nll / count)) if count else float("nan"))
+    return out
+
+
+def windowed_perplexity_terms(tokens, n_ctx: int, n_batch: int, eval_segment) -> np.ndarray:
+    """perplexity.cpp's loop (:37-113) on the host: for each whole window of n_ctx ids, with its id 0 replaced by BOS,
+    eval_segment(ids, n_past) -> logits [len(ids)][n_vocab] is called segment by segment (n_past 0 starts a window), and
+    the scored rows' terms are ppl_terms of those logits.  -> float32 [n_chunk][n_scored]."""
+    from .capi import ppl_window_rows
+    tokens = [int(t) for t in tokens]
+    n_chunk, n_batch, first, n_scored = ppl_window_rows(len(tokens), n_ctx, n_batch)
+    out = np.zeros((n_chunk, n_scored), np.float32)
+    for i in range(n_chunk):
+        start = i * n_ctx
+        ids = [1] + tokens[start + 1:start + n_ctx]          # llama_token_bos()
+        logits = np.concatenate([np.asarray(eval_segment(ids[j:j + n_batch], j), np.float32).reshape(len(ids[j:j + n_batch]), -1)
+                                 for j in range(0, n_ctx, n_batch)])
+        if n_scored:
+            out[i] = ppl_terms(logits[first:n_ctx - 1], tokens[start + first + 1:start + n_ctx])
+    return out
+
+
 class Sampler:
     """The reference's sampler, plus llama.cpp's top-k and top-p truncation (off when both are None, which runs the
     reference's arithmetic unchanged).  Truncation ranks the ids by the scaled logits y descending (equal y: lower id
@@ -175,6 +228,21 @@ class DistributedLLM:
         p = _softmax(logits, axis=1)[np.arange(n), tokens[1:]]
         return float(np.exp(-np.log(p).sum() / n))
 
+    def perplexity_windows(self, text, n_ctx: int = 512, n_batch: int = 512) -> List[float]:
+        """llama.cpp's windowed perplexity through the nodes: each window starts from cleared contexts and is fed segment
+        by segment, with get_logits(all) after each; the terms are ppl_terms.  -> the running perplexity after each
+        window, as perplexity.cpp prints it."""
+        extra = self.extra_layers_path
+        tokens = self.llm.tokenize_prompt(extra, text)
+
+        def eval_segment(ids, n_past):
+            if n_past == 0:
+                self.clear_context()
+            emb = self.propagate_tensor(self.llm.prepare_embeddings(extra, ids))
+            return np.array(self.llm.get_logits(extra, emb, True), np.float32).reshape(len(ids), -1)
+
+        return running_perplexity(windowed_perplexity_terms(tokens, n_ctx, n_batch, eval_segment))
+
     def clear_context(self):
         for address in self.addresses:
             Connection(address).clear_context()
@@ -203,11 +271,12 @@ class LocalPipeline:
     """All slices of a nodes_map on the GPUs of THIS box: slice i on device i, activations chained device to
     device (peer copy) -- the single-process equivalent of the NCCL pipeline bench.py runs with one rank per GPU."""
 
-    def __init__(self, slice_paths: Sequence[str], devices: Sequence[int] = None, n_ctx: int = 0):
+    def __init__(self, slice_paths: Sequence[str], devices: Sequence[int] = None, n_ctx: int = 0, n_sessions: int = 1):
+        """n_sessions: KV-cache sessions per slice (perplexity_windows runs up to that many windows per pass)."""
         from . import capi
         self.capi = capi
         devices = list(devices) if devices is not None else list(range(len(slice_paths)))
-        self.slices = [capi.Slice(p, d, n_ctx) for p, d in zip(slice_paths, devices)]
+        self.slices = [capi.Slice(p, d, n_ctx, n_sessions=n_sessions) for p, d in zip(slice_paths, devices)]
         self.slices.sort(key=lambda s: s.info.first_layer)
         self._extra = None
 
@@ -313,6 +382,21 @@ class LocalPipeline:
         for v in self.capi.score(self.slices, extra, [0], [tokens])[0]:
             nll += v
         return float(np.exp(nll / n))
+
+    def perplexity_windows(self, extra_path: str, text: str, n_ctx: int = 512, n_batch: int = 512, sessions=None,
+                           fast: bool = False) -> List[float]:
+        """llama.cpp's `perplexity` on this box (capi.perplexity_windows): tokenize with BOS, cut into windows of n_ctx
+        ids, evaluate each from an empty context in segments of n_batch rows, score the second half of each window on
+        the device.  -> the running perplexity after each window, as perplexity.cpp prints it (nll summed in float64 in
+        its order).  sessions: the sessions that windows run in side by side (default: every session of the slices, so
+        load them with n_sessions > 1 for several windows per pass); they are left at n_past 0.  fast: the
+        tensor-core prefill on Q4_0 / Q8_0 slices.  Needs every slice on one device."""
+        extra = self._device_extra(extra_path, "windowed perplexity")
+        if sessions is None:
+            sessions = list(range(min(s.n_sessions for s in self.slices)))
+        tokens = extra.tokenize(text)
+        terms = self.capi.perplexity_windows(self.slices, extra, sessions, tokens, n_ctx, n_batch, fast=fast)
+        return running_perplexity(terms)
 
     def propagate_tensor(self, embeddings) -> np.ndarray:
         x = np.ascontiguousarray(embeddings, dtype=np.float32)

@@ -84,6 +84,7 @@ struct b200_slice {
     bool skip_attention = false;   // measurement aid: replay only the weight matmuls of a step (bench.py roofline)
     bool attn_lut_smem = true;     // single-token attention stages the exp table in shared memory (decided at load)
     bool fast_prefill = false; int fast_min_tokens = 32; uint16_t * xh = nullptr;   // tensor-core prefill (fast mode)
+    bool fast_pass = false;        // b200_perplexity_windows(fast = 1): mixed passes of any row count take fast mode too
     int opt_ns = 0, opt_cta_per_sm = 0, opt_nc = 0, opt_pre = 3, opt_nomath = 0;   // read once at load (environment)
     float ema_token_ms = 0.f;              // host-buffer decode calls: smoothed device time of one token (sleep-then-poll wait)
     std::mutex mu;
@@ -689,8 +690,9 @@ static int enqueue_layers(b200_slice * s, const float * in, int N, float * out) 
         float * nxt = (il == s->L - 1) ? out : ((il & 1) ? s->xb : s->xa);
         // fast mode is for single-session prefill calls only: a single-token step, a batched step or a mixed pass (cols:
         // columns of several sessions) stays exact, so decode, batch_forward and mixed_forward keep the reference's bits
-        // whatever min_tokens is
-        const bool fast = s->fast_prefill && N > 1 && !s->cols && N >= s->fast_min_tokens &&
+        // whatever min_tokens is.  The windowed perplexity's fast mode (fast_pass) is the one caller that asks for it in
+        // mixed passes: it only needs each window's rows close to exact
+        const bool fast = N > 1 && ((s->fast_prefill && !s->cols && N >= s->fast_min_tokens) || s->fast_pass) &&
                           (s->wtype == kWT_Q4_0 || s->wtype == kWT_Q8_0) &&
                           (Lw.qkv.n_tiles * Lw.qkv.TR) % 16 == 0 &&
                           (Lw.wo.n_tiles * Lw.wo.TR) % 16 == 0 && (Lw.w13.n_tiles * Lw.w13.TR) % 16 == 0;
@@ -2143,6 +2145,8 @@ struct b200_extra {
     uint32_t * d_pen = nullptr; uint64_t * d_seeds = nullptr; int * d_bad = nullptr; int cap_sample = 0;
     // scoring (b200_score): the embedded rows of one pass [rows][n_embd], and the NLL of every scored row
     float * d_sx = nullptr; int cap_sx = 0; double * d_nll = nullptr; int cap_nll = 0;
+    // windowed perplexity (b200_perplexity_windows): every window's terms
+    float * d_terms = nullptr; int cap_terms = 0;
     // log-probabilities (k_logprob_rows): lp [rows], top ids and their lp [rows][n_top]
     double * d_lp = nullptr; int cap_lp = 0; int32_t * d_topi = nullptr; int cap_topi = 0; double * d_topl = nullptr; int cap_topl = 0;
     std::vector<std::pair<std::string, float>> vocab;
@@ -2728,6 +2732,71 @@ __global__ void __launch_bounds__(1024) k_nll_rows(const float * logits, int n, 
     double m, S;
     const bool ok = row_softmax(x, n, &m, &S);
     if (threadIdx.x == 0) nll[k] = ok ? -row_logp(x[tgt[k]], m, S) : __longlong_as_double(0x7ff8000000000000ll);
+}
+
+// ---- llama.cpp's perplexity term (b200_perplexity_windows, b200_extra_ppl_terms): perplexity.cpp:12-26 and 103-113.
+// For a row x of n logits and target t: m = max x, e_i = expf(x_i - m) with the subtraction in float, S = the e_i summed
+// in double strictly in index order 0 .. n-1, prob = (float)(e_t / S), term = -logf(prob) (std::log of a float is the
+// float overload).  expf / logf here are the double functions rounded to float; perplexity.cpp calls glibc's, which are
+// not correctly rounded near float midpoints, so that is the one place the two can give different bits.  A row with a
+// NaN or +inf logit, or all -inf, gives NaN (as k_nll_rows); a prob that underflows to 0 gives +inf.
+// The ordered sum is a dependent chain of n double additions per row, so a block takes kPplRows rows at once: warp w < 8
+// finds row w's max, then warps 1.. compute the e_i of a tile of every row into shared memory while lane r of warp 0 adds
+// the previous tile's row-r values to its one accumulator (double-buffered; rows padded a float so the eight summing
+// lanes read eight banks).
+constexpr int kPplRows = 8, kPplTile = 512, kPplThreads = 256;
+
+__device__ __forceinline__ float ppl_expf(float v) { return __double2float_rn(exp((double) v)); }
+
+__global__ void __launch_bounds__(kPplThreads) k_ppl_rows(const float * logits, int n, int n_rows, const int32_t * tgt,
+                                                          float * term) {
+    __shared__ float s_e[2][kPplRows][kPplTile + 1];
+    __shared__ float s_m[kPplRows];
+    __shared__ int s_ok[kPplRows];
+    const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
+    const int r0 = blockIdx.x * kPplRows, nr = min(kPplRows, n_rows - r0);
+    if (wid < nr) {
+        const float * x = logits + (size_t)(r0 + wid) * n;
+        float mx = -INFINITY; bool bad = false;
+        for (int i = lane; i < n; i += 32) { const float v = x[i]; bad |= v != v || v == INFINITY; mx = fmaxf(mx, v); }
+        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        bad = __any_sync(0xffffffffu, bad);
+        if (lane == 0) { s_m[wid] = mx; s_ok[wid] = !bad && mx != -INFINITY; }
+    }
+    __syncthreads();
+    const int n_tiles = (n + kPplTile - 1) / kPplTile;
+    auto produce = [&](int tile) {                        // warps 1..: e_i of columns [tile * kPplTile, +kPplTile)
+        const int c0 = tile * kPplTile, cn = min(kPplTile, n - c0);
+        float (*dst)[kPplTile + 1] = s_e[tile & 1];
+        for (int idx = t - 32; idx < nr * kPplTile; idx += kPplThreads - 32) {
+            const int r = idx / kPplTile, c = idx % kPplTile;
+            if (c < cn) dst[r][c] = ppl_expf(__fsub_rn(logits[(size_t)(r0 + r) * n + c0 + c], s_m[r]));
+        }
+    };
+    if (wid > 0) produce(0);
+    __syncthreads();
+    double S = 0.0;
+    for (int k = 0; k < n_tiles; k++) {
+        if (wid > 0) {
+            if (k + 1 < n_tiles) produce(k + 1);
+        } else if (t < nr) {
+            const float * e = s_e[k & 1][t];
+            const int cn = min(kPplTile, n - k * kPplTile);
+#pragma unroll 8
+            for (int c = 0; c < cn; c++) S = __dadd_rn(S, (double) e[c]);
+        }
+        __syncthreads();
+    }
+    if (t < nr) {
+        const int r = r0 + t;
+        float out = __int_as_float(0x7fc00000);
+        if (s_ok[t]) {
+            const float et = ppl_expf(__fsub_rn(logits[(size_t) r * n + tgt[r]], s_m[t]));
+            const float prob = __double2float_rn(__ddiv_rn((double) et, S));
+            out = -__double2float_rn(log((double) prob));
+        }
+        term[r] = out;
+    }
 }
 
 // ---- log-probabilities of drawn ids (b200_generate_lp, b200_stream_read_lp, b200_extra_logprobs): the raw distribution
@@ -3389,6 +3458,134 @@ static int score_locked(b200_slice * const * slices, int n_slices, b200_extra * 
     return 0;
 }
 
+// ---------------------------------------------------------------- windowed perplexity (b200_perplexity_windows)
+// Rows the windowed perplexity's lm_head and k_ppl_rows take at a time: a window's scored rows of one pass (255 at
+// n_ctx 512) in one block; the logits scratch is 32 MB at 32000 ids.  Rows of the lm_head are independent.
+static constexpr int kPplLmRows = 256;
+
+// perplexity.cpp:37, 48, 103 and 130: the windows, their segments and their scored rows; and the waves.
+struct PplPlan { int n_ctx, n_batch, first, n_scored, n_chunk, n_pass, W; };
+
+// Everything b200_perplexity_windows checks before it changes anything (the handles' mutexes are held).
+static int ppl_check(b200_slice * const * slices, int n_slices, const b200_extra * e, const int * sessions, int n_sessions,
+                     const int32_t * tokens, int n_tokens, int n_ctx, int n_batch, PplPlan & p) {
+    if (int rc = chain_check(slices, n_slices, e)) return rc;
+    if (n_ctx < 2) return fail(B200_EINVAL, "n_ctx must be at least 2 (got %d)", n_ctx);
+    if (n_batch < 1) return fail(B200_EINVAL, "n_batch must be positive (got %d)", n_batch);
+    if (n_tokens < 0) return fail(B200_EINVAL, "n_tokens must not be negative (got %d)", n_tokens);
+    int pass_rows = INT_MAX;
+    for (int i = 0; i < n_slices; i++) {
+        const b200_slice * s = slices[i];
+        if (n_ctx > s->n_ctx) return fail(B200_ECONTEXT, "window n_ctx %d exceeds slice %d's n_ctx %d", n_ctx, i, s->n_ctx);
+        for (int k = 0; k < n_sessions; k++)
+            if (sessions[k] < 0 || sessions[k] >= s->n_sessions)
+                return fail(B200_EINVAL, "session %d outside [0, %d) on slice %d", sessions[k], s->n_sessions, i);
+        pass_rows = std::min(pass_rows, s->n_ctx);
+    }
+    std::vector<char> seen(slices[0]->n_sessions, 0);
+    for (int k = 0; k < n_sessions; k++) {
+        if (seen[sessions[k]]) return fail(B200_EINVAL, "session %d listed twice", sessions[k]);
+        seen[sessions[k]] = 1;
+    }
+    if (int rc = check_tokens(tokens, n_tokens, e->n_vocab, "token")) return rc;
+    p.n_ctx = n_ctx;
+    p.n_batch = std::min(n_batch, n_ctx);
+    p.first = std::min(512, n_ctx / 2);
+    p.n_scored = n_ctx - 1 - p.first;
+    p.n_chunk = n_tokens / n_ctx;
+    p.n_pass = (n_ctx + p.n_batch - 1) / p.n_batch;
+    p.W = std::min(n_sessions, pass_rows / p.n_batch);     // >= 1: n_batch <= n_ctx <= pass_rows
+    return 0;
+}
+
+// Sets the slices' fast_pass for the life of the call.
+struct FastPass {
+    std::vector<b200_slice *> slices;
+    FastPass(b200_slice * const * s, int n, bool on) : slices(s, s + n) { for (b200_slice * p : slices) p->fast_pass = on; }
+    ~FastPass() { for (b200_slice * p : slices) p->fast_pass = false; }
+};
+
+// n sessions back to n_past 0 on every slice, stream-ordered on the loop's stream.
+static int ppl_reset(b200_slice * const * slices, int n_slices, const int * sessions, int n) {
+    for (int i = 0; i < n_slices; i++)
+        for (int k = 0; k < n; k++) {
+            b200_slice * s = slices[i];
+            B200_CUDA(cudaMemsetAsync(s->d_npast + sessions[k], 0, 4, s->stream));
+            s->past[sessions[k]] = 0;
+        }
+    return 0;
+}
+
+// Uploaded ids: the fed ids in the order the passes take them (wave by wave, pass by pass, window by window, so each
+// pass's rows are contiguous), every window's id 0 already BOS, then the targets in the layout of terms.  Each pass:
+// embed its rows, run them through every slice as one mixed pass (segment p of each window of the wave at positions
+// p * n_batch ..), then for each window the lm_head and k_ppl_rows over its scored rows only.
+static int ppl_locked(b200_slice * const * slices, int n_slices, b200_extra * e, const int * sessions, int n_sessions,
+                      const int32_t * tokens, const PplPlan & P, bool fast, float * terms) {
+    b200_slice * x = &e->ctx;
+    B200_CUDA(cudaSetDevice(x->device));
+    for (int i = 0; i < n_slices; i++) B200_CUDA(cudaStreamSynchronize(slices[i]->stream));
+    const size_t n_fed = (size_t) P.n_chunk * P.n_ctx, n_terms = (size_t) P.n_chunk * P.n_scored;
+    StreamLoan loan(slices, n_slices, x->stream);
+    if (int rc = ppl_reset(slices, n_slices, sessions, n_sessions)) return rc;
+    if (n_terms == 0) return 0;
+    std::vector<int32_t> ids(n_fed + n_terms);
+    size_t at = 0;
+    for (int c0 = 0; c0 < P.n_chunk; c0 += P.W)
+        for (int p = 0; p < P.n_pass; p++) {
+            const int j0 = p * P.n_batch, cp = std::min(P.n_batch, P.n_ctx - j0);
+            for (int c = c0; c < std::min(c0 + P.W, P.n_chunk); c++)
+                for (int j = j0; j < j0 + cp; j++) ids[at++] = j == 0 ? 1 : tokens[(size_t) c * P.n_ctx + j];   // BOS = 1
+        }
+    for (int c = 0; c < P.n_chunk; c++)
+        for (int j = P.first; j < P.n_ctx - 1; j++) ids[at++] = tokens[(size_t) c * P.n_ctx + j + 1];
+    int rc;
+    if ((rc = extra_reserve(e, kPplLmRows)) || (rc = extra_reserve_ids(e, (int) ids.size())) ||
+        (rc = extra_regrow(e, e->d_sx, e->cap_sx, (size_t) e->E, P.W * P.n_batch)) ||
+        (rc = extra_regrow(e, e->d_terms, e->cap_terms, 1, (int) n_terms)))
+        return rc;
+    B200_CUDA(cudaMemcpyAsync(e->d_ids, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice, x->stream));
+    FastPass fp(slices, n_slices, fast);
+    const int32_t * d_tgt = e->d_ids + n_fed;
+    std::vector<int> counts(P.W);
+    size_t row0 = 0;
+    for (int c0 = 0; c0 < P.n_chunk; c0 += P.W) {
+        const int nw = std::min(P.W, P.n_chunk - c0);
+        if (c0 > 0 && (rc = ppl_reset(slices, n_slices, sessions, nw))) return rc;
+        for (int p = 0; p < P.n_pass; p++) {
+            const int j0 = p * P.n_batch, cp = std::min(P.n_batch, P.n_ctx - j0), N = nw * cp;
+            std::fill(counts.begin(), counts.end(), cp);
+            k_embed_rows<<<dim3((e->E + 255) / 256, N), 256, 0, x->stream>>>(e->emb_raw, e->emb_type, e->E, e->d_ids + row0,
+                                                                               e->n_vocab, e->d_sx);
+            B200_CUDA(cudaGetLastError());
+            x->launches++;
+            row0 += N;
+            const float * cur = e->d_sx;
+            for (int i = 0; i < n_slices; i++) {
+                b200_slice * s = slices[i];
+                if ((rc = pass_locked(s, sessions, counts.data(), nw, cur, s->d_out, false))) return rc;
+                cur = s->d_out;
+            }
+            // scored rows of this segment: j in [max(first, j0), min(n_ctx - 1, j0 + cp))
+            const int a = std::max(P.first, j0), b = std::min(P.n_ctx - 1, j0 + cp);
+            for (int w = 0; w < nw; w++)
+                for (int j = a; j < b; j += kPplLmRows) {
+                    const int nb = std::min(kPplLmRows, b - j);
+                    const size_t t0 = (size_t)(c0 + w) * P.n_scored + (j - P.first);
+                    if ((rc = extra_lmhead(e, cur + ((size_t) w * cp + (j - j0)) * e->E, nb))) return rc;
+                    k_ppl_rows<<<(nb + kPplRows - 1) / kPplRows, kPplThreads, 0, x->stream>>>(e->d_logits, e->n_vocab, nb,
+                                                                                           d_tgt + t0, e->d_terms + t0);
+                    B200_CUDA(cudaGetLastError());
+                    x->launches++;
+                }
+        }
+    }
+    if ((rc = ppl_reset(slices, n_slices, sessions, n_sessions))) return rc;
+    B200_CUDA(cudaMemcpyAsync(terms, e->d_terms, n_terms * 4, cudaMemcpyDeviceToHost, x->stream));
+    B200_CUDA(cudaStreamSynchronize(x->stream));
+    return 0;
+}
+
 // ---------------------------------------------------------------- speculative decoding (b200_generate_speculative)
 // One iteration, with t the last emitted id, m the ids emitted so far and p the target's position (where t goes):
 //   draft  a two-row decode pass [token at p - 1, t], then k - 1 replays of its decode step, each followed by its lm_head
@@ -3819,6 +4016,37 @@ int b200_extra_nll(b200_extra_t * e, const float * logits, int n_rows, const int
     B200_CUDA(cudaGetLastError());
     s->launches++;
     B200_CUDA(cudaMemcpyAsync(nll, e->d_nll, (size_t) n_rows * 8, cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    return 0;
+}
+
+int b200_perplexity_windows(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
+                            int n_sessions, const int32_t * tokens, int n_tokens, int n_ctx, int n_batch, int fast,
+                            float * terms) {
+    if (!slices || n_slices < 1 || !e || !sessions || n_sessions < 1 || (!tokens && n_tokens > 0) || (!terms && n_tokens > 0))
+        return fail(B200_EINVAL, "b200_perplexity_windows: null argument or empty list");
+    std::vector<std::unique_lock<std::mutex>> locks;
+    if (int rc = lock_handles(slices, n_slices, e, locks)) return rc;
+    PplPlan plan;
+    if (int rc = ppl_check(slices, n_slices, e, sessions, n_sessions, tokens, n_tokens, n_ctx, n_batch, plan)) return rc;
+    return ppl_locked(slices, n_slices, e, sessions, n_sessions, tokens, plan, fast != 0, terms);
+}
+
+int b200_extra_ppl_terms(b200_extra_t * e, const float * logits, int n_rows, const int32_t * targets, float * terms) {
+    if (!e || !logits || n_rows < 1 || !targets || !terms) return fail(B200_EINVAL, "b200_extra_ppl_terms: null argument or no rows");
+    std::lock_guard<std::mutex> lk(e->mu); B200_UNOWNED(&e->ctx);
+    if (int rc = check_tokens(targets, n_rows, e->n_vocab, "target")) return rc;
+    b200_slice * s = &e->ctx;
+    B200_CUDA(cudaSetDevice(s->device));
+    int rc;
+    if ((rc = extra_reserve(e, n_rows)) || (rc = extra_reserve_ids(e, n_rows)) || (rc = extra_regrow(e, e->d_terms, e->cap_terms, 1, n_rows)))
+        return rc;
+    B200_CUDA(cudaMemcpyAsync(e->d_logits, logits, (size_t) n_rows * e->n_vocab * 4, cudaMemcpyHostToDevice, s->stream));
+    B200_CUDA(cudaMemcpyAsync(e->d_ids, targets, (size_t) n_rows * 4, cudaMemcpyHostToDevice, s->stream));
+    k_ppl_rows<<<(n_rows + kPplRows - 1) / kPplRows, kPplThreads, 0, s->stream>>>(e->d_logits, e->n_vocab, n_rows, e->d_ids, e->d_terms);
+    B200_CUDA(cudaGetLastError());
+    s->launches++;
+    B200_CUDA(cudaMemcpyAsync(terms, e->d_terms, (size_t) n_rows * 4, cudaMemcpyDeviceToHost, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     return 0;
 }

@@ -369,6 +369,37 @@ int b200_score(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, co
  * nll[k] as b200_score computes it for row k and target targets[k]; a target outside [0, n_vocab) is B200_EINVAL. */
 int b200_extra_nll(b200_extra_t * e, const float * logits, int n_rows, const int32_t * targets, double * nll);
 
+/* ---- llama.cpp's windowed perplexity (examples/perplexity/perplexity.cpp:29-117, 130) -----------------------------------
+ * tokens (n_tokens ids, the text tokenized with BOS) are cut into n_chunk = n_tokens / n_ctx windows; a trailing partial
+ * window is dropped, and fewer than n_ctx ids give zero windows (not an error).  n_batch is first cut to min(n_batch, n_ctx)
+ * (the program's command line also caps -b at 512, examples/common.cpp:263; this call takes any n_batch).
+ * Window i is tokens[i*n_ctx, (i+1)*n_ctx) with its id 0 replaced by BOS (1); it runs from n_past 0 in segments of n_batch
+ * rows at positions 0, n_batch, ... (the last one may be shorter), and rows j in [first, n_ctx - 1), first =
+ * min(512, n_ctx / 2), are scored against tokens[i*n_ctx + j + 1]:
+ *     terms[i][j - first] = -logf(prob),  prob = (float)(e_t / S),  e_k = expf(x_k - m) (the subtraction in float),
+ *     m = max x,  S = sum of the e_k in double, strictly in index order 0 .. n_vocab-1.
+ * expf / logf are the double functions rounded to float: (float) exp((double) v), (float) log((double) p).  glibc's
+ * expf / logf, which perplexity.cpp calls, differ from these only at float rounding midpoints.  A row with a NaN or +inf
+ * logit, or all -inf, gives NaN; a prob that underflows to 0 gives +inf.  Summing the terms window by window, row by row,
+ * in double gives the running perplexity perplexity.cpp prints after each window, exp(nll / count).
+ *   - Windows run in waves of W = min(n_sessions, pass rows / n_batch), pass rows being the smallest slice n_ctx; window
+ *     w of a wave uses sessions[w].  A wave takes ceil(n_ctx / n_batch) mixed passes, pass p carrying segment p of every
+ *     window in it, so each window's rows equal b200_session_forward per segment on that window alone.  The lm_head and
+ *     the term kernel run only on scored rows.
+ *   - fast = 1 runs the passes' matmuls on the tensor-core prefill where a slice's format has it (Q4_0, Q8_0); other
+ *     formats ignore it.  fast = 0: every row is exact.
+ *   - The ids go up once (BOS already in place), the host synchronises once and reads back only terms
+ *     [n_chunk][n_ctx - 1 - first].  The listed sessions are cleared first and left at n_past 0 on every slice.
+ *   - Locking, slice checks and all-or-nothing errors are as b200_score: B200_EINVAL for n_ctx < 2, n_batch < 1, a
+ *     session listed twice or out of range, an id outside [0, n_vocab) or a null argument; B200_ECONTEXT when n_ctx is
+ *     larger than some slice's n_ctx. */
+int b200_perplexity_windows(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
+                            int n_sessions, const int32_t * tokens, int n_tokens, int n_ctx, int n_batch, int fast,
+                            float * terms);
+/* The term kernel on host logits [n_rows][n_vocab]: terms[k] as b200_perplexity_windows computes it for row k and target
+ * targets[k]; a target outside [0, n_vocab) is B200_EINVAL. */
+int b200_extra_ppl_terms(b200_extra_t * e, const float * logits, int n_rows, const int32_t * targets, float * terms);
+
 /* ---- log-probabilities of generated ids ("logprobs") ------------------------------------------------------------------
  * For the logits row x (n_vocab floats) that a step drew id t from:
  *   - the distribution is the model's raw one, softmax(x) in float64: before temperature, repeat penalty and top-k/top-p,
