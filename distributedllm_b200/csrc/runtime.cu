@@ -1730,12 +1730,12 @@ int b200_debug_trace_read(b200_slice_t * s, unsigned long long * out, int * cls,
 
 /* Test hook: copy `count` 32-bit words of an internal activation buffer to the host after a
  * forward (0 qkv, 1 att, 2 ffin, 3 gate, 4 xa, 5 xb, 6 q16, 7 k-cache, 8 v-cache, 9 xh: the fp16 activations of the
- * last fast-mode matmul). */
+ * last fast-mode matmul, 10 the slice's output staging buffer d_out). */
 int b200_debug_read(b200_slice_t * s, int which, size_t offset_words, size_t count, void * out) {
     if (!s || !out) return fail(B200_EINVAL, "null argument");
     B200_UNOWNED(s);
-    const void * src[10] = {s->qkv, s->att, s->ffin, s->gate, s->xa, s->xb, s->q16, s->kc, s->vc, s->xh};
-    if (which < 0 || which > 9) return fail(B200_EINVAL, "bad buffer id %d", which);
+    const void * src[11] = {s->qkv, s->att, s->ffin, s->gate, s->xa, s->xb, s->q16, s->kc, s->vc, s->xh, s->d_out};
+    if (which < 0 || which > 10) return fail(B200_EINVAL, "bad buffer id %d", which);
     B200_CUDA(cudaSetDevice(s->device));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     B200_CUDA(cudaMemcpy(out, (const uint32_t *) src[which] + offset_words, count * 4, cudaMemcpyDeviceToHost));

@@ -149,9 +149,14 @@ int b200_mixed_forward_device(b200_slice_t * s, const int * sessions, const int 
  * the dequantisation fused in (csrc/fastgemm2.cuh; Q4_1, Q5_0, Q5_1, Q4_K / Q6_K and F16 slices ignore the switch and stay exact).
  * NOT bit-exact: operands are rounded to fp16 after the reference's Q8_0 activation quantisation and summed in fp32.
  * Each matmul output is within TAU * sum_k |w16 * x16| of the float64 sum of the same fp16 operands (TAU <= 2^-16, see
- * tests/test_gpu_fast_prefill.py, which also bounds the deviation from exact mode).  Off by default (or
+ * tests/test_gpu_fast_prefill.py, which also bounds the deviation from exact mode).  The bound is checked per matmul in
+ * every kind of call that takes fast mode (tests/test_gpu_fast_prefill_calls.py): prompts from position 0 of up to
+ * n_ctx - 1 rows, later chunks of any session (past the 512-row staged attention window too), the last layer of a
+ * multi-layer slice, and the mixed passes of b200_perplexity_windows(fast = 1).  Off by default (or
  * B200_FAST_PREFILL=1).  Fast mode never applies to a single-token step, a batched step (b200_batch_forward) or a mixed pass (b200_mixed_forward),
- * whatever min_tokens is: decode always runs in exact mode. */
+ * whatever min_tokens is: decode always runs in exact mode, on a cache a fast prefill wrote too (the same bits as an
+ * exact handle restored from that cache).  A call of fewer than min_tokens rows, or any call after the switch is
+ * turned off, is exact mode. */
 int b200_slice_set_fast_prefill(b200_slice_t * s, int on, int min_tokens);
 
 /* Block until everything queued on the slice's stream has finished. */
@@ -182,7 +187,9 @@ float * b200_slice_dev_out(b200_slice_t * s);
 
 /* Test hook: copy `count` 32-bit words of an internal activation buffer to the host after a forward
  * (0 qkv, 1 att, 2 ffin, 3 gate, 4 xa, 5 xb, 6 q16, 7 k-cache, 8 v-cache, 9 xh: the [n_tokens][K] fp16 activations of
- * the last fast-mode matmul, i.e. w2's input after a fast prefill).  Not part of the drop-in surface. */
+ * the last fast-mode matmul, i.e. w2's input after a fast prefill, 10 the slice's output staging buffer
+ * [n_tokens][n_embd] f32, where b200_perplexity_windows' passes leave the last layer's output).  Not part of the
+ * drop-in surface. */
 int b200_debug_read(b200_slice_t * s, int which, size_t offset_words, size_t count, void * out);
 
 /* Measurement aid (bench.py roofline): while on, a decode step launches only its weight-matmul kernels. */

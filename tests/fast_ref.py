@@ -153,3 +153,118 @@ def row_sample(rows: int, tile: int) -> np.ndarray:
     t = r // tile
     keep = (t == 0) | (t == t[-1]) | (r % 8 == t % 8)
     return r[keep]
+
+
+TOKEN_SAMPLE_ABOVE = 512
+
+
+def token_sample(n: int) -> np.ndarray:
+    """The tokens a call of n rows is checked on: all of them up to TOKEN_SAMPLE_ABOVE rows, else row_sample(n, 256) --
+    every row of the first and the last 256-token tile (so of the first and last 128-token tile too) and 32 rows of
+    every other 256-token tile (so at least 16 of every 128-token tile), which keeps the float64 sums a few seconds."""
+    return np.arange(n) if n <= TOKEN_SAMPLE_ABOVE else row_sample(n, 256)
+
+
+# ---------------------------------------------------------------------------------------------- one layer
+class LayerWeights:
+    """A row sample of one layer's matrices as fp16 (every row of the first and last 128-row tile of qkv, wo and w2, of
+    the first and last 64-row tile of w1 / w3, and one row per 8-row group in the others) and its norm weights."""
+
+    def __init__(self, path: str, layer: int, n_embd: int, n_ff: int):
+        E, FF = n_embd, n_ff
+        self.layer, self.E, self.FF = layer, E, FF
+        self.r_qkv, self.r_e, self.r_ff = row_sample(3 * E, 128), row_sample(E, 128), row_sample(FF, 64)
+        pre = "layers.%d." % layer
+        self.w_qkv = stacked_rows(path, [pre + "attention.wq.weight", pre + "attention.wk.weight",
+                                         pre + "attention.wv.weight"], E, self.r_qkv)
+        self.w_o = stacked_rows(path, [pre + "attention.wo.weight"], E, self.r_e)
+        self.w_1 = stacked_rows(path, [pre + "feed_forward.w1.weight"], FF, self.r_ff)
+        self.w_3 = stacked_rows(path, [pre + "feed_forward.w3.weight"], FF, self.r_ff)
+        self.w_2 = stacked_rows(path, [pre + "feed_forward.w2.weight"], E, self.r_e)
+        self.attn_norm = file_f32(path, pre + "attention_norm.weight")
+        self.ffn_norm = file_f32(path, pre + "ffn_norm.weight")
+
+
+def stacked_rows(path: str, names, per: int, sample: np.ndarray) -> np.ndarray:
+    """fp16 weights of `sample` rows of the matrices `names` stacked by rows (`per` rows each), as the packer stacks them."""
+    parts = []
+    for i, nm in enumerate(names):
+        sel = sample[(sample >= i * per) & (sample < (i + 1) * per)] - i * per
+        if len(sel):
+            parts.append(file_rows(path, nm, sel)[0])
+    return np.concatenate(parts)
+
+
+def read_layer(gpu, n: int, E: int, FF: int) -> dict:
+    """The debug reads of the last layer a fast call of n rows ran: the qkv, att, ffin and gate buffers and xh (w2's
+    fp16 input, as uint16)."""
+    return {"qkv": gpu.debug_read(0, n * 3 * E).reshape(n, 3 * E),
+            "att": gpu.debug_read(1, n * E).reshape(n, E),
+            "ffin": gpu.debug_read(2, n * E).reshape(n, E),
+            "gate": gpu.debug_read(3, n * FF).reshape(n, FF),
+            "xh": gpu.debug_read(9, n * FF // 2, np.uint32).view(np.uint16).reshape(n, FF)}
+
+
+def check_layer(w: LayerWeights, x: np.ndarray, reads: dict, y: np.ndarray, tau, floor: float, label: str,
+                tokens: np.ndarray = None, lost_tokens: int = 1) -> tuple:
+    """The four matmuls of one fast-mode layer against the float64 bound, on the rows `tokens` (default: all) of a call.
+    x is the layer's input rows, reads what read_layer returned, y the layer's output rows; tau(K) is the bound of a
+    matmul with K-wide rows, floor the share of outputs one lost 32-wide K block must move outside it.
+      * xh == prep(gate) bit for bit on every row: the activation restatement the bound relies on;
+      * per matmul, the largest normalised error |y - y_ref| / sum_k |w16 * x16| over the sampled rows <= tau(K);
+      * zeroing activation block (K / 32) / 3 in the reference puts >= floor of the outputs outside the bound (numpy
+        only: the bound is tight enough to see one lost block).  lost_tokens = 1 zeroes it in the middle sampled token;
+        more zero it in that many sampled tokens spread from the first to the last and pool their outputs, which
+        estimates the same share from lost_tokens times as many outputs.
+    Returns ({matmul: largest normalised error}, {matmul: share moved by the lost block})."""
+    n = x.shape[0]
+    tokens = np.arange(n) if tokens is None else np.asarray(tokens)
+    assert tokens[0] == 0 and tokens[-1] == n - 1
+    qkv, att, ffin, gate, xh = (reads[k] for k in ("qkv", "att", "ffin", "gate", "xh"))
+    x_2 = prep(gate)
+    bad = int((xh != x_2.view(np.uint16)).sum())
+    assert bad == 0, "%s: xh differs from prep(gate) at %d of %d halves" % (label, bad, xh.size)
+    tk = tokens
+    x_2 = x_2[tk]
+    xs, atts, ffins, gates, ys, qkvs = x[tk], att[tk], ffin[tk], gate[tk], y[tk], qkv[tk]
+    x_qkv, x_o, x_13 = prep(xs, w.attn_norm), prep(atts), prep(ffins, w.ffn_norm)
+    r_qkv, r_e, r_ff = w.r_qkv, w.r_e, w.r_ff
+    errs, moved = {}, {}
+    t = np.array([len(tk) // 2]) if lost_tokens == 1 else np.unique(np.linspace(0, len(tk) - 1, lost_tokens).astype(int))
+    # qkv: plain store
+    ref, mag = reference(w.w_qkv, x_qkv)
+    errs["qkv"] = store_error(qkvs[:, r_qkv], ref, mag)
+    moved["qkv"] = (x_qkv, lambda xm: store_error(qkvs[t][:, r_qkv], *reference(w.w_qkv, xm)))
+    # wo: + residual (the layer input)
+    ref, mag = reference(w.w_o, x_o)
+    errs["wo"] = store_error(ffins[:, r_e], ref, mag, xs[:, r_e])
+    moved["wo"] = (x_o, lambda xm: store_error(ffins[t][:, r_e], *reference(w.w_o, xm), xs[t][:, r_e]))
+    # w1 | w3: SiLU gate
+    g, sg = reference(w.w_1, x_13)
+    u, su = reference(w.w_3, x_13)
+    errs["w13"] = gate_error(gates[:, r_ff], g, sg, u, su)
+    moved["w13"] = (x_13, lambda xm: gate_error(gates[t][:, r_ff], *reference(w.w_1, xm), *reference(w.w_3, xm)))
+    # w2: + residual (ffin)
+    ref, mag = reference(w.w_2, x_2)
+    errs["w2"] = store_error(ys[:, r_e], ref, mag, ffins[:, r_e])
+    moved["w2"] = (x_2, lambda xm: store_error(ys[t][:, r_e], *reference(w.w_2, xm), ffins[t][:, r_e]))
+    worst = {mat: float(e.max()) for mat, e in errs.items()}
+    print("\n[fast-matmul] %s  max normalised error  %s" % (label, "  ".join("%s %.3g" % (m, worst[m]) for m in errs)))
+    bound = {mat: tau(w.FF if mat == "w2" else w.E) for mat in errs}
+    for mat, e in errs.items():
+        assert e.max() <= bound[mat], "%s %s: normalised error %.3g > TAU %.3g at %d outputs" % (
+            label, mat, e.max(), bound[mat], int((e > bound[mat]).sum()))
+    lost = {}
+    for mat, (xa, err_of) in moved.items():
+        xm = xa[t].copy()
+        blk = (xm.shape[1] // 32) // 3
+        xm[:, blk * 32:(blk + 1) * 32] = 0
+        outside = err_of(xm) > bound[mat]
+        lost[mat] = float(np.mean(outside))
+        each = "" if len(t) == 1 else " (%d tokens pooled; per token %.4f .. %.4f)" % (
+            len(t), outside.mean(axis=1).min(), outside.mean(axis=1).max())
+        print("[fast-matmul] %s  %s: a lost K block moves %.4f of the outputs outside the bound%s" % (
+            label, mat, lost[mat], each))
+        assert lost[mat] >= floor, "%s %s: a lost K block moves only %.3f of the outputs outside the bound" % (
+            label, mat, lost[mat])
+    return worst, lost

@@ -217,40 +217,20 @@ def test_cases_run_every_instantiation_over_several_ragged_token_tiles():
     assert want <= covered, (n_sm, sorted(want - covered))
 
 
-def _stacked_rows(path, names, per, sample):
-    """fp16 weights of `sample` rows of the matrices `names` stacked by rows (`per` rows each), as the packer stacks them."""
-    parts = []
-    for i, nm in enumerate(names):
-        sel = sample[(sample >= i * per) & (sample < (i + 1) * per)] - i * per
-        if len(sel):
-            parts.append(fast_ref.file_rows(path, "layers.0." + nm, sel)[0])
-    return np.concatenate(parts)
-
-
-def _outside_fraction(err_of_mutated, bound: float) -> float:
-    return float(np.mean(err_of_mutated > bound))
-
-
 @pytest.mark.parametrize("shape,wtype,ns", MATMUL_CASES, ids=_CASE_IDS)
 def test_each_fast_matmul_is_within_the_float64_bound(tmp_models, big_models, shape, wtype, ns):
     """Every token and a row sample (every row of the first and last tile, 1/8 of the others, every 8-row position) of
-    the four matmuls of one layer, against fast_ref's float64 sum of the same fp16 operands.  The fp16 activations the
-    kernels read are proven bit-exact through the w2 input left in xh.  Also checks, in numpy only, that the bound is
-    tight enough to see one lost 32-wide K block: zeroing one activation block of one token in the reference must put
-    >= 99 % (95 % at 30B / 65B) of that token's outputs outside it."""
+    the four matmuls of one layer, against fast_ref's float64 sum of the same fp16 operands (fast_ref.check_layer).
+    The fp16 activations the kernels read are proven bit-exact through the w2 input left in xh.  Also checks, in numpy
+    only, that the bound is tight enough to see one lost 32-wide K block: zeroing one activation block of one token in
+    the reference must put >= 99 % (95 % at 30B / 65B) of that token's outputs outside it."""
     from distributedllm_b200 import capi
     sh = ggjt.SHAPES[shape]
     E, FF = sh.n_embd, sh.n_ff
     path = tmp_models(shape, wtype, 0, 0) if shape.startswith("tiny") else big_models(shape, wtype)
     t0 = time.time()
-    r_qkv, r_e, r_ff = fast_ref.row_sample(3 * E, 128), fast_ref.row_sample(E, 128), fast_ref.row_sample(FF, 64)
-    w_qkv = _stacked_rows(path, ["attention.wq.weight", "attention.wk.weight", "attention.wv.weight"], E, r_qkv)
-    w_o = _stacked_rows(path, ["attention.wo.weight"], E, r_e)
-    w_1 = _stacked_rows(path, ["feed_forward.w1.weight"], FF, r_ff)
-    w_3 = _stacked_rows(path, ["feed_forward.w3.weight"], FF, r_ff)
-    w_2 = _stacked_rows(path, ["feed_forward.w2.weight"], E, r_e)
-    attn_norm = fast_ref.file_f32(path, "layers.0.attention_norm.weight")
-    ffn_norm = fast_ref.file_f32(path, "layers.0.ffn_norm.weight")
+    w = fast_ref.LayerWeights(path, 0, E, FF)
+    floor = LOST_BLOCK_LARGE if shape in ("30b", "65b") else LOST_BLOCK
     gpu = capi.Slice(path, 0, 1024)
     gpu.set_fast_prefill(True, 32)
     worst = {}
@@ -259,52 +239,10 @@ def test_each_fast_matmul_is_within_the_float64_bound(tmp_models, big_models, sh
             gpu.clear_context()
             x = np.random.default_rng([n, E]).standard_normal((n, E), dtype=np.float32)
             y = gpu.forward(x)
-            qkv = gpu.debug_read(0, n * 3 * E).reshape(n, 3 * E)
-            att = gpu.debug_read(1, n * E).reshape(n, E)
-            ffin = gpu.debug_read(2, n * E).reshape(n, E)
-            gate = gpu.debug_read(3, n * FF).reshape(n, FF)
-            xh = gpu.debug_read(9, n * FF // 2, np.uint32).view(np.uint16).reshape(n, FF)
-            # the activation restatement the bound relies on: k_prep_q8_f16 of w2's input, bit for bit
-            x_2 = fast_ref.prep(gate)
-            bad = int((xh != x_2.view(np.uint16)).sum())
-            assert bad == 0, "N=%d: xh differs from prep(gate) at %d of %d halves" % (n, bad, xh.size)
-            x_qkv, x_o, x_13 = fast_ref.prep(x, attn_norm), fast_ref.prep(att), fast_ref.prep(ffin, ffn_norm)
-            t, errs, moved = n // 2, {}, {}
-            # qkv: plain store
-            ref, mag = fast_ref.reference(w_qkv, x_qkv)
-            errs["qkv"] = fast_ref.store_error(qkv[:, r_qkv], ref, mag)
-            moved["qkv"] = (x_qkv, lambda xm, t=t: fast_ref.store_error(qkv[t:t + 1, r_qkv], *fast_ref.reference(w_qkv, xm)))
-            # wo: + residual (the layer input)
-            ref, mag = fast_ref.reference(w_o, x_o)
-            errs["wo"] = fast_ref.store_error(ffin[:, r_e], ref, mag, x[:, r_e])
-            moved["wo"] = (x_o, lambda xm, t=t: fast_ref.store_error(ffin[t:t + 1, r_e], *fast_ref.reference(w_o, xm), x[t:t + 1, r_e]))
-            # w1 | w3: SiLU gate
-            g, sg = fast_ref.reference(w_1, x_13)
-            u, su = fast_ref.reference(w_3, x_13)
-            errs["w13"] = fast_ref.gate_error(gate[:, r_ff], g, sg, u, su)
-            moved["w13"] = (x_13, lambda xm, t=t: fast_ref.gate_error(gate[t:t + 1, r_ff], *fast_ref.reference(w_1, xm),
-                                                                         *fast_ref.reference(w_3, xm)))
-            # w2: + residual (ffin)
-            ref, mag = fast_ref.reference(w_2, x_2)
-            errs["w2"] = fast_ref.store_error(y[:, r_e], ref, mag, ffin[:, r_e])
-            moved["w2"] = (x_2, lambda xm, t=t: fast_ref.store_error(y[t:t + 1, r_e], *fast_ref.reference(w_2, xm), ffin[t:t + 1, r_e]))
+            label = "%s %s N=%d" % (shape, ggjt.TYPE_NAME[wtype], n)
+            errs, _ = fast_ref.check_layer(w, x, fast_ref.read_layer(gpu, n, E, FF), y, tau, floor, label)
             for mat, e in errs.items():
-                worst[(n, mat)] = float(e.max())
-            print("\n[fast-matmul] %s %s N=%d  max normalised error  %s" % (
-                shape, ggjt.TYPE_NAME[wtype], n, "  ".join("%s %.3g" % (m, worst[(n, m)]) for m in errs)))
-            bound = {mat: tau(FF if mat == "w2" else E) for mat in errs}
-            for mat, e in errs.items():
-                assert e.max() <= bound[mat], "%s N=%d: normalised error %.3g > TAU %.3g at %d outputs" % (
-                    mat, n, e.max(), bound[mat], int((e > bound[mat]).sum()))
-            floor = LOST_BLOCK_LARGE if shape in ("30b", "65b") else LOST_BLOCK
-            for mat, (xa, err_of) in moved.items():
-                xm = xa[t:t + 1].copy()
-                blk = (xm.shape[1] // 32) // 3
-                xm[0, blk * 32:(blk + 1) * 32] = 0
-                frac = _outside_fraction(err_of(xm), bound[mat])
-                print("[fast-matmul] %s %s N=%d  %s: a lost K block moves %.4f of the outputs outside the bound" % (
-                    shape, ggjt.TYPE_NAME[wtype], n, mat, frac))
-                assert frac >= floor, "%s N=%d: a lost K block moves only %.3f of the outputs outside the bound" % (mat, n, frac)
+                worst[(n, mat)] = e
     finally:
         gpu.close()
     print("[fast-matmul] %s %s  largest %.3g (2^%.2f)  %.1f s" % (
