@@ -123,6 +123,8 @@ def lib() -> C.CDLL:
                            ("b200_stream_add_lp", [vp, ci, vp, ci, ci, vp, vp, ci, ci]),
                            ("b200_stream_read_lp", [vp, vp, vp, vp, vp, vp, ci, C.POINTER(ci)]),
                            ("b200_stream_fork", [vp, ci, ci, ci]),
+                           ("b200_stream_open_ex", [vp, ci, vp, ci, ci, ci, C.POINTER(vp)]),
+                           ("b200_stream_stats", [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(ci)]),
                            ("b200_session_copy", [vp, ci, vp, ci, ci]),
                            ("b200_session_state_size", [vp, ci, C.POINTER(C.c_size_t)]),
                            ("b200_session_save", [vp, ci, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
@@ -669,19 +671,26 @@ class Stream:
     with its prompt and budget; read() returns (session, id) pairs as the device draws them; a session leaves at its
     budget, at a stop id (delivered), on cancel() or at close().  Each session's ids equal generate_greedy /
     generate_sample for it alone.  While the stream is open its handles belong to it.  A context manager (close on exit)
-    and an iterator of (session, id) pairs, read one at a time, that ends when no session is left."""
+    and an iterator of (session, id) pairs, read one at a time, that ends when no session is left.  prefill_chunk C > 0
+    feeds each prompt in chunks of C ids beside the other sessions' decode rows (b200_stream_open_ex): a session's ids
+    then equal session_forward of each non-final chunk, then generate_* with the last chunk as its prompt."""
 
-    def __init__(self, slices, extra: Extra, max_rows: int = 0, lookahead: int = 0):
+    def __init__(self, slices, extra: Extra, max_rows: int = 0, lookahead: int = 0, prefill_chunk: int = 0):
         self._h = None
         slices = list(slices)
         if not slices:
             raise ValueError("a stream needs at least one slice")
         max_rows = _int("max_rows", max_rows, -2 ** 31, 2 ** 31 - 1)
         lookahead = _int("lookahead", lookahead, -2 ** 31, 2 ** 31 - 1)
+        prefill_chunk = _int("prefill_chunk", prefill_chunk, 0, 2 ** 31 - 1)
         self.n_vocab = extra.n_vocab
         handles = (C.c_void_p * len(slices))(*[s.handle for s in slices])
         h = C.c_void_p()
-        check(lib().b200_stream_open(handles, len(slices), extra.handle, max_rows, lookahead, C.byref(h)))
+        if prefill_chunk:
+            check(lib().b200_stream_open_ex(handles, len(slices), extra.handle, max_rows, lookahead, prefill_chunk,
+                                            C.byref(h)))
+        else:
+            check(lib().b200_stream_open(handles, len(slices), extra.handle, max_rows, lookahead, C.byref(h)))
         self._h = h
 
     def _handle(self) -> C.c_void_p:
@@ -756,6 +765,13 @@ class Stream:
         dst = _int("dst", dst, 0, 2 ** 31 - 1)
         n_keep = _int("n_keep", n_keep, 0, 2 ** 31 - 1)
         check(lib().b200_stream_fork(self._handle(), src, dst, n_keep))
+
+    def stats(self) -> dict:
+        """The load so far (b200_stream_stats): steps enqueued, the token rows they carried, and the rows of the largest
+        step."""
+        steps, rows, most = C.c_int64(), C.c_int64(), C.c_int()
+        check(lib().b200_stream_stats(self._handle(), C.byref(steps), C.byref(rows), C.byref(most)))
+        return {"steps": steps.value, "rows": rows.value, "most_rows": most.value}
 
     def close(self) -> None:
         if self._h:

@@ -2650,6 +2650,10 @@ __global__ void k_stream_tokens(const int32_t * spec, const int32_t * last, int 
     }
 }
 
+// A stream step with no draw (only non-final prompt chunks) publishes its completion here instead: cell 0 of its publish
+// ring, which the host set to INT32_MIN, so the region is not reused before the step's k_stream_tokens has read it.
+__global__ void k_stream_mark(int32_t * cell) { *(volatile int32_t *) cell = 0; }
+
 // Row k of out is row rows[k].gather of x: each session's last row of a mixed pass, packed for the lm_head.
 __global__ void k_gather_rows(const float * x, const StreamRow * rows, int E, float * out) {
     __shared__ int g;
@@ -4097,25 +4101,29 @@ struct b200_stream {
     std::vector<b200_slice *> slices; b200_extra * e = nullptr;
     std::unique_ptr<b200::StreamLoan> loan;
     int max_rows = 0, lookahead = 0, n_sess = 0, rows_cap = 0, nw = 0;   // rows_cap: sessions one step can hold
+    int chunk = 0;                        // prefill_chunk: prompt ids per segment (0: the whole prompt)
     // device: per-session sampler slots, penalty bitmaps [n_sess][nw], last ids
     b200::StreamSlot * d_slots = nullptr; uint32_t * d_pen = nullptr; int32_t * d_last = nullptr;
     // mapped pinned, one region per step in flight (lookahead + 1): token specs [max_rows], rows [rows_cap], ids [rows_cap]
     int32_t * h_spec = nullptr; b200::StreamRow * h_rows = nullptr; int32_t * h_ring = nullptr;
     b200::LpRecord * h_lp = nullptr;      // mapped pinned, [regions][rows_cap]: the logprob ring beside h_ring
     struct Sess {
-        int state = 0;                    // 0 not in the stream, 1 queued, 2 admitted (its prompt is enqueued)
+        int state = 0;                    // 0 not in the stream, 1 queued, 2 admitted (its first chunk is enqueued)
         unsigned gen = 0;                 // bumped when the session leaves: rows of steps enqueued before are dropped
         std::vector<int32_t> prompt, stops;
         std::vector<int> old;             // n_past on each slice when it was added
+        int fed = 0;                      // prompt ids enqueued; the session decodes once fed == prompt.size()
         int max_tokens = 0, enq = 0, delivered = 0;   // ids enqueued / returned by b200_stream_read
         int n_top = -1;                   // log-probabilities with n_top alternatives; -1: none
         long long first_draw = 0;
     };
     std::vector<Sess> sess;
-    std::deque<int> queue;                // added, not admitted yet, in add order
-    struct Step { int region; std::vector<std::pair<int, unsigned>> rows; size_t next = 0; };   // row k: (session, gen)
-    std::deque<Step> pending;             // enqueued steps whose ids have not all been read
-    long long n_steps = 0;
+    std::deque<int> queue;                // sessions whose prompt is not fully enqueued, in add order (the partly fed first)
+    // row k: (session, gen); a step without rows carries only non-final chunks and is done when k_stream_mark stores cell 0
+    struct Step { int region; std::vector<std::pair<int, unsigned>> rows; size_t next = 0; };
+    std::deque<Step> pending;             // enqueued steps whose ids have not all been read (or whose mark has not come)
+    long long n_steps = 0, n_rows = 0;    // steps enqueued and the token rows they carried (b200_stream_stats)
+    int most_rows = 0;                    // rows of the largest step
 };
 
 namespace b200 {
@@ -4124,10 +4132,10 @@ constexpr int kStreamLookahead = 4;
 
 // The session leaves the stream: n_past = old + n_prompt + delivered - 1 (old when nothing was delivered) on every slice,
 // host copy now and device copy in stream order, behind any step the device still runs for it.  Those steps' rows are at
-// or above the new n_past, so they are unreachable.
+// or above the new n_past, so they are unreachable; so are the rows of its prompt chunks when it leaves mid-prefill.
 static int stream_finish(b200_stream * st, int k) {
     b200_stream::Sess & z = st->sess[k];
-    if (z.state == 1) st->queue.erase(std::find(st->queue.begin(), st->queue.end(), k));
+    if (z.fed < (int) z.prompt.size()) st->queue.erase(std::find(st->queue.begin(), st->queue.end(), k));
     if (z.state == 2) {
         for (size_t i = 0; i < st->slices.size(); i++) {
             b200_slice * s = st->slices[i];
@@ -4141,21 +4149,24 @@ static int stream_finish(b200_stream * st, int k) {
     return 0;
 }
 
-// Schedules and enqueues one step (*did = false when no session has anything to run): every admitted session that still
-// owes ids decodes one row; queued prompts join in add order while the rows fit in max_rows.
+// Schedules and enqueues one step (*did = false when no session has anything to run): every session whose prompt is fully
+// fed and that still owes ids decodes one row; then the sessions with prompt ids left, in add order, each get their next
+// chunk (the whole prompt when chunk == 0) while the rows fit in max_rows; the first that does not fit ends the step.
+// Only a session whose last chunk is in the pass draws, from that chunk's last row.
 static int stream_step(b200_stream * st, bool * did) {
     *did = false;
     std::vector<int> ses, cnt;
     int N = 0;
     for (int k = 0; k < st->n_sess; k++) {
         const b200_stream::Sess & z = st->sess[k];
-        if (z.state == 2 && z.enq < z.max_tokens) { ses.push_back(k); cnt.push_back(1); N++; }
+        if (z.state == 2 && z.fed == (int) z.prompt.size() && z.enq < z.max_tokens) { ses.push_back(k); cnt.push_back(1); N++; }
     }
     const int n_decode = (int) ses.size();
-    while (!st->queue.empty() && N + (int) st->sess[st->queue.front()].prompt.size() <= st->max_rows) {
-        const int k = st->queue.front();
-        st->queue.pop_front();
-        ses.push_back(k); cnt.push_back((int) st->sess[k].prompt.size()); N += cnt.back();
+    for (int k : st->queue) {
+        const b200_stream::Sess & z = st->sess[k];
+        const int left = (int) z.prompt.size() - z.fed, c = st->chunk ? std::min(st->chunk, left) : left;
+        if (N + c > st->max_rows) break;
+        ses.push_back(k); cnt.push_back(c); N += c;
     }
     const int n = (int) ses.size();
     if (n == 0) return 0;
@@ -4165,15 +4176,21 @@ static int stream_step(b200_stream * st, bool * did) {
     volatile int32_t * ring = st->h_ring + (size_t) q * st->rows_cap;
     b200_stream::Step step{q, {}, 0};
     bool any_lp = false;
+    std::vector<int> drawing;                       // the sessions that draw, in row order of the pass
     for (int j = 0, r = 0; j < n; j++) {
         b200_stream::Sess & z = st->sess[ses[j]];
         if (j < n_decode) spec[r++] = ~ses[j];
-        else for (int32_t t : z.prompt) spec[r++] = t;
-        rows[j] = {z.first_draw + z.enq, ses[j], r - 1, z.n_top};
+        else for (int i = z.fed; i < z.fed + cnt[j]; i++) spec[r++] = z.prompt[i];
+        if (j >= n_decode && z.fed + cnt[j] < (int) z.prompt.size()) continue;   // a non-final chunk: no draw
+        const int d = (int) drawing.size();
+        rows[d] = {z.first_draw + z.enq, ses[j], r - 1, z.n_top};
         any_lp |= z.n_top >= 0;
-        ring[j] = INT32_MIN;
+        ring[d] = INT32_MIN;
         step.rows.emplace_back(ses[j], z.gen);
+        drawing.push_back(ses[j]);
     }
+    const int n_draw = (int) drawing.size();
+    if (n_draw == 0) ring[0] = INT32_MIN;
     b200_extra * e = st->e;
     b200_slice * x = &e->ctx;
     k_stream_tokens<<<(N + 255) / 256, 256, 0, x->stream>>>(spec, st->d_last, N, e->d_tok);
@@ -4190,28 +4207,38 @@ static int stream_step(b200_stream * st, bool * did) {
         if (rc) return rc;
         cur = s->d_out;
     }
-    if (N > n) {                                    // each session's last row, packed for the lm_head
-        k_gather_rows<<<dim3((e->E + 255) / 256, n), 256, 0, x->stream>>>(cur, rows, e->E, e->d_x);
+    int32_t * cells = st->h_ring + (size_t) q * st->rows_cap;
+    if (n_draw == 0) {
+        k_stream_mark<<<1, 1, 0, x->stream>>>(cells);
         B200_CUDA(cudaGetLastError());
         x->launches++;
-        cur = e->d_x;
-    }
-    if ((rc = extra_lmhead(e, cur, n))) return rc;
-    k_stream_draw<<<n, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, rows, st->d_slots, st->d_pen, st->d_last, st->h_ring + (size_t) q * st->rows_cap);
-    B200_CUDA(cudaGetLastError());
-    x->launches++;
-    if (any_lp) {                                   // publishes the rows that asked, after their records
-        k_stream_logprobs<<<n, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, rows, st->d_last, st->h_ring + (size_t) q * st->rows_cap,
-                                                     st->h_lp + (size_t) q * st->rows_cap);
+    } else {
+        if (N > n_draw) {                           // each drawing session's last row, packed for the lm_head
+            k_gather_rows<<<dim3((e->E + 255) / 256, n_draw), 256, 0, x->stream>>>(cur, rows, e->E, e->d_x);
+            B200_CUDA(cudaGetLastError());
+            x->launches++;
+            cur = e->d_x;
+        }
+        if ((rc = extra_lmhead(e, cur, n_draw))) return rc;
+        k_stream_draw<<<n_draw, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, rows, st->d_slots, st->d_pen, st->d_last, cells);
         B200_CUDA(cudaGetLastError());
         x->launches++;
+        if (any_lp) {                               // publishes the rows that asked, after their records
+            k_stream_logprobs<<<n_draw, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, rows, st->d_last, cells,
+                                                              st->h_lp + (size_t) q * st->rows_cap);
+            B200_CUDA(cudaGetLastError());
+            x->launches++;
+        }
     }
-    for (int j = 0; j < n; j++) {
+    for (int j = n_decode; j < n; j++) {
         b200_stream::Sess & z = st->sess[ses[j]];
-        z.state = 2; z.enq++;
+        z.state = 2; z.fed += cnt[j];
     }
+    st->queue.erase(std::remove_if(st->queue.begin(), st->queue.end(),
+                                   [st](int k) { return st->sess[k].fed == (int) st->sess[k].prompt.size(); }), st->queue.end());
+    for (int k : drawing) st->sess[k].enq++;
     st->pending.push_back(std::move(step));
-    st->n_steps++;
+    st->n_steps++; st->n_rows += N; st->most_rows = std::max(st->most_rows, N);
     *did = true;
     return 0;
 }
@@ -4243,7 +4270,10 @@ static int stream_read(b200_stream * st, int32_t * sessions, int32_t * ids, doub
     int got = 0;
     long long spins = 0;
     for (;;) {
-        while ((int) st->pending.size() <= st->lookahead) {
+        // a chunked stream tops up only while nothing is in hand: its chunk steps fill the device queue, enqueueing a step
+        // then waits for the device, and ids already published would wait with it (they would reach the caller in one
+        // burst).  A prefill_chunk 0 stream keeps its pacing: a session added between reads joins the same step as before.
+        while ((got == 0 || !st->chunk) && (int) st->pending.size() <= st->lookahead) {
             bool did = false;
             if (int rc = stream_step(st, &did)) return rc;
             if (!did) break;
@@ -4251,6 +4281,7 @@ static int stream_read(b200_stream * st, int32_t * sessions, int32_t * ids, doub
         if (got == cap || st->pending.empty()) break;
         b200_stream::Step & f = st->pending.front();
         const volatile int32_t * ring = st->h_ring + (size_t) f.region * st->rows_cap;
+        if (f.rows.empty() && ring[0] != INT32_MIN) { st->pending.pop_front(); spins = 0; continue; }   // a no-draw step ran
         while (f.next < f.rows.size() && got < cap) {
             const int32_t id = ring[f.next];
             if (id == INT32_MIN) break;
@@ -4274,7 +4305,7 @@ static int stream_read(b200_stream * st, int32_t * sessions, int32_t * ids, doub
             if (id < 0 || z.delivered == z.max_tokens || std::find(z.stops.begin(), z.stops.end(), id) != z.stops.end())
                 if (int rc = stream_finish(st, k)) return rc;
         }
-        if (f.next == f.rows.size()) { st->pending.pop_front(); spins = 0; continue; }
+        if (!f.rows.empty() && f.next == f.rows.size()) { st->pending.pop_front(); spins = 0; continue; }
         if (got > 0) break;
         // nothing published yet: poll; now and then make sure the device is still running the steps
         if (++spins % 4096 == 0) {
@@ -4295,6 +4326,11 @@ extern "C" {
 
 int b200_stream_open(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int max_rows, int lookahead,
                      b200_stream_t ** out) {
+    return b200_stream_open_ex(slices, n_slices, e, max_rows, lookahead, 0, out);
+}
+
+int b200_stream_open_ex(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int max_rows, int lookahead,
+                        int prefill_chunk, b200_stream_t ** out) {
     if (!slices || n_slices < 1 || !e || !out) return fail(B200_EINVAL, "b200_stream_open: null argument or no slices");
     *out = nullptr;
     int ndev = 0;
@@ -4306,12 +4342,14 @@ int b200_stream_open(b200_slice_t * const * slices, int n_slices, b200_extra_t *
     for (int i = 0; i < n_slices; i++) { n_ctx = std::min(n_ctx, slices[i]->n_ctx); n_sess = std::min(n_sess, slices[i]->n_sessions); }
     if (max_rows <= 0) max_rows = n_ctx;
     if (max_rows > n_ctx) return fail(B200_EINVAL, "max_rows %d exceeds the smallest n_ctx %d", max_rows, n_ctx);
+    if (prefill_chunk < 0 || prefill_chunk > max_rows)
+        return fail(B200_EINVAL, "prefill_chunk %d outside [0, max_rows %d]", prefill_chunk, max_rows);
     if (lookahead <= 0) lookahead = kStreamLookahead;
     if (lookahead > 1024) return fail(B200_EINVAL, "lookahead %d exceeds 1024", lookahead);
     B200_CUDA(cudaSetDevice(e->ctx.device));
     b200_stream * st = new b200_stream();
     st->slices.assign(slices, slices + n_slices); st->e = e;
-    st->max_rows = max_rows; st->lookahead = lookahead; st->n_sess = n_sess;
+    st->max_rows = max_rows; st->lookahead = lookahead; st->n_sess = n_sess; st->chunk = prefill_chunk;
     st->rows_cap = std::min(n_sess, max_rows); st->nw = (e->n_vocab + 31) / 32;
     st->sess.resize(n_sess);
     const size_t regions = (size_t) lookahead + 1;
@@ -4366,7 +4404,7 @@ int b200_stream_add_lp(b200_stream_t * st, int session, const int32_t * prompt, 
             return fail(B200_ECONTEXT, "context overflow: slice %zu session %d n_past %d + %d prompt tokens + %d steps > n_ctx %d",
                         i, session, s->past[session], n_prompt, max_tokens - 1, s->n_ctx);
     }
-    if (n_prompt > st->max_rows)
+    if (!st->chunk && n_prompt > st->max_rows)
         return fail(B200_EINVAL, "session %d: a prompt of %d ids exceeds max_rows %d (a prompt is never split)", session, n_prompt, st->max_rows);
     // the slot's sampler state, in stream order behind any step still running for an earlier stay of the session
     const double dt = sp ? sp->temperature + 1e-5 : 1.0;
@@ -4384,7 +4422,7 @@ int b200_stream_add_lp(b200_stream_t * st, int session, const int32_t * prompt, 
     z.stops.assign(stop_ids, stop_ids + n_stop);
     z.old.clear();
     for (const b200_slice * s : st->slices) z.old.push_back(s->past[session]);
-    z.max_tokens = max_tokens; z.enq = 0; z.delivered = 0; z.n_top = n_top;
+    z.fed = 0; z.max_tokens = max_tokens; z.enq = 0; z.delivered = 0; z.n_top = n_top;
     z.first_draw = sp ? sp->first_draw : 0;
     z.state = 1;
     st->queue.push_back(session);
@@ -4428,6 +4466,14 @@ int b200_stream_fork(b200_stream_t * st, int src, int dst, int n_keep) {
     // in stream order, behind every step still in flight for either session
     for (b200_slice * s : st->slices)
         if (int rc = kv_fork(s, src, &dst, 1, n_keep, st->e->ctx.stream)) return rc;
+    return 0;
+}
+
+int b200_stream_stats(b200_stream_t * st, int64_t * steps, int64_t * rows, int * most_rows) {
+    if (!steps || !rows || !most_rows) return fail(B200_EINVAL, "b200_stream_stats: null argument");
+    std::vector<std::unique_lock<std::mutex>> locks;
+    if (int rc = stream_lock(st, locks)) return rc;
+    *steps = st->n_steps; *rows = st->n_rows; *most_rows = st->most_rows;
     return 0;
 }
 

@@ -452,8 +452,9 @@ int b200_extra_logprobs(b200_extra_t * e, const float * logits, int n_rows, cons
  * A stream runs the generation loop of b200_generate_greedy / b200_generate_sample over a chain of slices on one GPU (the
  * same handle checks: contiguous layers, one device, no pipeline, the extra layers' n_embd), but open-ended:
  *   - b200_stream_add queues a session.  Its whole prompt is one segment of one mixed pass at the next step with room for
- *     it (never split: a segment's rows depend on its length); decode rows of other sessions may share that pass.  Every
- *     later step feeds the session the id it drew last.  sp NULL: greedy (the argmax of the raw logits, first maximum
+ *     it (on a stream opened with prefill_chunk 0: never split, a segment's rows depend on its length; see
+ *     b200_stream_open_ex for chunks); decode rows of other sessions may share that pass.  Every later step feeds the
+ *     session the id it drew last.  sp NULL: greedy (the argmax of the raw logits, first maximum
  *     wins); else sampled with sp's temperature, penalty, top_k and top_p, key seeds[0], history (history_counts[0] ids)
  *     and draw first_draw + j for its j-th id.  Greedy and sampled sessions with any settings share a stream.
  *   - A session ends after its max_tokens-th id, after the first id in stop_ids (delivered), or with id -1 when its logits
@@ -472,15 +473,40 @@ int b200_extra_logprobs(b200_extra_t * e, const float * logits, int n_rows, cons
  *     b200_extra_tokenize and b200_extra_token_text, which only read.  b200_stream_close gives them back.
  *   - One stream is driven from one thread.
  * b200_stream_open: max_rows = rows per step (<= the smallest n_ctx; <= 0: that n_ctx); lookahead <= 0: 4.  Sizes every
- *   buffer once.  B200_EINVAL for bad handles or sizes, B200_ENODEV without a device.
+ *   buffer once.  B200_EINVAL for bad handles or sizes, B200_ENODEV without a device.  b200_stream_open_ex with
+ *   prefill_chunk 0.
  * b200_stream_add: all-or-nothing.  B200_EINVAL: a session out of range or already in the stream, n_prompt < 1 or
- *   > max_rows, max_tokens < 1, an id outside [0, n_vocab) in prompt, history or stop_ids, bad sampling settings (as
- *   b200_generate_sample); B200_ECONTEXT: n_past + n_prompt + max_tokens - 1 > n_ctx on some slice.
+ *   > max_rows (prefill_chunk 0 only), max_tokens < 1, an id outside [0, n_vocab) in prompt, history or stop_ids, bad
+ *   sampling settings (as b200_generate_sample); B200_ECONTEXT: n_past + n_prompt + max_tokens - 1 > n_ctx on some
+ *   slice.
  * b200_stream_cancel: ends a queued or active session now (B200_EINVAL if it is neither); ids not yet read are dropped.
  * b200_stream_close: ends every session, waits for the device and frees the stream. */
 typedef struct b200_stream b200_stream_t;
 int b200_stream_open(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int max_rows, int lookahead,
                      b200_stream_t ** out);
+/* b200_stream_open whose prompts are fed in chunks of prefill_chunk = C ids, so a long prompt neither waits for a step
+ * with room for all of it nor stalls the decoding sessions for a whole prompt pass.  C = 0 is b200_stream_open, bit for
+ * bit and refusal for refusal.  B200_EINVAL for C < 0 or C > max_rows (after max_rows <= 0 became the smallest n_ctx).
+ * With C > 0:
+ *   - A prompt of n ids is fed as the chunks [0, C), [C, 2C), ... (the last one may be shorter), one segment each, at
+ *     most one per session per step.  The boundaries count from the prompt's first id and never depend on what else is
+ *     in the stream, so a session's rows are independent of its neighbours.  n_prompt > max_rows is accepted.
+ *   - Each step, on the host: every session whose prompt is fully fed and that still owes ids gets one decode row; then
+ *     the sessions with prompt ids left, in add order (so the partly fed ones before the queued ones), each get their
+ *     next chunk while the step stays within max_rows; the first chunk that does not fit ends the step (no overtaking).
+ *   - Only the session whose last chunk is in the step draws, from that chunk's last row; a non-final chunk takes no
+ *     draw index and its rows skip the lm_head.  A step of non-final chunks only draws nothing: it stores a completion
+ *     cell the host waits for before it reuses the step's buffers, and counts against lookahead as any step.
+ *     b200_stream_read still blocks until an id is available.  It tops up the lookahead only while it holds no id, so
+ *     the decode ids of steps beside a long prompt reach the caller step by step rather than in one burst.
+ *   - Contract: a session with prompt P yields the ids (and log-probabilities) of b200_session_forward of each
+ *     non-final chunk in order on every slice, then b200_generate_greedy / _sample / _lp with prompt = the last chunk,
+ *     the same settings and n_steps = delivered; whatever joined, ran beside it or left.  If every prompt has at most C
+ *     ids, the ids and positions are those of a prefill_chunk 0 stream.
+ *   - The position rule is unchanged, also for a session cancelled or closed mid-prefill (back at old: the chunks still
+ *     in flight write rows at or above old).  b200_stream_fork refuses a session still prefilling (it is active). */
+int b200_stream_open_ex(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, int max_rows, int lookahead,
+                        int prefill_chunk, b200_stream_t ** out);
 int b200_stream_add(b200_stream_t * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
                     const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop);
 int b200_stream_read(b200_stream_t * st, int32_t * sessions, int32_t * ids, int cap, int * n_out);
@@ -505,6 +531,9 @@ int b200_stream_cancel(b200_stream_t * st, int session);
  * session out of range, queued or active, src == dst, n_keep outside [0, n_past of src] on a slice, or slices whose
  * n_past of src differ. */
 int b200_stream_fork(b200_stream_t * st, int src, int dst, int n_keep);
+/* The stream's load so far: steps enqueued, the token rows they carried (decode rows and prompt ids), and the rows of
+ * the largest step (never more than max_rows). */
+int b200_stream_stats(b200_stream_t * st, int64_t * steps, int64_t * rows, int * most_rows);
 int b200_stream_close(b200_stream_t * st);
 /* llm.tokenize_prompt(path, prompt): BOS + sentencepiece-style merge (tensor_processor.cpp:1596-1714).
  * Returns the token count (may exceed cap; only cap are written) or a negative error. */
