@@ -55,6 +55,8 @@ def lib() -> C.CDLL:
         L.b200_version.restype = C.c_char_p
         L.b200_slice_load.argtypes = [C.c_char_p, ci, ci, C.POINTER(vp)]
         L.b200_slice_load_ex.argtypes = [C.c_char_p, ci, ci, ci, C.POINTER(vp)]
+        if hasattr(L, "b200_slice_load_lora"):
+            L.b200_slice_load_lora.argtypes = [C.c_char_p, ci, ci, ci, C.c_char_p, C.c_char_p, C.POINTER(vp)]
         L.b200_session_count.argtypes = [vp]
         L.b200_session_n_past.argtypes = [vp, ci]
         L.b200_session_clear.argtypes = [vp, ci]
@@ -150,9 +152,18 @@ def _ptr(a: np.ndarray) -> C.c_void_p:
 class Slice:
     """One slice resident on one GPU (mirrors llm.load_slice / propagate_forward / clear_context)."""
 
-    def __init__(self, path: str, device: int = 0, n_ctx: int = 0, n_sessions: int = 1):
+    def __init__(self, path: str, device: int = 0, n_ctx: int = 0, n_sessions: int = 1, lora: Optional[str] = None,
+                 lora_base: Optional[str] = None):
+        """lora: a `ggla` adapter merged into the weights at load (b200_slice_load_lora); lora_base: the F16 / F32 slice
+        file whose matrices the adapted ones are computed from (llama.cpp's --lora-base)."""
+        if lora_base is not None and lora is None:
+            raise ValueError("lora_base needs lora")
         self._h = C.c_void_p()
-        check(lib().b200_slice_load_ex(os.fsencode(path), device, n_ctx, n_sessions, C.byref(self._h)))
+        if lora is None:
+            check(lib().b200_slice_load_ex(os.fsencode(path), device, n_ctx, n_sessions, C.byref(self._h)))
+        else:
+            check(lib().b200_slice_load_lora(os.fsencode(path), device, n_ctx, n_sessions, os.fsencode(lora),
+                                             None if lora_base is None else os.fsencode(lora_base), C.byref(self._h)))
         self.info = self._info()
         self.n_sessions = n_sessions
 

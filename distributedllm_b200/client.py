@@ -271,12 +271,18 @@ class LocalPipeline:
     """All slices of a nodes_map on the GPUs of THIS box: slice i on device i, activations chained device to
     device (peer copy) -- the single-process equivalent of the NCCL pipeline bench.py runs with one rank per GPU."""
 
-    def __init__(self, slice_paths: Sequence[str], devices: Sequence[int] = None, n_ctx: int = 0, n_sessions: int = 1):
-        """n_sessions: KV-cache sessions per slice (perplexity_windows runs up to that many windows per pass)."""
+    def __init__(self, slice_paths: Sequence[str], devices: Sequence[int] = None, n_ctx: int = 0, n_sessions: int = 1,
+                 lora: str = None, lora_base: str = None):
+        """n_sessions: KV-cache sessions per slice (perplexity_windows runs up to that many windows per pass).
+        lora: one adapter file applied to every slice (capi.Slice); each slice takes the adapter's tensors for its own
+        layers.  lora_base: the F16 / F32 base as one slice file covering every slice's layers, or one file per slice."""
         from . import capi
         self.capi = capi
         devices = list(devices) if devices is not None else list(range(len(slice_paths)))
-        self.slices = [capi.Slice(p, d, n_ctx, n_sessions=n_sessions) for p, d in zip(slice_paths, devices)]
+        if isinstance(lora_base, str) or lora_base is None:
+            lora_base = [lora_base] * len(slice_paths)
+        self.slices = [capi.Slice(p, d, n_ctx, n_sessions=n_sessions, lora=lora, lora_base=b)
+                       for p, d, b in zip(slice_paths, devices, lora_base)]
         self.slices.sort(key=lambda s: s.info.first_layer)
         self._extra = None
 

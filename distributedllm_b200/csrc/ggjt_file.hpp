@@ -123,4 +123,68 @@ struct GgjtFile {
     const uint8_t * data(const GgjtTensor & t) const { return base + t.offset; }
 };
 
+// Read-only view of a LoRA adapter file (`ggla` v1), as convert-lora-to-ggml.py:49-74,111-131 writes it and
+// llama_apply_lora_from_file_internal (llama.cpp:2846-2960) reads it: magic, version, r, alpha (i32), then per tensor
+// n_dims, name_len, ftype (0 F32, 1 F16), ne[n_dims], the name, and the data at the next multiple of 32 bytes.
+// Only the layout is checked here; what the tensors may be is the loader's business.
+struct GglaFile {
+    int fd = -1;
+    const uint8_t * base = nullptr;
+    size_t size = 0;
+    int32_t r = 0, alpha = 0;
+    std::vector<GgjtTensor> tensors;    // file order; ne holds n_dims entries
+
+    explicit GglaFile(const std::string & path) {
+        try { parse(path); }
+        catch (...) { release(); throw; }
+    }
+    void release() {
+        if (base) { munmap((void *) base, size); base = nullptr; }
+        if (fd >= 0) { ::close(fd); fd = -1; }
+    }
+    void parse(const std::string & path) {
+        fd = ::open(path.c_str(), O_RDONLY);
+        if (fd < 0) throw std::runtime_error("cannot open adapter " + path);
+        struct stat st;
+        if (fstat(fd, &st) != 0 || st.st_size <= 0) throw std::runtime_error("cannot stat (or empty file) adapter " + path);
+        size = (size_t) st.st_size;
+        void * p = mmap(nullptr, size, PROT_READ, MAP_PRIVATE, fd, 0);
+        if (p == MAP_FAILED) throw std::runtime_error("mmap failed for adapter " + path);
+        base = (const uint8_t *) p;
+        size_t pos = 0;
+        auto u32 = [&](const char * what) -> uint32_t {
+            if (pos + 4 > size) throw std::runtime_error(std::string("adapter truncated in ") + what + ": " + path);
+            uint32_t v; memcpy(&v, base + pos, 4); pos += 4; return v;
+        };
+        const uint32_t magic = u32("the header"), version = u32("the header");
+        if (magic != 0x67676c61u) throw std::runtime_error("bad magic: not a ggla adapter file: " + path);
+        if (version != 1) throw std::runtime_error("unsupported ggla version " + std::to_string(version) + " (expected 1): " + path);
+        r = (int32_t) u32("the header"); alpha = (int32_t) u32("the header");
+        if (r <= 0) throw std::runtime_error("adapter rank r = " + std::to_string(r) + " is not positive: " + path);
+        while (pos < size) {
+            GgjtTensor t;
+            const uint32_t n_dims = u32("a tensor record"), name_len = u32("a tensor record");
+            t.type = u32("a tensor record");
+            if (n_dims < 1 || n_dims > 4 || name_len > 1024)
+                throw std::runtime_error("malformed tensor record at byte " + std::to_string(pos - 12) + " (n_dims " +
+                                         std::to_string(n_dims) + ", name length " + std::to_string(name_len) + ")");
+            size_t nelem = 1;
+            for (uint32_t d = 0; d < n_dims; d++) { t.ne.push_back(u32("a tensor record")); nelem *= t.ne.back(); }
+            if (pos + name_len > size) throw std::runtime_error("adapter truncated in a tensor name: " + path);
+            t.name.assign((const char *) base + pos, name_len); pos += name_len;
+            if (t.type != GT_F32 && t.type != GT_F16)
+                throw std::runtime_error("tensor '" + t.name + "' has ftype " + std::to_string(t.type) + " (0 = F32, 1 = F16)");
+            pos = (pos + 31) & ~(size_t) 31;
+            t.offset = pos; t.nbytes = nelem * (t.type == GT_F32 ? 4 : 2);
+            if (pos + t.nbytes > size) throw std::runtime_error("tensor '" + t.name + "' runs past the end of " + path);
+            pos += t.nbytes;
+            tensors.push_back(std::move(t));
+        }
+    }
+    ~GglaFile() { release(); }
+    GglaFile(const GglaFile &) = delete;
+    GglaFile & operator=(const GglaFile &) = delete;
+    const uint8_t * data(const GgjtTensor & t) const { return base + t.offset; }
+};
+
 }  // namespace b200

@@ -933,6 +933,145 @@ static int pass_locked(b200_slice * s, const int * sessions, const int * counts,
     return 0;
 }
 
+// Element j of one 32-weight block of a block-quantised type, as ggml's dequantize_row_* computes it (ggml.c:1523-1633,
+// built without contraction): q * d, and for Q4_1 / Q5_1 then + m (two roundings).
+__device__ __forceinline__ float deq32(const uint8_t * blk, int type, int j) {
+    const float d = h2f(*(const uint16_t *) blk);
+    if (type == kWT_Q8_0) return fmul((float)((const int8_t *)(blk + 2))[j], d);
+    if (type == kWT_Q4_0 || type == kWT_Q4_1) {
+        const int q = blk[(type == kWT_Q4_1 ? 4 : 2) + (j & 15)], x = j < 16 ? (q & 0x0F) : (q >> 4);
+        return type == kWT_Q4_1 ? fadd(fmul((float) x, d), h2f(*(const uint16_t *)(blk + 2))) : fmul((float)(x - 8), d);
+    }
+    const bool q51 = type == kWT_Q5_1;                    // Q5_0 / Q5_1
+    const uint8_t * qh = blk + (q51 ? 4 : 2);
+    const int q = qh[4 + (j & 15)];
+    const int x = (j < 16 ? (q & 0x0F) : (q >> 4)) | (((qh[j >> 3] >> (j & 7)) & 1) << 4);
+    return q51 ? fadd(fmul((float) x, d), h2f(*(const uint16_t *)(blk + 2))) : fmul((float)(x - 16), d);
+}
+
+// ---------------------------------------------------------------- LoRA merge (b200_slice_load_lora)
+// llama_apply_lora_from_file_internal (llama.cpp:3054-3100) per matrix W [rows][K] with loraA (ne [r, K]) and loraB
+// (ne [r, rows]):  BA = ggml_mul_mat(loraA, loraB), BA *= s when s = alpha / r != 1, then W += BA (or W = base + BA).
+// One CTA takes one 32-column block of W and kLoraRows rows; a warp takes one row at a time, lane l column l, so the
+// warp holds one whole quantisation block and requantises it with shuffles.
+constexpr int kLoraRows = 64, kLoraWarps = 8;
+
+struct LoraMergeArgs {
+    const uint8_t * in;    // W's blocks / F16 values, or the base tensor (F16 / F32) when btype >= 0
+    uint8_t * out;         // W-type output (== in when there is no base: each warp reads its block before it writes it)
+    const float * A, * B;  // [K][r], [rows][r]
+    int r, K, rows, wtype, btype;
+    float scale; int scaled;
+};
+
+// ggml_vec_dot_f32 (ggml.c:2286) in the AVX2 + FMA build: lane m of accumulator j sums x[i]*y[i] for i = 32c + 8j + m
+// with one FMA per element, GGML_F32x8_REDUCE (ggml.c:1895) folds the 32 partial sums in a fixed tree, and the last
+// r % 32 products are added one by one (multiply, then add).
+__device__ __forceinline__ float lora_dot(const float * As, const float * Bs, int r, int lane) {
+    const int np = r & ~31;
+    float sum = 0.f;
+    if (np) {
+        auto P = [&](int i) { float acc = 0.f; for (int c = 0; c < np; c += 32) acc = __fmaf_rn(As[(c + i) * 32 + lane], Bs[c + i], acc); return acc; };
+        auto V = [&](int m) { return fadd(fadd(P(m), P(16 + m)), fadd(P(8 + m), P(24 + m))); };   // (x0 + x2) + (x1 + x3)
+        sum = fadd(fadd(fadd(V(0), V(4)), fadd(V(1), V(5))), fadd(fadd(V(2), V(6)), fadd(V(3), V(7))));
+    }
+    for (int i = np; i < r; i++) sum = fadd(sum, fmul(As[i * 32 + lane], Bs[i]));
+    return sum;
+}
+
+// The warp's first lane (in lane order) whose v wins under `better`; ties keep the lower lane, as a forward scan with a
+// strict comparison does.
+template <typename F> __device__ __forceinline__ float warp_pick(float v, F better) {
+    int idx = threadIdx.x & 31;
+    for (int o = 16; o; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, v, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
+        if (better(ov, v) || (!better(v, ov) && oi < idx)) { v = ov; idx = oi; }
+    }
+    return v;
+}
+
+// Lane l holds element l of a block; writes it as one `type` block (ggml.c quantize_row_*_reference for the 4- and
+// 5-bit types, the AVX2 quantize_row_q8_0 for Q8_0: that is type_traits[type].from_float, ggml.c:1655-1690).
+__device__ void quant32(float x, int type, uint8_t * blk) {
+    const int lane = threadIdx.x & 31;
+    if (type == kWT_Q8_0) {                                  // ggml.c:1180-1240: id = 127 / amax, round half to even
+        float amax = fabsf(x);
+        for (int o = 16; o; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+        const float d = __fdiv_rn(amax, 127.f), id = amax != 0.f ? __fdiv_rn(127.f, amax) : 0.f;
+        const int q = __float2int_rn(fmul(x, id));
+        if (lane == 0) *(uint16_t *) blk = __half_as_ushort(__float2half_rn(d));
+        blk[2 + lane] = (uint8_t)(int8_t) q;
+        return;
+    }
+    int xi;
+    float d, m = 0.f;
+    if (type == kWT_Q4_0 || type == kWT_Q5_0) {              // max = the first v of largest |v| (0 when every v is 0)
+        const float half = type == kWT_Q4_0 ? 8.f : 16.f;
+        float mx = warp_pick(x, [](float a, float b) { return fabsf(a) > fabsf(b); });
+        if (fabsf(mx) == 0.f) mx = 0.f;
+        d = __fdiv_rn(mx, -half);
+        const float id = d != 0.f ? __fdiv_rn(1.f, d) : 0.f;
+        xi = min(type == kWT_Q4_0 ? 15 : 31, __float2int_rz(fadd(fmul(x, id), half + 0.5f)));
+    } else {                                                 // Q4_1 / Q5_1: the first minimum and maximum
+        const bool q41 = type == kWT_Q4_1;
+        m = warp_pick(x, [](float a, float b) { return a < b; });
+        const float mx = warp_pick(x, [](float a, float b) { return a > b; });
+        d = __fdiv_rn(fsub(mx, m), q41 ? 15.f : 31.f);
+        const float id = d != 0.f ? __fdiv_rn(1.f, d) : 0.f;
+        xi = __float2int_rz(fadd(fmul(fsub(x, m), id), 0.5f));
+        xi = q41 ? min(15, xi) : (xi & 0xFF);
+    }
+    const int hi = __shfl_down_sync(0xffffffffu, xi, 16);
+    const unsigned qh = __ballot_sync(0xffffffffu, (xi & 0x10) != 0);
+    const bool has_m = type == kWT_Q4_1 || type == kWT_Q5_1, five = type == kWT_Q5_0 || type == kWT_Q5_1;
+    uint8_t * qs = blk + 2 + (has_m ? 2 : 0) + (five ? 4 : 0);
+    if (lane < 16) qs[lane] = (uint8_t)((xi & 0x0F) | ((hi & 0x0F) << 4));
+    if (lane == 0) {
+        *(uint16_t *) blk = __half_as_ushort(__float2half_rn(d));
+        if (has_m) *(uint16_t *)(blk + 2) = __half_as_ushort(__float2half_rn(m));
+    }
+    if (five && lane < 4) blk[2 + (has_m ? 2 : 0) + lane] = (uint8_t)(qh >> (8 * lane));
+}
+
+__global__ void __launch_bounds__(kLoraWarps * 32) k_lora_merge(LoraMergeArgs a) {
+    extern __shared__ float lsm[];
+    float * As = lsm;                                        // [r][32]: the block's 32 columns of loraA, k-major
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, cb = blockIdx.x, c = cb * 32 + lane;
+    float * Bs = lsm + (size_t) a.r * 32 + (size_t) warp * a.r;
+    for (int i = threadIdx.x; i < 32 * a.r; i += blockDim.x) {
+        const int l = i / a.r, k = i - l * a.r;
+        As[k * 32 + l] = a.A[(size_t)(cb * 32 + l) * a.r + k];
+    }
+    __syncthreads();
+    const int nb = a.K / 32, row_end = min(a.rows, (int)(blockIdx.y + 1) * kLoraRows);
+    for (int j = blockIdx.y * kLoraRows + warp; j < row_end; j += kLoraWarps) {
+        for (int k = lane; k < a.r; k += 32) Bs[k] = a.B[(size_t) j * a.r + k];
+        __syncwarp();
+        float ba = lora_dot(As, Bs, a.r, lane);
+        if (a.scaled) ba = fmul(ba, a.scale);                // ggml_vec_scale_f32
+        const size_t e = (size_t) j * a.K + c;
+        float x;
+        if (a.btype == kWT_F16) {                            // ggml_add of an F16 base gives an F16 tensor
+            const uint16_t h = __half_as_ushort(__float2half_rn(fadd(h2f(((const uint16_t *) a.in)[e]), ba)));
+            if (a.wtype == kWT_F16) { ((uint16_t *) a.out)[e] = h; __syncwarp(); continue; }
+            x = h2f(h);
+        } else if (a.btype == 0) {                           // F32 base
+            x = fadd(((const float *) a.in)[e], ba);
+        } else if (a.wtype == kWT_F16) {                     // ggml_compute_forward_add_f16_f32 (ggml.c:8375)
+            x = fadd(h2f(((const uint16_t *) a.in)[e]), ba);
+        } else {                                             // ggml_compute_forward_add_q_f32 (ggml.c:8483)
+            x = fadd(deq32(a.in + ((size_t) j * nb + cb) * wt_traits(a.wtype).block_bytes, a.wtype, lane), ba);
+        }
+        __syncwarp();                                        // every lane has read the block before it is overwritten
+        if (a.wtype == kWT_F16) ((uint16_t *) a.out)[e] = __half_as_ushort(__float2half_rn(x));
+        else quant32(x, a.wtype, a.out + ((size_t) j * nb + cb) * wt_traits(a.wtype).block_bytes);
+        __syncwarp();
+    }
+}
+
+static size_t lora_smem(int r) { return (size_t)(32 + kLoraWarps) * r * sizeof(float); }
+
 // ---------------------------------------------------------------- loader
 // file (mmap, page cache) --reader thread--> pinned staging ring --DMA--> device scratch ring --k_repack--> packed HBM.
 // Three slots are in flight: while slot j is repacked on the GPU, slot j+1 is on the PCIe bus and the reader thread is
@@ -946,8 +1085,28 @@ struct LoadJob {
     PackedW * out = nullptr;      // kind 0
     uint16_t ** outf = nullptr; uint16_t * into = nullptr;   // kind 1
     uint8_t * raw_dst = nullptr;  // kind 2
-    size_t bytes() const { size_t n = 0; for (int i = 0; i < nsrc; i++) n += (src[i]->nbytes + 255) & ~(size_t) 255; return n; }
+    // LoRA (b200_slice_load_lora): source i is merged on the device before the repack.  With a base file, base[i] (F16
+    // or F32) is uploaded in its place and the merge writes source-type blocks into a region behind the uploaded ones.
+    const struct LoraPair * lora[3] = {nullptr, nullptr, nullptr};
+    const GgjtTensor * base[3] = {nullptr, nullptr, nullptr};
+    const GgjtFile * base_file = nullptr;
+    static size_t al(size_t n) { return (n + 255) & ~(size_t) 255; }
+    const GgjtTensor & up(int i) const { return base[i] ? *base[i] : *src[i]; }
+    size_t up_bytes() const { size_t n = 0; for (int i = 0; i < nsrc; i++) n += al(up(i).nbytes); return n; }
+    size_t bytes() const { size_t n = up_bytes(); for (int i = 0; i < nsrc; i++) if (base[i]) n += al(src[i]->nbytes); return n; }
+    // where source i's uploaded bytes, and its (merged) source-type bytes, sit in a slot
+    uint8_t * up_at(uint8_t * slot, int i) const { size_t o = 0; for (int k = 0; k < i; k++) o += al(up(k).nbytes); return slot + o; }
+    uint8_t * src_at(uint8_t * slot, int i) const {
+        if (!base[i]) return up_at(slot, i);
+        size_t o = up_bytes();
+        for (int k = 0; k < i; k++) if (base[k]) o += al(src[k]->nbytes);
+        return slot + o;
+    }
 };
+
+// One adapted matrix: loraA [K][r] and loraB [rows][r] in device memory
+struct LoraPair { const float * A = nullptr, * B = nullptr; int r = 0; };
+struct LoraMerge { float scale = 1.f; int scaled = 0; };
 
 struct LoadPipe {
     static constexpr int NB = 3;
@@ -964,7 +1123,7 @@ struct LoadPipe {
     }
 };
 
-static int run_load_jobs(b200_slice * s, const GgjtFile & f, std::vector<LoadJob> & jobs) {
+static int run_load_jobs(b200_slice * s, const GgjtFile & f, std::vector<LoadJob> & jobs, const LoraMerge & lm = LoraMerge()) {
     if (jobs.empty()) return 0;
     LoadPipe lp;
     for (const LoadJob & j : jobs) lp.slot_bytes = std::max(lp.slot_bytes, j.bytes());
@@ -990,22 +1149,24 @@ static int run_load_jobs(b200_slice * s, const GgjtFile & f, std::vector<LoadJob
             if (j >= LoadPipe::NB) cudaEventSynchronize(lp.ev[slot]);    // the slot's previous repack has read its scratch
             // pread straight into the pinned slot: page-cache copy without the per-4-KiB minor faults a private file
             // mapping costs; the job is cut in two so a second thread overlaps its copy
-            struct Piece { uint8_t * dst; size_t off, n; };
+            struct Piece { uint8_t * dst; size_t off, n; const GgjtFile * file; };
             std::vector<Piece> pieces;
             size_t off = 0;
             for (int i = 0; i < jobs[j].nsrc; i++) {
-                const GgjtTensor & t = *jobs[j].src[i];
+                const GgjtTensor & t = jobs[j].up(i);
+                const GgjtFile * tf = jobs[j].base[i] ? jobs[j].base_file : &f;
                 const size_t half = (t.nbytes / 2) & ~(size_t) 4095;
-                pieces.push_back({lp.pinned[slot] + off, t.offset, half});
-                pieces.push_back({lp.pinned[slot] + off + half, t.offset + half, t.nbytes - half});
+                pieces.push_back({lp.pinned[slot] + off, t.offset, half, tf});
+                pieces.push_back({lp.pinned[slot] + off + half, t.offset + half, t.nbytes - half, tf});
                 off += (t.nbytes + 255) & ~(size_t) 255;
             }
             auto pull = [&](int first) {
                 for (size_t k = first; k < pieces.size(); k += 2) {
                     size_t done = 0;
+                    const GgjtFile & pf = *pieces[k].file;
                     while (done < pieces[k].n) {
-                        const ssize_t got = pread(f.fd, pieces[k].dst + done, pieces[k].n - done, (off_t)(pieces[k].off + done));
-                        if (got <= 0) { memcpy(pieces[k].dst + done, f.base + pieces[k].off + done, pieces[k].n - done); break; }
+                        const ssize_t got = pread(pf.fd, pieces[k].dst + done, pieces[k].n - done, (off_t)(pieces[k].off + done));
+                        if (got <= 0) { memcpy(pieces[k].dst + done, pf.base + pieces[k].off + done, pieces[k].n - done); break; }
                         done += (size_t) got;
                     }
                 }
@@ -1022,8 +1183,19 @@ static int run_load_jobs(b200_slice * s, const GgjtFile & f, std::vector<LoadJob
         const int slot = (int)(j % LoadPipe::NB);
         LoadJob & job = jobs[j];
         { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return filled > j; }); }
-        cudaError_t e = cudaMemcpyAsync(lp.scratch[slot], lp.pinned[slot], job.bytes(), cudaMemcpyHostToDevice, s->stream);
+        cudaError_t e = cudaMemcpyAsync(lp.scratch[slot], lp.pinned[slot], job.up_bytes(), cudaMemcpyHostToDevice, s->stream);
         if (e != cudaSuccess) { rc = fail(B200_ECUDA, "weight upload failed: %s", cudaGetErrorString(e)); break; }
+        for (int i = 0; i < job.nsrc; i++) {
+            if (!job.lora[i]) continue;
+            const GgjtTensor & t = *job.src[i];
+            LoraMergeArgs la{};
+            la.in = job.up_at(lp.scratch[slot], i); la.out = job.src_at(lp.scratch[slot], i);
+            la.A = job.lora[i]->A; la.B = job.lora[i]->B; la.r = job.lora[i]->r;
+            la.K = (int) t.ne[0]; la.rows = (int) t.ne[1]; la.wtype = (int) t.type;
+            la.btype = job.base[i] ? (int) job.base[i]->type : -1;
+            la.scale = lm.scale; la.scaled = lm.scaled;
+            k_lora_merge<<<dim3(la.K / 32, (la.rows + kLoraRows - 1) / kLoraRows), kLoraWarps * 32, lora_smem(la.r), s->stream>>>(la);
+        }
         if (job.kind == 0) {
             const int wt = (int) job.src[0]->type;
             const bool kqt = wt_kquant(wt);             // k-quants: nb / nbq count 256-wide super-blocks
@@ -1036,8 +1208,7 @@ static int run_load_jobs(b200_slice * s, const GgjtFile & f, std::vector<LoadJob
             uint8_t * dst = nullptr;
             if ((rc = dev_alloc(s, &dst, (size_t) n_tiles * tile_bytes))) break;
             RepackArgs ra{};
-            size_t off = 0;
-            for (int i = 0; i < job.nsrc; i++) { ra.src[i] = lp.scratch[slot] + off; off += (job.src[i]->nbytes + 255) & ~(size_t) 255; }
+            for (int i = 0; i < job.nsrc; i++) ra.src[i] = job.src_at(lp.scratch[slot], i);
             ra.mode = job.mode; ra.wtype = wt; ra.rows_per_src = rows_per; ra.nb = nb; ra.nbq = nbq; ra.TR = TR; ra.n_tiles = n_tiles;
             ra.dst = dst;
             if (kqt) k_repack_kq<<<s->n_sm * 8, 256, 0, s->stream>>>(ra);
@@ -1051,7 +1222,7 @@ static int run_load_jobs(b200_slice * s, const GgjtFile & f, std::vector<LoadJob
             const int nchunk = K / 32, nc8 = (nchunk + 7) / 8;
             uint16_t * dst = job.into;
             if (!dst && (rc = dev_alloc(s, &dst, (size_t) rows * nc8 * 256 + 8))) break;
-            k_repack_f16<<<s->n_sm * 8, 256, 0, s->stream>>>((const uint16_t *) lp.scratch[slot], dst, dst /*no tail: K%32==0*/, rows, K);
+            k_repack_f16<<<s->n_sm * 8, 256, 0, s->stream>>>((const uint16_t *) job.src_at(lp.scratch[slot], 0), dst, dst /*no tail: K%32==0*/, rows, K);
             *job.outf = dst;
         } else {
             e = cudaMemcpyAsync(job.raw_dst, lp.scratch[slot], job.src[0]->nbytes, cudaMemcpyDeviceToDevice, s->stream);
@@ -1098,7 +1269,141 @@ static int build_tables(b200_slice * s) {
     return 0;
 }
 
-static int load_locked(b200_slice * s, const char * path) {
+// ---------------------------------------------------------------- LoRA adapter plan
+constexpr int kLoraMaxRank = 1024;      // loraA's 32 columns of one block stay in shared memory (160 KB at this rank)
+
+// What an adapter contributes to one load: the parsed files, loraA / loraB of every adapted matrix in device memory
+// (freed when the load ends), and the merge's scale.
+struct LoraState {
+    std::unique_ptr<GglaFile> ad;
+    std::unique_ptr<GgjtFile> base;
+    float * dev = nullptr;
+    std::vector<LoraPair> pairs;
+    LoraMerge merge;
+    ~LoraState() { if (dev) cudaFree(dev); }
+};
+
+// layers.N.attention.w{q,k,v,o}.weight or layers.N.feed_forward.w{1,2,3}.weight: its layer N
+static bool lora_target(const std::string & n, int * layer) {
+    if (n.compare(0, 7, "layers.") != 0) return false;
+    size_t q = 7;
+    while (q < n.size() && isdigit((unsigned char) n[q])) q++;
+    if (q == 7 || q - 7 > 6 || q >= n.size() || n[q] != '.') return false;
+    const std::string rest = n.substr(q + 1);
+    for (const char * m : {"attention.wq.weight", "attention.wk.weight", "attention.wv.weight", "attention.wo.weight",
+                           "feed_forward.w1.weight", "feed_forward.w2.weight", "feed_forward.w3.weight"})
+        if (rest == m) { *layer = atoi(n.c_str() + 7); return true; }
+    return false;
+}
+
+static std::string ne_str(const std::vector<uint32_t> & ne) {
+    std::string r = "[";
+    for (size_t i = 0; i < ne.size(); i++) r += (i ? ", " : "") + std::to_string(ne[i]);
+    return r + "]";
+}
+
+// Checks the adapter (and base) against slice file f, uploads loraA / loraB of every matrix of the slice it adapts, and
+// points the jobs' sources at them.  Nothing is repacked yet, so a refusal here leaves nothing behind but what the
+// failed load frees anyway.
+static int plan_lora(b200_slice * s, const GgjtFile & f, const char * lora_path, const char * base_path,
+                     std::vector<LoadJob> & jobs, LoraState & st) {
+    try { st.ad.reset(new GglaFile(lora_path)); }
+    catch (const std::exception & e) { return fail(B200_EFILE, "error loading LoRA adapter: %s", e.what()); }
+    if (base_path) {
+        try { st.base.reset(new GgjtFile(base_path, false)); }
+        catch (const std::exception & e) { return fail(B200_EFILE, "error loading LoRA base: %s", e.what()); }
+    }
+    const GglaFile & ad = *st.ad;
+    struct Pair { const GgjtTensor * a = nullptr, * b = nullptr, * w = nullptr, * bw = nullptr; };
+    std::map<std::string, Pair> by;                   // adapted matrices of this slice, by W's name
+    for (const GgjtTensor & t : ad.tensors) {
+        const size_t pos = t.name.rfind(".lora");
+        const std::string kind = pos == std::string::npos ? "" : t.name.substr(pos + 5);
+        if (kind != "A" && kind != "B")
+            return fail(B200_EFILE, "adapter tensor '%s' is not a LoRA tensor (its name must end in .loraA or .loraB)", t.name.c_str());
+        const std::string bn = t.name.substr(0, pos);
+        int layer = -1;
+        if (!lora_target(bn, &layer))
+            return fail(B200_EFILE, "adapter tensor '%s': '%s' is not a layer matrix (layers.N.attention.wq/wk/wv/wo.weight, "
+                                    "layers.N.feed_forward.w1/w2/w3.weight)", t.name.c_str(), bn.c_str());
+        if (t.ne.size() != 2)
+            return fail(B200_EFILE, "adapter tensor '%s' has %zu dimensions; LoRA tensors are 2-D", t.name.c_str(), t.ne.size());
+        if (t.type != GT_F32)
+            return fail(B200_EFILE, "adapter tensor '%s' is F16; LoRA tensors must be F32 (convert the checkpoint's loraA to float32)",
+                        t.name.c_str());
+        if (layer < s->first_layer || layer >= s->first_layer + s->L) continue;   // another slice's layer
+        Pair & p = by[bn];
+        const GgjtTensor *& slot = kind == "A" ? p.a : p.b;
+        if (slot) return fail(B200_EFILE, "adapter tensor '%s' appears twice", t.name.c_str());
+        slot = &t;
+    }
+    size_t floats = 0;
+    int max_r = 0;
+    for (auto & kv : by) {
+        Pair & p = kv.second;
+        const std::string & bn = kv.first;
+        if (!p.a || !p.b)
+            return fail(B200_EFILE, "adapter has %s.lora%s but no %s.lora%s for this slice's matrix (a lone A or B is refused)",
+                        bn.c_str(), p.a ? "A" : "B", bn.c_str(), p.a ? "B" : "A");
+        auto it = f.index.find(bn);
+        if (it == f.index.end()) return fail(B200_EFILE, "adapter tensor '%s.loraA': the slice has no %s", bn.c_str(), bn.c_str());
+        p.w = &f.tensors[it->second];
+        if (wt_kquant((int) p.w->type))
+            return fail(B200_EFILE, "adapter targets %s, a k-quant matrix (type %u): LoRA on Q4_K / Q6_K matrices is not supported",
+                        bn.c_str(), p.w->type);
+        const uint32_t r = p.a->ne[0];
+        if (p.b->ne[0] != r)
+            return fail(B200_EFILE, "adapter tensors %s.loraA (rank %u) and %s.loraB (rank %u) differ in rank", bn.c_str(), r,
+                        bn.c_str(), p.b->ne[0]);
+        if (p.a->ne[1] != p.w->ne[0] || p.b->ne[1] != p.w->ne[1])
+            return fail(B200_EFILE, "adapter tensors %s.loraA %s / .loraB %s do not fit %s %s (want [r, %u] and [r, %u])", bn.c_str(),
+                        ne_str(p.a->ne).c_str(), ne_str(p.b->ne).c_str(), bn.c_str(), ne_str(p.w->ne).c_str(), p.w->ne[0], p.w->ne[1]);
+        if (r == 0 || r > (uint32_t) kLoraMaxRank)
+            return fail(B200_EFILE, "adapter tensor %s.loraA has rank %u (supported: 1 .. %d)", bn.c_str(), r, kLoraMaxRank);
+        if (st.base) {
+            auto bt = st.base->index.find(bn);
+            if (bt == st.base->index.end()) return fail(B200_EFILE, "LoRA base lacks tensor '%s'", bn.c_str());
+            p.bw = &st.base->tensors[bt->second];
+            if (p.bw->ne != p.w->ne)
+                return fail(B200_EFILE, "LoRA base tensor '%s' has shape %s, the slice's has %s", bn.c_str(), ne_str(p.bw->ne).c_str(),
+                            ne_str(p.w->ne).c_str());
+            if (p.bw->type != GT_F16 && p.bw->type != GT_F32)
+                return fail(B200_EFILE, "LoRA base tensor '%s' has type %u; a base must be F16 (1) or F32 (0)", bn.c_str(), p.bw->type);
+        }
+        floats += (p.a->nbytes + p.b->nbytes) / 4;
+        max_r = std::max(max_r, (int) r);
+    }
+    if (by.empty()) return 0;                         // the adapter touches nothing here: a plain load
+    B200_CUDA(cudaMalloc((void **) &st.dev, floats * 4));
+    st.pairs.resize(by.size());
+    std::map<std::string, const LoraPair *> pair_of;
+    size_t off = 0, k = 0;
+    for (auto & kv : by) {
+        LoraPair & lp = st.pairs[k++];
+        lp.r = (int) kv.second.a->ne[0];
+        lp.A = st.dev + off;
+        B200_CUDA(cudaMemcpy(st.dev + off, ad.data(*kv.second.a), kv.second.a->nbytes, cudaMemcpyHostToDevice));
+        off += kv.second.a->nbytes / 4;
+        lp.B = st.dev + off;
+        B200_CUDA(cudaMemcpy(st.dev + off, ad.data(*kv.second.b), kv.second.b->nbytes, cudaMemcpyHostToDevice));
+        off += kv.second.b->nbytes / 4;
+        pair_of[kv.first] = &lp;
+    }
+    for (LoadJob & j : jobs)
+        for (int i = 0; i < j.nsrc; i++) {
+            auto it = pair_of.find(j.src[i]->name);
+            if (it == pair_of.end()) continue;
+            j.lora[i] = it->second;
+            if (st.base) { j.base[i] = by[it->first].bw; j.base_file = st.base.get(); }
+        }
+    st.merge.scale = (float) ad.alpha / (float) ad.r;    // llama.cpp:2878
+    st.merge.scaled = st.merge.scale != 1.0f;
+    if (lora_smem(max_r) > 48 * 1024)
+        B200_CUDA(cudaFuncSetAttribute(k_lora_merge, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) lora_smem(max_r)));
+    return 0;
+}
+
+static int load_locked(b200_slice * s, const char * path, const char * lora_path = nullptr, const char * base_path = nullptr) {
     const bool ltrace = env_int("B200_LOAD_TRACE", 0) != 0;
     auto tnow = [] { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
     const double t_begin = tnow(); double t_last = t_begin;
@@ -1126,6 +1431,7 @@ static int load_locked(b200_slice * s, const char * path) {
     int rc;
     std::vector<LoadJob> jobs;
     std::vector<float> norms;                       // all norm weights, one upload
+    LoraState lora;
     try {
         const std::string p0 = "layers." + std::to_string(s->first_layer);
         s->wtype = (int) f.get(p0 + ".attention.wq.weight", {E, E}).type;
@@ -1195,7 +1501,8 @@ static int load_locked(b200_slice * s, const char * path) {
             s->weight_bytes += (int64_t)(an.nbytes + fn.nbytes + wq.nbytes + wk.nbytes + wv.nbytes + wo.nbytes + w1.nbytes + w2.nbytes + w3.nbytes);
         }
         B200_CUDA(cudaMemcpyAsync(d_norms, norms.data(), norms.size() * 4, cudaMemcpyHostToDevice, s->stream));
-        if ((rc = run_load_jobs(s, f, jobs))) return rc;
+        if (lora_path && (rc = plan_lora(s, f, lora_path, base_path, jobs, lora))) return rc;
+        if ((rc = run_load_jobs(s, f, jobs, lora.merge))) return rc;
     } catch (const std::exception & e) {
         return fail(B200_EFILE, "error loading model: %s", e.what());
     }
@@ -1330,7 +1637,13 @@ int b200_slice_load(const char * path, int device, int n_ctx, b200_slice_t ** ou
 }
 
 int b200_slice_load_ex(const char * path, int device, int n_ctx, int n_sessions, b200_slice_t ** out) {
+    return b200_slice_load_lora(path, device, n_ctx, n_sessions, nullptr, nullptr, out);
+}
+
+int b200_slice_load_lora(const char * path, int device, int n_ctx, int n_sessions, const char * lora_path,
+                         const char * lora_base_path, b200_slice_t ** out) {
     if (!path || !out) return fail(B200_EINVAL, "b200_slice_load: null argument");
+    if (lora_base_path && !lora_path) return fail(B200_EINVAL, "b200_slice_load_lora: a LoRA base without an adapter");
     *out = nullptr;
     if (n_sessions < 1 || n_sessions > 4096) return fail(B200_EINVAL, "n_sessions %d outside [1, 4096]", n_sessions);
     int ndev = 0;
@@ -1358,7 +1671,7 @@ int b200_slice_load_ex(const char * path, int device, int n_ctx, int n_sessions,
     s->f16_ring = env_int("B200_F16_RING", 1) != 0;          // F16-weight slices: TMA-ring matmul for single-token steps
     cudaError_t e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
     if (e != cudaSuccess) { delete s; return fail(B200_ECUDA, "cudaStreamCreate failed: %s", cudaGetErrorString(e)); }
-    int rc = load_locked(s, path);
+    int rc = load_locked(s, path, lora_path, lora_base_path);
     if (rc) { destroy(s); return rc; }
     *out = s;
     return 0;
@@ -2162,30 +2475,10 @@ __global__ void k_embed_rows(const uint8_t * emb, int type, int E, const int32_t
     if (t < 0 || t >= n_vocab) { for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < E; i += gridDim.x * blockDim.x) dst[i] = 0.f; return; }
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < E; i += gridDim.x * blockDim.x) {
         float v;
-        if (type == kWT_Q4_0) {                      // dequantize_row_q4_0, ggml.c:1523-1541
-            const uint8_t * blk = emb + ((size_t) t * (E / 32) + i / 32) * 18;
-            const float d = h2f(*(const uint16_t *) blk);
-            const int j = i & 31, q = blk[2 + (j & 15)];
-            v = fmul((float)((j < 16 ? (q & 0x0F) : (q >> 4)) - 8), d);
-        } else if (type == kWT_Q4_1) {               // dequantize_row_q4_1, ggml.c:1543-1562: nibble * d, then + m (two roundings)
-            const uint8_t * blk = emb + ((size_t) t * (E / 32) + i / 32) * 20;
-            const float d = h2f(*(const uint16_t *) blk), m = h2f(*(const uint16_t *)(blk + 2));
-            const int j = i & 31, q = blk[4 + (j & 15)];
-            v = fadd(fmul((float)(j < 16 ? (q & 0x0F) : (q >> 4)), d), m);
-        } else if (type == kWT_Q5_0 || type == kWT_Q5_1) {  // dequantize_row_q5_0 / _q5_1, ggml.c:1564-1611
-            const bool q51 = type == kWT_Q5_1;
-            const uint8_t * blk = emb + ((size_t) t * (E / 32) + i / 32) * (q51 ? 24 : 22);
-            const float d = h2f(*(const uint16_t *) blk);
-            const uint8_t * qh = blk + (q51 ? 4 : 2);
-            const int j = i & 31, q = qh[4 + (j & 15)];
-            const int x = (j < 16 ? (q & 0x0F) : (q >> 4)) | (((qh[j >> 3] >> (j & 7)) & 1) << 4);
-            if (q51) v = fadd(fmul((float) x, d), h2f(*(const uint16_t *)(blk + 2)));   // x * d, then + m (two roundings)
-            else     v = fmul((float)(x - 16), d);
+        if (wt_block_quant(type)) {
+            v = deq32(emb + ((size_t) t * (E / 32) + i / 32) * wt_traits(type).block_bytes, type, i & 31);
         } else if (type == kWT_Q4_K) {
             v = dequant_q4k(emb + ((size_t) t * (E / 256) + i / 256) * 144, i & 255);
-        } else if (type == kWT_Q8_0) {
-            const uint8_t * blk = emb + ((size_t) t * (E / 32) + i / 32) * 34;
-            v = fmul((float)((const int8_t *)(blk + 2))[i & 31], h2f(*(const uint16_t *) blk));
         } else if (type == kWT_F16) v = h2f(((const uint16_t *) emb)[(size_t) t * E + i]);
         else v = ((const float *) emb)[(size_t) t * E + i];
         dst[i] = v;

@@ -917,3 +917,46 @@ def write_kquant_extra(path: str, shape: ModelShape, mix: str = "q4_K_M", seed: 
         _write_tensor(f, "norm.weight", T_F32, (e,), (1.0 + 0.1 * rng.standard_normal(e)).astype(np.float32).tobytes())
         w.write(f, "output.weight", T_Q6_K, e, v, rng)
         return f.tell()
+
+
+# --------------------------------------------------------------------------- LoRA adapters (ggla v1)
+MAGIC_GGLA = 0x67676C61
+
+
+def write_lora(path: str, r: int, alpha: int, tensors: Iterable[Tuple[str, np.ndarray]],
+               magic: int = MAGIC_GGLA, version: int = 1) -> None:
+    """A LoRA adapter file as convert-lora-to-ggml.py:49-74,111-131 writes it: magic, version, r, alpha (i32), then per
+    tensor n_dims, name length, ftype (0 F32 / 1 F16), ne (the numpy shape reversed), the name, and the data at the next
+    multiple of 32 bytes.  loraA of W [rows][K] is a [K][r] array (ne [r, K]), loraB a [rows][r] array (ne [r, rows])."""
+    with open(path, "wb") as f:
+        f.write(struct.pack("<IIii", magic, version, r, alpha))
+        for name, a in tensors:
+            a = np.ascontiguousarray(a)
+            ftype = {np.dtype(np.float32): 0, np.dtype(np.float16): 1}[a.dtype]
+            nm = name.encode("utf-8")
+            f.write(struct.pack("<iii", a.ndim, len(nm), ftype))
+            f.write(struct.pack("<%di" % a.ndim, *a.shape[::-1]))
+            f.write(nm)
+            f.write(b"\0" * ((-f.tell()) & 31))
+            f.write(a.tobytes())
+
+
+def read_lora(path: str) -> Tuple[int, int, Dict[str, np.ndarray]]:
+    """(r, alpha, {name: array}) of a `ggla` v1 file, tensors in file order with the numpy shapes write_lora took."""
+    with open(path, "rb") as f:
+        data = f.read()
+    magic, version, r, alpha = struct.unpack_from("<IIii", data, 0)
+    if magic != MAGIC_GGLA or version != 1:
+        raise ValueError("not a ggla v1 file: magic %08x version %d" % (magic, version))
+    pos, out = 16, {}
+    while pos < len(data):
+        n_dims, name_len, ftype = struct.unpack_from("<iii", data, pos)
+        ne = struct.unpack_from("<%di" % n_dims, data, pos + 12)
+        pos += 12 + 4 * n_dims
+        name = data[pos:pos + name_len].decode("utf-8")
+        pos = (pos + name_len + 31) & ~31
+        dt = np.float32 if ftype == 0 else np.float16
+        n = int(np.prod(ne))
+        out[name] = np.frombuffer(data, dt, n, pos).reshape(ne[::-1]).copy()
+        pos += n * np.dtype(dt).itemsize
+    return r, alpha, out

@@ -88,6 +88,26 @@ int b200_slice_forward_device(b200_slice_t * s, const float * d_in, int n_tokens
  * Session 0 is the context every b200_slice_* call above uses.  Each session behaves exactly like a reference slice
  * of its own: results are bit-identical to a private slice fed the same tokens. */
 int b200_slice_load_ex(const char * path, int device, int n_ctx, int n_sessions, b200_slice_t ** out);
+/* b200_slice_load_ex with a LoRA adapter merged into the weights on the device, bit-identical to llama.cpp's
+ * llama_model_apply_lora_from_file (main --lora / --lora-base, llama.cpp:2846-3124) followed by a plain load.
+ * lora_path is a `ggla` v1 file as convert-lora-to-ggml.py writes it.  For each layer matrix W of the slice
+ * (attention.wq/wk/wv/wo, feed_forward.w1/w2/w3) with W.loraA (ne [r, K]) and W.loraB (ne [r, rows]):
+ *   BA = loraA^T loraB in ggml_vec_dot_f32's AVX2 order, BA *= alpha / r unless that is 1, then
+ *   no base:   W = W + BA (quantised W: dequantise, add, requantise with type_traits[W].from_float -- for Q8_0 the AVX2
+ *              quantize_row_q8_0, round half to even; F16 W: fp16(fp32(w) + ba));
+ *   with base: W = quantise(base + BA), the base tensor (F16: an F16 sum; F32) read in W's place from lora_base_path, a
+ *              GGJT v3 slice file of the F16 / F32 model holding the slice's layers (slice_model cuts one).
+ * Weight families: Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, F16.  Adapter tensors of layers outside the slice are skipped, so one
+ * file serves every slice of a model; an adapter that touches nothing in the slice loads bit-identical to
+ * b200_slice_load_ex.  lora_base_path may be NULL.  Everything the adapter contributes is read and checked before the
+ * first matrix is repacked; on any error nothing stays loaded.
+ * B200_EINVAL: lora_base_path without lora_path.  B200_EFILE, naming the tensor: bad magic or version, a truncated file,
+ * r <= 0; a name without the .loraA / .loraB suffix or whose base is not a layer matrix; a lora tensor that is not 2-D or
+ * not F32 (llama.cpp asserts on F16); an A / B rank or shape mismatch; rank above 1024; a lone A or B for a matrix of the
+ * slice (llama.cpp skips it silently; this refuses it); a targeted Q4_K / Q6_K matrix; a base that lacks the tensor,
+ * has another shape, or is not F16 / F32. */
+int b200_slice_load_lora(const char * path, int device, int n_ctx, int n_sessions, const char * lora_path,
+                         const char * lora_base_path, b200_slice_t ** out);
 int b200_session_count(b200_slice_t * s);
 int b200_session_n_past(b200_slice_t * s, int session);                      /* -1 on a bad argument */
 int b200_session_clear(b200_slice_t * s, int session);                       /* session -1 = every session */
