@@ -85,6 +85,7 @@ def lib() -> C.CDLL:
         L.b200_slice_profile.argtypes = [vp, ci]
         L.b200_slice_profile_read.argtypes = [vp, vp, vp, ci]
         L.b200_debug_read.argtypes = [vp, ci, C.c_size_t, C.c_size_t, vp]
+        L.b200_debug_weights.argtypes = [vp, ci, ci, C.c_size_t, C.c_size_t, vp, C.POINTER(C.c_size_t)]
         L.b200_debug_trace_enable.argtypes = [vp, ci]
         L.b200_debug_skip_attention.argtypes = [vp, ci]
         L.b200_debug_trace_read.argtypes = [vp, vp, vp, vp, ci]
@@ -332,6 +333,16 @@ class Slice:
         out = np.zeros(count, np.uint32)
         check(lib().b200_debug_read(self._h, which, 0, count, _ptr(out)))
         return out.view(dtype)
+
+    def debug_weights(self, layer: int, which: int) -> np.ndarray:
+        """Packed device bytes of one matrix (b200_debug_weights): qkv / wo / w13 / w2 (0..3), or wq .. w3 (0..6) of an
+        F16 slice.  A test hook; nothing on a serving path calls it."""
+        n = C.c_size_t(0)
+        check(lib().b200_debug_weights(self._h, layer, which, 0, 0, None, C.byref(n)))
+        out = np.zeros(n.value, np.uint8)
+        if n.value:
+            check(lib().b200_debug_weights(self._h, layer, which, 0, n.value, _ptr(out), None))
+        return out
 
     def skip_attention(self, on: bool) -> None:
         check(lib().b200_debug_skip_attention(self._h, int(on)))

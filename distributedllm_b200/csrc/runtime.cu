@@ -2055,6 +2055,40 @@ int b200_debug_read(b200_slice_t * s, int which, size_t offset_words, size_t cou
     return 0;
 }
 
+/* Test hook: the packed bytes of one weight matrix of layer `layer` (0 = the slice's first).  Block-quantised and
+ * k-quant slices: which 0 qkv, 1 wo, 2 w13, 3 w2, 4 / 5 the second / third qkv run of a k-quant slice; F16 slices:
+ * which 0..6 = wq, wk, wv, wo, w1, w2, w3.  k_repack / k_repack_kq write every word of n_tiles * tile_bytes and
+ * k_repack_f16 every element of rows * nc8 * 256 (padding as zeros), so two loads of equal source bytes give equal
+ * bytes here.  *size (if not null) receives the matrix's byte count; `count` bytes from `offset` are copied to out. */
+int b200_debug_weights(b200_slice_t * s, int layer, int which, size_t offset, size_t count, void * out, size_t * size) {
+    if (!s) return fail(B200_EINVAL, "null handle");
+    B200_UNOWNED(s);
+    if (layer < 0 || layer >= s->L) return fail(B200_EINVAL, "layer %d outside [0, %d)", layer, s->L);
+    const LayerW & Lw = s->layers[layer];
+    const void * src = nullptr;
+    size_t n = 0;
+    if (s->wtype == kWT_F16) {
+        if (which < 0 || which > 6) return fail(B200_EINVAL, "bad F16 matrix id %d (0..6: wq wk wv wo w1 w2 w3)", which);
+        const uint16_t * f[7] = {Lw.f_q, Lw.f_k, Lw.f_v, Lw.f_o, Lw.f_1, Lw.f_2, Lw.f_3};
+        const int rows = which == 4 || which == 6 ? s->FF : s->E, K = which == 5 ? s->FF : s->E;
+        src = f[which];
+        n = (size_t) rows * ((K / 32 + 7) / 8) * 256 * 2;
+    } else {
+        if (which < 0 || which > 5) return fail(B200_EINVAL, "bad matrix id %d (0..5: qkv wo w13 w2 qkv_more[0..1])", which);
+        const PackedW * w[6] = {&Lw.qkv, &Lw.wo, &Lw.w13, &Lw.w2, &Lw.qkv_more[0], &Lw.qkv_more[1]};
+        src = w[which]->data;
+        n = src ? (size_t) w[which]->n_tiles * (size_t) w[which]->tile_bytes : 0;
+    }
+    if (size) *size = n;
+    if (!count) return 0;
+    if (!out) return fail(B200_EINVAL, "null argument");
+    if (offset > n || count > n - offset) return fail(B200_EINVAL, "bytes [%zu, %zu) outside the matrix's %zu", offset, offset + count, n);
+    B200_CUDA(cudaSetDevice(s->device));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    B200_CUDA(cudaMemcpy(out, (const uint8_t *) src + offset, count, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
 }  // extern "C"
 
 

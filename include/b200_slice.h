@@ -212,6 +212,12 @@ float * b200_slice_dev_out(b200_slice_t * s);
  * drop-in surface. */
 int b200_debug_read(b200_slice_t * s, int which, size_t offset_words, size_t count, void * out);
 
+/* Test hook: the packed device bytes of one weight matrix of the slice's layer `layer` (0 = its first).  Block-quantised
+ * and k-quant slices: which 0 qkv, 1 wo, 2 w13, 3 w2, 4 / 5 further qkv runs of a k-quant slice; F16 slices: 0..6 = wq,
+ * wk, wv, wo, w1, w2, w3.  Every byte of the range is written by the load, so two loads of equal source bytes return
+ * equal bytes.  *size (may be null) receives the byte count; count == 0 only queries it. */
+int b200_debug_weights(b200_slice_t * s, int layer, int which, size_t offset, size_t count, void * out, size_t * size);
+
 /* Measurement aid (bench.py roofline): while on, a decode step launches only its weight-matmul kernels. */
 int b200_debug_skip_attention(b200_slice_t * s, int on);
 

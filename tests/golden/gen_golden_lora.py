@@ -1,4 +1,4 @@
-"""Write tests/golden/ref_digests_lora.json: for every case of tests/lora_ref.cases(), the sha256 of each layer matrix
+"""Write tests/golden/ref_digests_lora.json: for every case of tests/lora_ref.cases() and .edges(), the sha256 of each layer matrix
 after llama.cpp's LoRA merge (oracle/_ref/lora_merge on the case's full model).  The CPU tests then check the host twin
 against these digests where oracle/_ref is absent.
 
@@ -35,7 +35,7 @@ def oracle_digests(c, d: str) -> dict:
 
 def main() -> None:
     res = {}
-    for c in lora_ref.cases():
+    for c in lora_ref.cases() + lora_ref.edges():
         with tempfile.TemporaryDirectory() as d:
             res[lora_ref.case_id(c)] = oracle_digests(c, d)
     with open(OUT, "w") as f:

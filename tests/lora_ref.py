@@ -188,9 +188,147 @@ def cases():
     return out
 
 
+EDGE_RANKS = (2, 33, 63, 64, 65, 96, 128, 307, 308, 1024)   # 307 / 308: the last rank under / first over 48 KB of smem
+MIXED_RANKS = {"attention.wq.weight": 8, "attention.wk.weight": 40, "attention.wv.weight": 16, "attention.wo.weight": 64,
+               "feed_forward.w1.weight": 40, "feed_forward.w2.weight": 16, "feed_forward.w3.weight": 8}
+MIXED_LAYER1 = {"attention.wq.weight": 64, "attention.wv.weight": 8}
+
+
+def edges():
+    """Cases beyond cases(): every rank path at a scale that is not a power of two, alpha of 1, 0 and negative, one
+    adapter whose tensors have ranks other than its header's r (kind "mixed"), and requantisation edges built into an
+    F32 base (kind "designed", see designed_blocks)."""
+    out = []
+    for fam in FAMILIES:
+        for r in EDGE_RANKS:
+            out.append((fam, r, 2 * r + 1, None))
+        for r in (8, 64):
+            for alpha in (1, r + 3, 3 * r, 0, -r, -(r + 3)):
+                if (fam, r, alpha, None) not in out and (fam, r, alpha, None) not in cases():
+                    out.append((fam, r, alpha, None))
+        out.append((fam, 16, 19, None, "mixed"))
+        out.append((fam, 2, -4, "f32", "designed"))
+    return out
+
+
 def case_id(c) -> str:
-    fam, r, alpha, base = c
-    return "%s_r%d_a%d_%s" % (fam, r, alpha, base or "nobase")
+    fam, r, alpha, base = c[:4]
+    kind = c[4] + "_" if len(c) > 4 else ""
+    return "%s_%sr%d_a%d_%s" % (fam, kind, r, alpha, base or "nobase")
+
+
+# ------------------------------------------------------------------ designed blocks
+# Layer 0's wq of a "designed" case: an F32 base and a rank-2 adapter of powers of two (scale -2), so BA is exact and
+# x = base + BA is exactly the target block.  Each target sits on one requantisation edge of its family.  Rows whose
+# loraB is zero get BA = -0 (+0 scaled by -2), so a -0 in the base stays -0 there.
+DESIGN_ROWS, DESIGN_K = 64, 64
+_ZERO_ROWS = (1, 2)                                     # loraB == 0: BA == -0
+
+
+def _fma_trunc_split(div: float):
+    """(mx, x): for a Q4_1 / Q5_1 block with m = 0 and max mx, a value x whose (x - m) * id + 0.5 truncates differently
+    when the multiply and add are one fma."""
+    for mx in np.arange(16.5, 40, 0.37, dtype=np.float64):
+        mx = F32(mx * (div / 15))
+        d = F32(mx / F32(div))
+        idv = F32(F32(1) / d)
+        x0 = F32(F32(0.5) / idv)
+        for k in range(-40, 41):
+            x = F32(x0 + F32(k) * np.spacing(x0))
+            two = np.trunc(F32(F32(x * idv) + F32(0.5)))
+            one = np.trunc(_fma(np.array([x]), np.array([idv]), np.array([F32(0.5)]))[0])
+            if two != one:
+                return mx, x
+    raise AssertionError("no fma split found")
+
+
+def designed_blocks(fam: str) -> Dict[str, np.ndarray]:
+    """Target blocks of family fam by edge name.  Names starting with "z_" need BA == -0 (a loraB-zero row)."""
+    wtype = FAMILIES[fam]
+    ar = np.arange(32, dtype=F32)
+    rng = np.random.default_rng(7)
+    small = lambda lo, hi: (np.round(rng.uniform(lo, hi, 32) * 4096) / 4096).astype(F32)   # noqa: E731
+    out = {"zero_from_base": np.zeros(32, F32)}         # base = -BA != 0
+    if wtype == ggjt.T_Q8_0:
+        h = ar - F32(15.5)
+        h[0] = 127                                      # amax 127: id 1, x * id half-way between integers
+        out["half"] = h
+        h2 = (ar - F32(15.5)) / F32(2)
+        h2[31] = F32(-63.5)                             # amax 63.5: id 2
+        out["half_id2"] = h2.astype(F32)
+    elif wtype in (ggjt.T_Q4_0, ggjt.T_Q5_0):
+        half = 8 if wtype == ggjt.T_Q4_0 else 16
+        t = small(-0.5, 0.5)
+        t[3], t[17] = 0.75, -0.75                       # +a first: max = +a
+        out["pm_tie"] = t
+        t = small(-0.5, 0.5)
+        t[2], t[30] = -0.75, 0.75                       # -a first: max = -a
+        out["mp_tie"] = t
+        t = (ar % (2 * half) - F32(half - 0.5)).astype(F32)
+        t[0] = -half                                    # max -half: d 1, id 1, x * id + half + 0.5 on integers
+        out["on_int"] = t
+    elif wtype in (ggjt.T_Q4_1, ggjt.T_Q5_1):
+        div = 15 if wtype == ggjt.T_Q4_1 else 31
+        out["min_eq_max"] = np.full(32, F32(0.3), F32)
+        t = (ar % div + F32(0.5)).astype(F32)
+        t[0], t[1] = 0, div                             # m 0, max div: d 1, id 1, (x - m) * id + 0.5 on integers
+        out["on_int"] = t
+        mx, x = _fma_trunc_split(div)
+        t = small(1.0, 2.0)
+        t[0], t[1], t[2] = 0, mx, x
+        out["fma_split"] = t
+        t = small(0.25, 0.5)
+        t[1], t[9] = 0, -0.0                            # minimum +0 first, -0 later
+        out["z_zero_tie"] = t
+        t = np.zeros(32, F32)
+        t[5::3] = -0.0                                  # all zero, lane 0 +0 and lane 31 -0: m and max are the first
+        t[31] = -0.0
+        out["z_all_zero_signs"] = t
+    else:                                               # F16
+        u = F32(2.0 ** -10)                             # ulp of fp16 at 1
+        out["ties"] = (np.where(ar < 16, 1, -1) * (1 + (ar % 16) * u + u / 2)).astype(F32)
+        s = F32(2.0 ** -24)                             # smallest fp16 subnormal
+        t = ((ar - 16) * s / 2).astype(F32)             # subnormals, half-way subnormals, +-2^-25 (ties with zero)
+        out["subnormal"] = t
+        t = np.zeros(32, F32)
+        t[1::2] = -0.0
+        out["z_signed_zero"] = t
+    return out
+
+
+def _design_ab():
+    """loraA [K][2], loraB [rows][2] of the designed matrix: powers of two, loraB zero on _ZERO_ROWS."""
+    A = np.zeros((DESIGN_K, 2), F32)
+    A[:, 0] = 2.0 ** -3
+    A[:, 1] = np.where(np.arange(DESIGN_K) % 2, 2.0 ** -6, -2.0 ** -6)
+    B = np.zeros((DESIGN_ROWS, 2), F32)
+    B[:, 0] = np.array([1, -1, 0.5, -0.5], F32)[np.arange(DESIGN_ROWS) % 4] * F32(2.0 ** -8)
+    B[1::2, 1] = B[1::2, 0]
+    B[list(_ZERO_ROWS)] = 0
+    return A, B
+
+
+def designed_matrix(fam: str):
+    """(base [64][64] F32, loraA, loraB, targets, placement {edge: (row, block)}) of a designed case."""
+    A, B = _design_ab()
+    d = ba(A, B, -4, 2)
+    rng = np.random.default_rng(8)
+    base = (rng.standard_normal((DESIGN_ROWS, DESIGN_K), dtype=F32) * F32(0.125)).astype(F32)
+    target = (base + d).astype(F32)
+    place = {}
+    rows = iter(r for r in range(DESIGN_ROWS) if r not in _ZERO_ROWS)
+    zrows = iter(_ZERO_ROWS)
+    for name, blk in designed_blocks(fam).items():
+        j = next(zrows) if name.startswith("z_") else next(rows)
+        dj = d[j, 0:32]
+        target[j, 0:32] = blk
+        base[j, 0:32] = np.where(dj == 0, blk, (blk.astype(np.float64) - dj).astype(F32))
+        place[name] = (j, 0)
+    for name, (j, b) in place.items():                  # every designed x is base + BA with no rounding
+        cols = slice(32 * b, 32 * b + 32)
+        assert np.array_equal(base[j, cols].astype(np.float64) + d[j, cols], target[j, cols].astype(np.float64)), name
+    assert np.array_equal((base + d).astype(F32).view(np.uint32), target.view(np.uint32))
+    return base, A, B, target, place
 
 
 def _matrix(rng, rows: int, k: int) -> np.ndarray:
@@ -207,10 +345,11 @@ def _matrix(rng, rows: int, k: int) -> np.ndarray:
 
 def write_case(d: str, c, seed: int = 0):
     """Full model, adapter (and base model) of case c under directory d: (model, adapter, base or None)."""
-    fam, r, alpha, base = c
+    fam, r, alpha, base = c[:4]
+    kind = c[4] if len(c) > 4 else None
     wtype = FAMILIES[fam]
     sh = SHAPE
-    rng = np.random.default_rng([seed, r, alpha, wtype])
+    rng = np.random.default_rng([seed, r, alpha % (1 << 32), wtype] + ([len(kind)] if kind else []))
     e, ff = sh.n_embd, sh.n_ff
     dims = {"attention.wq.weight": (e, e), "attention.wk.weight": (e, e), "attention.wv.weight": (e, e),
             "attention.wo.weight": (e, e), "feed_forward.w1.weight": (ff, e), "feed_forward.w2.weight": (e, ff),
@@ -219,6 +358,12 @@ def write_case(d: str, c, seed: int = 0):
     for layer in range(sh.n_layer):
         for nm in MATS:
             mats["layers.%d.%s" % (layer, nm)] = _matrix(rng, *dims[nm])
+    designed = {}
+    if kind == "designed":
+        wq = "layers.0.attention.wq.weight"
+        assert dims["attention.wq.weight"] == (DESIGN_ROWS, DESIGN_K)
+        mats[wq], dA, dB = designed_matrix(fam)[:3]
+        designed[wq] = (dA, dB)
     vocab = ggjt.default_vocab(sh.n_vocab)
 
     def model(wt):
@@ -250,9 +395,14 @@ def write_case(d: str, c, seed: int = 0):
         if layer == 1 and not name.endswith(("wq.weight", "wv.weight")):
             continue                                    # layer 1: alpaca-lora's targets only
         rows, k = w.shape
-        A = (rng.standard_normal((k, r), dtype=F32) * F32(0.05)).astype(F32)
-        B = (rng.standard_normal((rows, r), dtype=F32) * F32(0.05)).astype(F32)
-        B[:3] = 0                                       # the zero and tie rows keep their values (BA == +0)
+        rt = r
+        if kind == "mixed":                             # tensor ranks other than the header's r
+            rt = (MIXED_RANKS if layer == 0 else MIXED_LAYER1)[name.split(".", 2)[2]]
+        A = (rng.standard_normal((k, rt), dtype=F32) * F32(0.05)).astype(F32)
+        B = (rng.standard_normal((rows, rt), dtype=F32) * F32(0.05)).astype(F32)
+        B[:3] = 0                                       # the zero and tie rows keep their values (BA == +-0)
+        if name in designed:
+            A, B = designed[name]
         tens += [(name + ".loraA", A), (name + ".loraB", B)]
     apath = os.path.join(d, "adapter.bin")
     ggjt.write_lora(apath, r, alpha, tens)

@@ -246,6 +246,7 @@ def test_refusals_name_the_tensor_and_leave_nothing(tmp_path):
     add("3-D", wq + ".loraA", [(wq + ".loraA", np.zeros((2, E, 4), np.float32))])
     add("F16", wq + ".loraA", [(wq + ".loraA", A(E).astype(np.float16)), (wq + ".loraB", A(E))])
     add("rank mismatch", wq, [(wq + ".loraA", A(E, 8)), (wq + ".loraB", A(E, 4))])
+    add("rank 1025", wq, [(wq + ".loraA", A(E, 1025)), (wq + ".loraB", A(E, 1025))], r=1025)
     add("shape", wq, [(wq + ".loraA", A(E + 32)), (wq + ".loraB", A(E))])
     add("shape", "layers.0.feed_forward.w2.weight", [("layers.0.feed_forward.w2.weight.loraA", A(E)),
                                                       ("layers.0.feed_forward.w2.weight.loraB", A(E))])

@@ -16,7 +16,8 @@ from distributedllm_b200 import capi, ggjt
 HERE = os.path.dirname(os.path.abspath(__file__))
 TOOL = os.path.join(os.path.dirname(HERE), "oracle", "_ref", "lora_merge")
 GOLD = json.load(open(os.path.join(HERE, "golden", "ref_digests_lora.json")))
-CASES = lora_ref.cases()
+CASES = lora_ref.cases() + lora_ref.edges()
+TOOL_CASES = [c for c in CASES if c[1] in (1, 32, 40) or c in lora_ref.edges()]
 
 
 @pytest.mark.parametrize("case", CASES, ids=[lora_ref.case_id(c) for c in CASES])
@@ -30,8 +31,7 @@ def test_twin_matches_golden_digests(case, tmp_path):
 
 
 @pytest.mark.skipif(not os.path.isfile(TOOL), reason="oracle/_ref/lora_merge not built")
-@pytest.mark.parametrize("case", [c for c in CASES if c[1] in (1, 32, 40)],
-                         ids=[lora_ref.case_id(c) for c in CASES if c[1] in (1, 32, 40)])
+@pytest.mark.parametrize("case", TOOL_CASES, ids=[lora_ref.case_id(c) for c in TOOL_CASES])
 def test_twin_matches_llama_cpp_byte_for_byte(case, tmp_path):
     m, a, b = lora_ref.write_case(str(tmp_path), case)
     ref, twin = str(tmp_path / "ref.bin"), str(tmp_path / "twin.bin")
@@ -48,6 +48,126 @@ def test_cases_hit_ties_and_zero_blocks(tmp_path):
     q = q8[0, 2:].view(np.int8)
     assert q[0] == 127 and q[1] == -30 and q[2] == -30     # -30.5 and -29.5: half to even (roundf gives -31, -30)
     assert lora_ref.quantize(x[0:1], ggjt.T_Q4_0)[:2] == np.float16(-0.0).tobytes()
+
+
+def test_edge_cases_cover_the_rank_paths_and_scales():
+    e = lora_ref.edges()
+    for fam in lora_ref.FAMILIES:
+        ranks = {c[1] for c in e if c[0] == fam and len(c) == 4}
+        assert set(lora_ref.EDGE_RANKS) <= ranks
+        for c in e:                                     # the rank sweep's scales are not powers of two
+            if c[0] == fam and c[1] in lora_ref.EDGE_RANKS and c[2] == 2 * c[1] + 1:
+                s = np.float32(c[2]) / np.float32(c[1])
+                assert np.frexp(s)[0] != 0.5
+        for r in (8, 64):
+            alphas = {c[2] for c in lora_ref.cases() + e if c[0] == fam and c[1] == r and c[3] is None and len(c) == 4}
+            assert {1, r + 3, 3 * r, 0, -r, -(r + 3)} <= alphas
+    # one job of stacked sources with two ranks (wq | wk | wv and w1 | w3), none equal to the header's r = 16 there
+    assert lora_ref.MIXED_RANKS["attention.wq.weight"] != lora_ref.MIXED_RANKS["attention.wk.weight"]
+    assert lora_ref.MIXED_RANKS["feed_forward.w1.weight"] != lora_ref.MIXED_RANKS["feed_forward.w3.weight"]
+    assert {8, 16, 40, 64} == set(lora_ref.MIXED_RANKS.values())
+
+
+def _signs(x):
+    return np.signbit(np.asarray(x, np.float32))
+
+
+@pytest.mark.parametrize("fam", list(lora_ref.FAMILIES))
+def test_designed_blocks_reach_their_edges(fam):
+    """Each designed block of the "designed" cases sits on its edge once base + BA is formed: a check of the values the
+    merge quantises, so a block that misses its edge fails here rather than checking nothing."""
+    F = np.float32
+    base, A, B, target, place = lora_ref.designed_matrix(fam)
+    d = lora_ref.ba(A, B, -4, 2)
+    assert np.array_equal(A, np.exp2(np.round(np.log2(np.abs(A)))) * np.sign(A))      # powers of two
+    nz = B != 0
+    assert np.array_equal(B[nz], (np.exp2(np.round(np.log2(np.abs(B[nz])))) * np.sign(B[nz])).astype(F))
+    blk = {n: target[j, 32 * b:32 * b + 32] for n, (j, b) in place.items()}
+    bas = {n: base[j, 32 * b:32 * b + 32] for n, (j, b) in place.items()}
+    ba_ = {n: d[j, 32 * b:32 * b + 32] for n, (j, b) in place.items()}
+    for n in blk:
+        assert np.array_equal((bas[n] + ba_[n]).astype(F).view(np.uint32), blk[n].view(np.uint32)), n
+        if n.startswith("z_"):
+            assert np.all((ba_[n] == 0) & _signs(ba_[n])), n                       # BA == -0 (negative scale)
+        else:
+            assert np.all(ba_[n] != 0), n                                          # the edge is made by adding BA
+    z = blk["zero_from_base"]
+    assert np.all(z == 0) and not _signs(z).any() and np.all(bas["zero_from_base"] != 0)
+    wtype = lora_ref.FAMILIES[fam]
+    if wtype == ggjt.T_Q8_0:
+        for n in ("half", "half_id2"):
+            x = blk[n]
+            amax = np.abs(x).max()
+            p = (x * (F(127) / amax)).astype(F)
+            ties = (p - np.floor(p)) == 0.5
+            away = np.sign(p) * np.floor(np.abs(p) + 0.5)
+            assert ties.sum() >= 16 and (np.rint(p) != away).sum() >= 8, n       # half to even differs from roundf
+    elif wtype in (ggjt.T_Q4_0, ggjt.T_Q5_0):
+        half = F(8 if wtype == ggjt.T_Q4_0 else 16)
+        for n, first in (("pm_tie", 1), ("mp_tie", -1)):
+            a = np.abs(blk[n])
+            top = np.flatnonzero(a == a.max())
+            assert len(top) == 2 and np.sign(blk[n][top[0]]) == first and np.sign(blk[n][top[1]]) == -first, n
+        x = blk["on_int"]
+        mx = x[np.argmax(np.abs(x))]
+        idv = F(1) / F(mx / -half)
+        v = ((x * idv).astype(F) + (half + F(0.5))).astype(F)
+        assert (v == np.trunc(v)).sum() == 31 and mx == -half                       # all but the max itself
+    elif wtype in (ggjt.T_Q4_1, ggjt.T_Q5_1):
+        div = F(15 if wtype == ggjt.T_Q4_1 else 31)
+        x = blk["min_eq_max"]
+        assert x.min() == x.max() != 0
+        x = blk["on_int"]
+        idv = F(1) / F((x.max() - x.min()) / div)
+        v = (((x - x.min()).astype(F) * idv).astype(F) + F(0.5)).astype(F)
+        assert (v == np.trunc(v)).sum() == 30                                       # all but min and max
+        x = blk["fma_split"]
+        m, idv = x.min(), F(1) / F((x.max() - x.min()) / div)
+        two = np.trunc((((x - m).astype(F) * idv).astype(F) + F(0.5)).astype(F))
+        one = np.trunc(lora_ref._fma((x - m).astype(F), np.full(32, idv, F), np.full(32, F(0.5), F)))
+        assert (two != one).sum() == 1                                              # one product rounded, or not
+        x = blk["z_zero_tie"]                                                       # minimum: +0 first, -0 later
+        zi = np.flatnonzero(x == 0)
+        assert x.min() == 0 and len(zi) == 2 and not _signs(x[zi[0]]) and _signs(x[zi[1]])
+        x = blk["z_all_zero_signs"]
+        assert np.all(x == 0) and not _signs(x[0]) and _signs(x[31])
+    else:
+        x = blk["ties"]
+        h = x.astype(np.float16)
+        toward = np.where(h.astype(F) > x, np.float16(-np.inf), np.float16(np.inf)).astype(np.float16)
+        other = np.nextafter(h, toward)                                             # the fp16 neighbour across x
+        assert np.array_equal(h.astype(np.float64) + other.astype(np.float64), 2 * x.astype(np.float64))   # half-way
+        up = np.abs(h.astype(F)) > np.abs(x)                                        # half to even, away from zero
+        assert up.sum() >= 8 and (~up).sum() >= 8
+        x = blk["subnormal"]
+        h = x.astype(np.float16)
+        sub = (h != 0) & (np.abs(h) < np.float16(2.0 ** -14))
+        assert sub.sum() >= 20
+        assert (h == 0).any() and _signs(h.astype(F)[x < 0]).all()                  # -2^-25 rounds to -0
+        x = blk["z_signed_zero"]
+        assert np.all(x == 0) and _signs(x).sum() == 16
+
+
+def test_designed_cases_merge_their_edge_blocks():
+    """The twin's merged wq of a designed case is the quantised target: BA is exact, so the file holds exactly the
+    designed blocks' requantisation."""
+    for fam, wtype in lora_ref.FAMILIES.items():
+        base, A, B, target, place = lora_ref.designed_matrix(fam)
+        raw = lora_ref.merge_tensor(b"", wtype, 64, 64, A, B, -4, 2, base.tobytes(), ggjt.T_F32)
+        assert raw == lora_ref.quantize(target, wtype), fam
+
+
+def test_zero_b_rows_give_plus_zero():
+    """A row of loraB that is zero gives BA == +0 in every column at every rank path, and -0 under a negative scale:
+    the large-shape GPU tests compute BA only on the rows where loraB is nonzero."""
+    rng = np.random.default_rng(3)
+    for r in (1, 31, 32, 33, 64, 65, 308):
+        A = rng.standard_normal((96, r), dtype=np.float32)
+        B = rng.standard_normal((4, r), dtype=np.float32)
+        B[1] = 0
+        for alpha, neg in ((r, False), (2 * r + 1, False), (0, False), (-r - 3, True)):
+            z = lora_ref.ba(A, B, alpha, r)[1]
+            assert np.all(z == 0) and np.all(np.signbit(z) == neg), (r, alpha)
 
 
 def test_fma_is_exact():
