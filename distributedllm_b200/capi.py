@@ -43,6 +43,11 @@ MAX_TOP = 20            # the most alternatives a logprobs call returns per id (
 _lib: Optional[C.CDLL] = None
 
 
+class Guidance(C.Structure):
+    _fields_ = [("sessions", C.c_void_p), ("prompt_counts", C.c_void_p), ("prompt_tokens", C.c_void_p),
+                ("scale", C.c_float), ("smooth_factor", C.c_float)]
+
+
 def lib() -> C.CDLL:
     """Load the native library; raises if it has not been built (there is no fallback)."""
     global _lib
@@ -123,6 +128,9 @@ def lib() -> C.CDLL:
                            ("b200_generate_lp", [vp, ci, vp, vp, vp, ci, vp, ci, vp, vp, vp]),
                            ("b200_generate_speculative_lp", [vp, ci, vp, ci, vp, ci, vp, ci, vp, ci, ci, ci, vp, vp, vp, vp]),
                            ("b200_extra_logprobs", [vp, vp, ci, vp, ci, vp, vp, vp]),
+                           ("b200_generate_cfg", [vp, ci, vp, vp, vp, ci, vp, ci, vp, vp, vp, vp]),
+                           ("b200_extra_cfg", [vp, vp, vp, ci, cf, cf, vp, vp]),
+                           ("b200_stream_add_cfg", [vp, ci, vp, ci, ci, vp, vp, ci, ci, ci, vp, ci, cf, cf]),
                            ("b200_stream_add_lp", [vp, ci, vp, ci, ci, vp, vp, ci, ci]),
                            ("b200_stream_read_lp", [vp, vp, vp, vp, vp, vp, ci, C.POINTER(ci)]),
                            ("b200_stream_fork", [vp, ci, ci, ci]),
@@ -475,6 +483,19 @@ class Extra:
                                         _ptr(out.top_lp)))
         return out.lp, out.top_ids, out.top_lp
 
+    def cfg(self, base: np.ndarray, guidance: np.ndarray, scale: float, smooth_factor: float):
+        """llama.cpp's classifier-free guidance on the device (b200_extra_cfg) for each row pair of [n][n_vocab] logits
+        (client.cfg_logits is the host twin).  -> (out float32 [n][n_vocab], greedy ids [n])."""
+        b = np.ascontiguousarray(base, dtype=np.float32).reshape(-1, self.n_vocab)
+        g = np.ascontiguousarray(guidance, dtype=np.float32).reshape(-1, self.n_vocab)
+        if g.shape != b.shape:
+            raise ValueError("need one guidance row per base row (%d), got %d" % (len(b), len(g)))
+        out = np.zeros_like(b)
+        greedy = np.zeros(len(b), np.int32)
+        check(lib().b200_extra_cfg(self._h, _ptr(b), _ptr(g), len(b), float(scale), float(smooth_factor), _ptr(out),
+                                   _ptr(greedy)))
+        return out, greedy
+
     def close(self) -> None:
         if self._h:
             check(lib().b200_extra_unload(self._h))
@@ -502,17 +523,47 @@ class _LpOut:
                           self.top_lp.ctypes.data if n_top else None)
 
 
-def generate_greedy(slices, extra: Extra, sessions, prompts, n_steps: int, logprobs: Optional[int] = None):
+def _guidance(n: int, guidance):
+    """guidance = (sessions, negative prompts, scale, smooth_factor) -> (b200_guidance_t, the arrays it points into)."""
+    try:
+        sessions, prompts, scale, smooth_factor = guidance
+    except (TypeError, ValueError):
+        raise TypeError("guidance must be (sessions, negative prompts, scale, smooth_factor)") from None
+    gs = np.ascontiguousarray(sessions, dtype=np.int32)
+    if len(gs) != n or len(prompts) != n:
+        raise ValueError("need one guidance session and one negative prompt per listed session (%d)" % n)
+    counts = np.array([len(p) for p in prompts], np.int32)
+    toks = np.ascontiguousarray([int(t) for p in prompts for t in p] or [0], dtype=np.int32)
+    return Guidance(gs.ctypes.data, counts.ctypes.data, toks.ctypes.data, float(scale), float(smooth_factor)), [gs, counts, toks]
+
+
+def _generate_cfg(slices, extra, ids, counts, toks, n_steps, guidance, sp, logprobs):
+    """b200_generate_cfg for generate_greedy (sp None) and generate_sample."""
+    g, keep = _guidance(len(ids), guidance)
+    handles = (C.c_void_p * max(len(slices), 1))(*[s.handle for s in slices])
+    out = np.zeros((max(n_steps, 0), len(ids)), np.int32)
+    lp = _LpOut(out.shape, _n_top(logprobs, extra.n_vocab)) if logprobs is not None else None
+    check(lib().b200_generate_cfg(handles, len(slices), extra.handle, _ptr(ids), _ptr(counts), len(ids), _ptr(toks), n_steps,
+                                  C.byref(g), C.byref(sp) if sp is not None else None, _ptr(out),
+                                  C.byref(lp.c) if lp is not None else None))
+    return out if lp is None else (out, lp.lp, lp.top_ids, lp.top_lp)
+
+
+def generate_greedy(slices, extra: Extra, sessions, prompts, n_steps: int, logprobs: Optional[int] = None, guidance=None):
     """Greedy decoding on the device (b200_generate_greedy): session sessions[k] is fed prompts[k] (a list of token ids),
     then n_steps - 1 of its own ids.  `slices` are in layer order, all on the extra layers' GPU.  -> [n_steps][n_seq] ids.
     logprobs = n_top (0..20): b200_generate_lp instead, -> (ids, lp [n_steps][n_seq], top_ids and top_lp
-    [n_steps][n_seq][n_top]) in the raw distribution (include/b200_slice.h)."""
+    [n_steps][n_seq][n_top]) in the raw distribution (include/b200_slice.h).
+    guidance = (guidance sessions, negative prompts, scale, smooth_factor): classifier-free guidance (b200_generate_cfg),
+    guidance session k fed negative prompt k, then session k's ids."""
     ids = np.ascontiguousarray(sessions, dtype=np.int32)
     if len(prompts) != len(ids):
         raise ValueError("need one prompt per listed session")
     counts = np.array([len(p) for p in prompts], np.int32)
     toks = np.ascontiguousarray(np.concatenate([np.asarray(p, np.int64) for p in prompts]) if len(prompts) else [],
                                 dtype=np.int32)
+    if guidance is not None:
+        return _generate_cfg(slices, extra, ids, counts, toks, n_steps, guidance, None, logprobs)
     handles = (C.c_void_p * max(len(slices), 1))(*[s.handle for s in slices])
     out = np.zeros((max(n_steps, 0), len(ids)), np.int32)
     if logprobs is not None:
@@ -556,11 +607,12 @@ def _sampling(n: int, temperature: float, repeat_penalty: float, seeds, first_dr
 
 def generate_sample(slices, extra: Extra, sessions, prompts, n_steps: int, temperature: float, repeat_penalty: float,
                     seeds, first_draw: int = 0, history=None, top_k: int = 0, top_p: float = 0.0,
-                    logprobs: Optional[int] = None):
+                    logprobs: Optional[int] = None, guidance=None):
     """Sampled generation on the device (b200_generate_sample): generate_greedy's loop with the client's Sampler in place
     of the argmax.  Session sessions[k] draws from numpy.random.Philox(key=seeds[k]) starting at draw first_draw, with
     history[k] (ids it sampled before) penalised and every row truncated to top_k / top_p (0: off).
-    -> [n_steps][n_seq] ids; with logprobs = n_top, (ids, lp, top_ids, top_lp) as generate_greedy."""
+    -> [n_steps][n_seq] ids; with logprobs = n_top, (ids, lp, top_ids, top_lp) as generate_greedy.  guidance as
+    generate_greedy: the Sampler draws from the guided rows."""
     ids = np.ascontiguousarray(sessions, dtype=np.int32)
     if len(prompts) != len(ids):
         raise ValueError("need one prompt per listed session")
@@ -568,6 +620,8 @@ def generate_sample(slices, extra: Extra, sessions, prompts, n_steps: int, tempe
     counts = np.array([len(p) for p in prompts], np.int32)
     toks = np.ascontiguousarray(np.concatenate([np.asarray(p, np.int64) for p in prompts]) if len(prompts) else [],
                                 dtype=np.int32)
+    if guidance is not None:
+        return _generate_cfg(slices, extra, ids, counts, toks, n_steps, guidance, sp, logprobs)
     handles = (C.c_void_p * max(len(slices), 1))(*[s.handle for s in slices])
     out = np.zeros((max(n_steps, 0), len(ids)), np.int32)
     if logprobs is not None:
@@ -722,12 +776,13 @@ class Stream:
 
     def add(self, session: int, prompt, max_tokens: int, temperature: Optional[float] = None, repeat_penalty: float = 1.1,
             seed: int = 0, first_draw: int = 0, history=None, stop_ids=(), top_k: int = 0, top_p: float = 0.0,
-            logprobs: Optional[int] = None) -> None:
+            logprobs: Optional[int] = None, guidance=None) -> None:
         """Queue `session` with `prompt` (token ids) for at most max_tokens ids.  temperature None: greedy (the argmax of
         the raw logits); else the client's Sampler with repeat_penalty on numpy.random.Philox(key=seed), starting at draw
         first_draw, with history (ids sampled before) penalised, truncated to top_k / top_p (0: off).  The session ends
         after the first id in stop_ids.  logprobs = n_top (0..20): each id's record (read_logprobs) holds its
-        log-probability and n_top alternatives (b200_stream_add_lp)."""
+        log-probability and n_top alternatives (b200_stream_add_lp).  guidance = (guidance session, negative prompt ids,
+        scale, smooth_factor): classifier-free guidance (b200_stream_add_cfg); the pair enters and leaves as one."""
         session = _int("session", session, 0, 2 ** 31 - 1)
         p = _ids("prompt", prompt, self.n_vocab, 1)
         max_tokens = _int("max_tokens", max_tokens, 1, 2 ** 31 - 1)
@@ -746,6 +801,18 @@ class Stream:
             sp, keep = _sampling(1, t, rp, [seed], first_draw, history, top_k, top_p)
         elif history is not None or first_draw or _truncation(top_k, top_p) != (0, 0.0):
             raise ValueError("history, first_draw, top_k and top_p apply to sampled sessions (give a temperature)")
+        if guidance is not None:
+            try:
+                g_session, g_ids, scale, smooth_factor = guidance
+            except (TypeError, ValueError):
+                raise TypeError("guidance must be (session, negative prompt ids, scale, smooth_factor)") from None
+            g_session = _int("guidance session", g_session, 0, 2 ** 31 - 1)
+            neg = _ids("negative prompt", g_ids, self.n_vocab, 1)
+            n_top = -1 if logprobs is None else _n_top(logprobs, self.n_vocab)
+            check(lib().b200_stream_add_cfg(self._handle(), session, _ptr(p), len(prompt), max_tokens,
+                                            None if sp is None else C.byref(sp), _ptr(stops), len(stop_ids), n_top,
+                                            g_session, _ptr(neg), len(g_ids), float(scale), float(smooth_factor)))
+            return
         if logprobs is not None:
             n_top = _n_top(logprobs, self.n_vocab)
             check(lib().b200_stream_add_lp(self._handle(), session, _ptr(p), len(prompt), max_tokens,

@@ -100,6 +100,64 @@ def ppl_terms(logits, targets) -> np.ndarray:
     return out
 
 
+def _exp_f32(v: np.ndarray) -> np.ndarray:
+    return np.exp(v.astype(np.float64)).astype(np.float32)
+
+
+def _log_f32(v: np.ndarray) -> np.ndarray:
+    return np.log(v.astype(np.float64)).astype(np.float32)
+
+
+def _fma_f32(a, b, c) -> np.ndarray:
+    """float32 fma(a, b, c), rounded once: float64 a*b is exact, and a TwoSum plus round-to-odd keeps the float64 sum from
+    rounding twice."""
+    p = np.asarray(a, np.float32).astype(np.float64) * np.asarray(b, np.float32).astype(np.float64)
+    c64 = np.asarray(c, np.float32).astype(np.float64)
+    hi = p + c64
+    bb = hi - p
+    lo = (p - (hi - bb)) + (c64 - bb)
+    odd = (lo != 0) & ((hi.view(np.int64) & 1) == 0) & np.isfinite(hi)
+    hi = np.where(odd, np.nextafter(hi, np.where(lo > 0, np.inf, -np.inf)), hi)
+    return hi.astype(np.float32)
+
+
+def _log_softmax_f32(v: np.ndarray, expf, logf) -> np.ndarray:
+    """llama_log_softmax (llama.cpp:2170-2182) on one float32 row: m = *max_element (v_0 when it is NaN), p = expf(v - m),
+    the p summed in float32 in index order (np.add.accumulate is sequential), logf(p / sum)."""
+    m = v[0] if np.isnan(v[0]) else np.nanmax(v)
+    p = expf(v - np.float32(m))
+    S = np.add.accumulate(p, dtype=np.float32)[-1]
+    return logf(p / S)
+
+
+def cfg_logits(base, guidance, scale: float, smooth_factor: float, expf=_exp_f32, logf=_log_f32) -> np.ndarray:
+    """llama.cpp's classifier-free guidance (llama_sample_classifier_free_guidance) for each row pair of [n][n_vocab]
+    logits, the host twin of the device's (include/b200_slice.h): lb = log_softmax(base), lg = log_softmax(guidance),
+    mix = fmaf(scale, lb - lg, lg), out = fmaf(sf, log_softmax(mix), (1 - sf) * lb), every step in float32 and the two
+    FMAs rounded once.  expf / logf default to float64 exp / log rounded to float32, as on the device; pass libm's to get
+    the reference build's bits.  -> float32 [n][n_vocab]."""
+    b = np.asarray(base, np.float32)
+    g = np.asarray(guidance, np.float32).reshape(b.shape)
+    b2, g2 = b.reshape(-1, b.shape[-1]), g.reshape(-1, b.shape[-1])
+    out = np.empty_like(b2)
+    sc, sf = np.float32(scale), np.float32(smooth_factor)
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore", under="ignore"):
+        for k in range(len(b2)):
+            lb, lg = _log_softmax_f32(b2[k], expf, logf), _log_softmax_f32(g2[k], expf, logf)
+            lg2 = _log_softmax_f32(_fma_f32(sc, lb - lg, lg), expf, logf)
+            out[k] = _fma_f32(sf, lg2, (np.float32(1) - sf) * lb)
+    return out.reshape(b.shape)
+
+
+def cfg_greedy(row) -> int:
+    """llama_sample_token_greedy on one row: std::max_element with `<` -- the first element when it is NaN, else the
+    first largest non-NaN value."""
+    row = np.asarray(row, np.float32)
+    if np.isnan(row[0]):
+        return 0
+    return int(np.nanargmax(row))
+
+
 def running_perplexity(terms) -> List[float]:
     """The values perplexity.cpp prints after each window, from terms [n_chunk][n_scored]: nll (float64) adds the terms
     window by window, row by row,
@@ -298,17 +356,41 @@ class LocalPipeline:
             self._extra = (extra_path, self.capi.Extra(extra_path, devices[0]))
         return self._extra[1]
 
-    def generate_greedy(self, extra_path: str, prompt: str, max_steps: int = 200, logprobs: int = None) -> list:
+    def _guidance(self, extra, cfg_negative_prompt, cfg_scale: float, cfg_smooth_factor: float):
+        """llama.cpp main's --cfg-negative-prompt / --cfg-scale / --cfg-smooth-factor as capi's guidance= argument:
+        None when guidance is off (no negative prompt, or cfg_scale <= 1, as main), else session 1 fed the negative prompt,
+        tokenized as the prompt is."""
+        if cfg_negative_prompt is None or not cfg_scale > 1:
+            return None
+        if self.slices[0].n_sessions < 2:
+            raise ValueError("classifier-free guidance runs the negative prompt in session 1: load the slices with "
+                             "n_sessions >= 2 (they have %d)" % self.slices[0].n_sessions)
+        return ([1], [extra.tokenize(cfg_negative_prompt)], float(cfg_scale), float(cfg_smooth_factor))
+
+    def generate_greedy(self, extra_path: str, prompt: str, max_steps: int = 200, logprobs: int = None,
+                        cfg_negative_prompt: str = None, cfg_scale: float = 1.0, cfg_smooth_factor: float = 1.0) -> list:
         """DistributedLLM.generate_greedy on this box: clear the contexts, tokenize, then max_steps argmax steps, all on
         the GPU with no host round trip between tokens (capi.generate_greedy).  Needs every slice on one device.
-        logprobs = n_top (0..20): a list of (id, lp, [(id, lp), ...]) instead of ids."""
+        logprobs = n_top (0..20): a list of (id, lp, [(id, lp), ...]) instead of ids.  cfg_negative_prompt with
+        cfg_scale > 1: llama.cpp main's classifier-free guidance (capi.generate_greedy's guidance=), the negative prompt in
+        session 1; the log-probabilities stay those of the unguided logits."""
         extra = self._device_extra(extra_path, "greedy generation")
         if logprobs is not None:
             logprobs = _int("logprobs", logprobs, 0, MAX_TOP)
+        guidance = self._guidance(extra, cfg_negative_prompt, cfg_scale, cfg_smooth_factor)
         self.clear_context()
+        if guidance is not None:
+            for sl in self.slices:
+                sl.session_clear(1)
         tokens = extra.tokenize(prompt)
         if max_steps < 1:
             return []
+        if guidance is not None:
+            out = self.capi.generate_greedy(self.slices, extra, [0], [tokens], max_steps, logprobs=logprobs, guidance=guidance)
+            if logprobs is None:
+                return out[:, 0].tolist()
+            ids, lp, ti, tl = out
+            return _with_logprobs(ids[:, 0], lp[:, 0], ti[:, 0], tl[:, 0])
         if logprobs is None:
             return self.capi.generate_greedy(self.slices, extra, [0], [tokens], max_steps)[:, 0].tolist()
         ids, lp, ti, tl = self.capi.generate_greedy(self.slices, extra, [0], [tokens], max_steps, logprobs=logprobs)
@@ -316,7 +398,8 @@ class LocalPipeline:
 
     def generate(self, extra_path: str, prompt: str, max_steps: int = 200, temperature: float = 0.0,
                  repeat_penalty: float = 1.1, seed: int = None, stop_at_eos: bool = False, top_k: int = None,
-                 top_p: float = None, logprobs: int = None):
+                 top_p: float = None, logprobs: int = None, cfg_negative_prompt: str = None, cfg_scale: float = 1.0,
+                 cfg_smooth_factor: float = 1.0):
         """DistributedLLM.generate on this box: clear the contexts, tokenize, then up to max_steps steps of the client's
         Sampler, all on the GPU with no host round trip between tokens (a one-session capi.Stream).  Yields each token
         string as soon as its id is drawn; leaving the loop early cancels the steps that remain, and the slices' n_past
@@ -326,19 +409,26 @@ class LocalPipeline:
         stop_at_eos=True ends the run after the end-of-sequence id (EOS_ID, yielded); the default runs max_steps steps,
         as the reference does.  top_k / top_p truncate each draw as client.Sampler does (None: off).  logprobs = n_top
         (0..20): yield (text, lp, [(id, lp), ...]) as DistributedLLM.generate does, from the stream's records.  Needs
-        every slice on one device."""
+        every slice on one device.
+        cfg_negative_prompt with cfg_scale > 1: llama.cpp main's classifier-free guidance, the Sampler drawing from the
+        guided rows (capi.Stream.add's guidance=, the negative prompt in session 1, which ends with session 0)."""
         extra = self._device_extra(extra_path, "sampled generation")
         if logprobs is not None:
             logprobs = _int("logprobs", logprobs, 0, MAX_TOP)
         if seed is None:
             seed = int(np.random.randint(0, 2 ** 64, dtype=np.uint64))
+        guidance = self._guidance(extra, cfg_negative_prompt, cfg_scale, cfg_smooth_factor)
         self.clear_context()
+        if guidance is not None:
+            for sl in self.slices:
+                sl.session_clear(1)
         tokens = extra.tokenize(prompt)
         if max_steps < 1:
             return
         with self.capi.Stream(self.slices, extra) as st:
             st.add(0, tokens, max_steps, temperature, repeat_penalty, seed, stop_ids=[EOS_ID] if stop_at_eos else (),
-                   top_k=top_k or 0, top_p=top_p or 0.0, logprobs=logprobs)
+                   top_k=top_k or 0, top_p=top_p or 0.0, logprobs=logprobs,
+                   guidance=None if guidance is None else (1, guidance[1][0], guidance[2], guidance[3]))
             records = iter(st) if logprobs is None else _read_records(st)
             for j, rec in enumerate(records):
                 token_id = rec[1]

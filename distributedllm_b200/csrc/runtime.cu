@@ -2496,6 +2496,8 @@ struct b200_extra {
     float * d_terms = nullptr; int cap_terms = 0;
     // log-probabilities (k_logprob_rows): lp [rows], top ids and their lp [rows][n_top]
     double * d_lp = nullptr; int cap_lp = 0; int32_t * d_topi = nullptr; int cap_topi = 0; double * d_topl = nullptr; int cap_topl = 0;
+    // classifier-free guidance (k_cfg_rows): the guided rows [rows][n_vocab], kept apart so log-probabilities read raw rows
+    float * d_cfg = nullptr; int cap_cfg = 0;
     std::vector<std::pair<std::string, float>> vocab;
     std::unordered_map<std::string, int> token_to_id;
     std::mutex mu;
@@ -2964,9 +2966,10 @@ __global__ void __launch_bounds__(1024) k_sample_rows(SampleArgs a) {
 
 // ---- generation streams (b200_stream_*): the sampler's state lives in per-session slots, and a step's rows name their slot
 struct StreamSlot { uint64_t seed; double dt, dp; int sampled, top_k; double top_p; };   // device table, one per session
-struct StreamRow { long long draw; int slot, gather, n_top; };       // per step, in mapped pinned memory: draw index, slot,
-                                                                    // the session's last row in the pass, and its top-n
-                                                                    // (-1: no log-probabilities)
+struct StreamRow { long long draw; int slot, gather, n_top, gather2; };   // per step, in mapped pinned memory: draw index,
+                                                                    // slot, the session's last row in the pass, its top-n
+                                                                    // (-1: no log-probabilities), and its guidance
+                                                                    // session's last row (-1: unguided)
 
 // A step's token rows: row r is the prompt id spec[r] when spec[r] >= 0, else the last id slot ~spec[r] drew.  spec lies in
 // mapped pinned memory.
@@ -2981,10 +2984,11 @@ __global__ void k_stream_tokens(const int32_t * spec, const int32_t * last, int 
 // ring, which the host set to INT32_MIN, so the region is not reused before the step's k_stream_tokens has read it.
 __global__ void k_stream_mark(int32_t * cell) { *(volatile int32_t *) cell = 0; }
 
-// Row k of out is row rows[k].gather of x: each session's last row of a mixed pass, packed for the lm_head.
-__global__ void k_gather_rows(const float * x, const StreamRow * rows, int E, float * out) {
+// Row k of out is row rows[k].gather of x (rows[k].gather2 when second): each session's last row of a mixed pass, or its
+// guidance session's, packed for the lm_head.
+__global__ void k_gather_rows(const float * x, const StreamRow * rows, int E, float * out, bool second = false) {
     __shared__ int g;
-    if (threadIdx.x == 0) g = rows[blockIdx.y].gather;
+    if (threadIdx.x == 0) g = second ? rows[blockIdx.y].gather2 : rows[blockIdx.y].gather;
     __syncthreads();
     const float * src = x + (size_t) g * E;
     float * dst = out + (size_t) blockIdx.y * E;
@@ -2996,9 +3000,11 @@ __global__ void k_gather_rows(const float * x, const StreamRow * rows, int E, fl
 // (sample_row, which then marks the id in the slot's penalty bitmap).  The id becomes the slot's last id, which the next
 // step's k_stream_tokens reads, and is stored into cell k of the step's publish ring in mapped pinned memory: the host
 // sets every cell to INT32_MIN before it enqueues the step, so each cell carries its own readiness.  A row that asked for
-// log-probabilities is published by k_stream_logprobs instead, after its record.
+// log-probabilities is published by k_stream_logprobs instead, after its record.  Guided rows (logits: k_cfg_rows' rows)
+// take a greedy slot's id from pick[k], k_cfg_rows' max_element pick, instead of the argmax.
 __global__ void __launch_bounds__(1024) k_stream_draw(const float * logits, int n, const StreamRow * rows,
-                                                      const StreamSlot * slots, uint32_t * pen, int32_t * last, int32_t * ring) {
+                                                      const StreamSlot * slots, uint32_t * pen, int32_t * last, int32_t * ring,
+                                                      const int32_t * pick = nullptr) {
     __shared__ StreamRow s_row;
     const int k = blockIdx.x;
     if (threadIdx.x == 0) s_row = rows[k];
@@ -3007,7 +3013,8 @@ __global__ void __launch_bounds__(1024) k_stream_draw(const float * logits, int 
     const StreamSlot sl = slots[slot];
     const float * x = logits + (size_t) k * n;
     uint32_t * bits = pen + (size_t) slot * ((n + 31) >> 5);
-    const int id = sl.sampled ? sample_row(x, n, bits, sl.dt, sl.dp, sl.seed, s_row.draw, sl.top_k, sl.top_p) : argmax_row(x, n);
+    const int id = sl.sampled ? sample_row(x, n, bits, sl.dt, sl.dp, sl.seed, s_row.draw, sl.top_k, sl.top_p)
+                              : pick ? pick[k] : argmax_row(x, n);
     if (threadIdx.x != 0) return;
     if (sl.sampled && id >= 0) bits[id >> 5] |= 1u << (id & 31);
     last[slot] = id;
@@ -3128,6 +3135,135 @@ __global__ void __launch_bounds__(kPplThreads) k_ppl_rows(const float * logits, 
         }
         term[r] = out;
     }
+}
+
+// ---- llama.cpp's classifier-free guidance (b200_generate_cfg, b200_extra_cfg): llama_sample_classifier_free_guidance
+// (llama.cpp:2170-2225) on a pair of rows, b the session's logits and g its guidance session's:
+//   log_softmax(v): m = *max_element(v) (v_0 when v_0 is NaN, else the largest non-NaN v_i), p_i = expf(v_i - m), S = the
+//     p_i summed in FLOAT strictly in index order, v_i = logf(p_i / S);
+//   lb = log_softmax(b), lg = log_softmax(g), mix_i = fmaf(scale, lb_i - lg_i, lg_i), lg2 = log_softmax(mix),
+//   out_i = fmaf(sf, lg2_i, (1 - sf) * lb_i)
+// with the two FMAs the reference build contracts (vfmadd132ss, vfmadd231ss) and nothing else fused.  expf / logf are the
+// double functions rounded to float (ppl_expf, cfg_logf), so glibc's, which are not correctly rounded everywhere, are the
+// one place the reference can give other bits.  The float sums are dependent chains of n additions, so k_ppl_rows' shape:
+// producer warps fill tiles of p_i into shared memory while lanes 0 and 1 of warp 0 add b's and g's in order, then the mix
+// chain on lane 0.  The logs are recomputed from the inputs where needed (no n-float scratch besides the output row, which
+// holds mix until the last phase overwrites it).
+// pick[k] is max_element(out) (llama_sample_token_greedy: out_0 when it is NaN, else the first largest non-NaN value), or
+// -1 when b or g has no distribution (a NaN or +inf, or all -inf); then, when bad is given, atomicMin(bad, bad_base + k).
+constexpr int kCfgTile = 512, kCfgThreads = 256;
+
+__device__ __forceinline__ float cfg_logf(float v) { return __double2float_rn(log((double) v)); }
+
+struct CfgArgs {
+    const float * base, * guid;     // row k of each: [rows][n]
+    int n;
+    float scale, sf;
+    float * out;                    // [rows][n]
+    int32_t * pick, * pick2;        // [rows], either may be NULL (generation: the next step's token and the call's ids)
+    int * bad; int bad_base;        // may be NULL
+};
+
+// max_element's value over x[0, n) (NaN when x_0 is NaN) and whether x has a distribution, for a whole block.
+__device__ __forceinline__ float cfg_row_max(const float * x, int n, bool * ok) {
+    __shared__ float s_mx[32]; __shared__ int s_bad[32];
+    const int t = threadIdx.x, lane = t & 31, wid = t >> 5, nwarp = blockDim.x >> 5;
+    float mx = -INFINITY; bool bad = false;
+    for (int i = t; i < n; i += blockDim.x) { const float v = x[i]; bad |= v != v || v == INFINITY; mx = fmaxf(mx, v); }
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    bad = __any_sync(0xffffffffu, bad);
+    __syncthreads();                                     // the previous call's readers are done with s_mx
+    if (lane == 0) { s_mx[wid] = mx; s_bad[wid] = bad; }
+    __syncthreads();
+    mx = lane < nwarp ? s_mx[lane] : -INFINITY;
+    bad = lane < nwarp ? s_bad[lane] : false;
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    bad = __any_sync(0xffffffffu, bad);
+    *ok = !bad && mx != -INFINITY;
+    const float x0 = x[0];
+    return x0 != x0 ? x0 : mx;
+}
+
+// The in-order float sums of expf(x_r[i] - m[r]) for nr (1 or 2) rows, lane r of warp 0 holding row r's chain; every
+// thread gets them in S[0 .. nr).
+__device__ __forceinline__ void cfg_chains(const float * const * x, const float * m, int nr, int n, float * S) {
+    __shared__ float s_e[2][2][kCfgTile + 1];
+    __shared__ float s_S[2];
+    const int t = threadIdx.x, wid = t >> 5;
+    const int n_tiles = (n + kCfgTile - 1) / kCfgTile;
+    auto produce = [&](int tile) {
+        const int c0 = tile * kCfgTile, cn = min(kCfgTile, n - c0);
+        for (int idx = t - 32; idx < nr * kCfgTile; idx += kCfgThreads - 32) {
+            const int r = idx / kCfgTile, c = idx % kCfgTile;
+            if (c < cn) s_e[tile & 1][r][c] = ppl_expf(__fsub_rn(x[r][c0 + c], m[r]));
+        }
+    };
+    if (wid > 0) produce(0);
+    __syncthreads();
+    float acc = 0.f;
+    for (int k = 0; k < n_tiles; k++) {
+        if (wid > 0) {
+            if (k + 1 < n_tiles) produce(k + 1);
+        } else if (t < nr) {
+            const float * e = s_e[k & 1][t];
+            const int cn = min(kCfgTile, n - k * kCfgTile);
+#pragma unroll 8
+            for (int c = 0; c < cn; c++) acc = __fadd_rn(acc, e[c]);
+        }
+        __syncthreads();
+    }
+    if (t < nr) s_S[t] = acc;
+    __syncthreads();
+    for (int r = 0; r < nr; r++) S[r] = s_S[r];
+}
+
+__global__ void __launch_bounds__(kCfgThreads) k_cfg_rows(CfgArgs a) {
+    __shared__ float s_v[32]; __shared__ int s_i[32];
+    const int t = threadIdx.x, lane = t & 31, wid = t >> 5, nwarp = blockDim.x >> 5, n = a.n;
+    const size_t k = blockIdx.x;
+    const float * b = a.base + k * n, * g = a.guid + k * n;
+    float * out = a.out + k * n;
+    bool ok_b, ok_g;
+    float m[2];
+    m[0] = cfg_row_max(b, n, &ok_b);
+    m[1] = cfg_row_max(g, n, &ok_g);
+    const float * rows[2] = {b, g};
+    float S[2];
+    cfg_chains(rows, m, 2, n, S);
+    auto lb_at = [&](int i) { return cfg_logf(__fdiv_rn(ppl_expf(__fsub_rn(b[i], m[0])), S[0])); };
+    for (int i = t; i < n; i += blockDim.x) {
+        const float lb = lb_at(i), lg = cfg_logf(__fdiv_rn(ppl_expf(__fsub_rn(g[i], m[1])), S[1]));
+        out[i] = __fmaf_rn(a.scale, __fsub_rn(lb, lg), lg);
+    }
+    __syncthreads();                                     // out (the mix row) is visible to the whole block
+    bool ok_mix;                                         // unused: a mix row without a distribution is NaN by arithmetic
+    float m2[1] = {cfg_row_max(out, n, &ok_mix)};
+    const float * mrow[1] = {out};
+    float S2[1];
+    cfg_chains(mrow, m2, 1, n, S2);
+    const float one_minus = __fsub_rn(1.f, a.sf);
+    float bv = -INFINITY; int bi = 0x7fffffff;
+    for (int i = t; i < n; i += blockDim.x) {
+        const float lg2 = cfg_logf(__fdiv_rn(ppl_expf(__fsub_rn(out[i], m2[0])), S2[0]));
+        const float v = __fmaf_rn(a.sf, lg2, __fmul_rn(one_minus, lb_at(i)));
+        out[i] = v;
+        if (v > bv) { bv = v; bi = i; }                  // NaN never wins; ascending i keeps the first of equals
+    }
+    auto better = [](float v, int i, float bv, int bi) { return v > bv || (v == bv && i < bi); };
+    for (int o = 16; o > 0; o >>= 1) {
+        const float v = __shfl_xor_sync(0xffffffffu, bv, o); const int i = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (better(v, i, bv, bi)) { bv = v; bi = i; }
+    }
+    if (lane == 0) { s_v[wid] = bv; s_i[wid] = bi; }
+    __syncthreads();
+    if (t != 0) return;
+    bv = s_v[0]; bi = s_i[0];
+    for (int w = 1; w < nwarp; w++) if (better(s_v[w], s_i[w], bv, bi)) { bv = s_v[w]; bi = s_i[w]; }
+    const float o0 = out[0];
+    const int id = !(ok_b && ok_g) ? -1 : (o0 != o0 || bi == 0x7fffffff) ? 0 : bi;
+    if (a.pick) a.pick[k] = id;
+    if (a.pick2) a.pick2[k] = id;
+    if (id < 0 && a.bad) atomicMin(a.bad, a.bad_base + (int) k);
 }
 
 // ---- log-probabilities of drawn ids (b200_generate_lp, b200_stream_read_lp, b200_extra_logprobs): the raw distribution
@@ -3524,11 +3660,12 @@ static int sample_start(b200_extra * e, const b200_sampling_t * sp, int n_seq) {
     return 0;
 }
 
-// k_sample_rows on the first `rows` rows of d_logits with draw first_draw + step; a bad row k is recorded as
-// step * rows + k.
-static int sample_launch(b200_extra * e, const b200_sampling_t * sp, int rows, int step, int32_t * ids) {
+// k_sample_rows on the first `rows` rows of d_logits (or of `logits`) with draw first_draw + step; a bad row k is
+// recorded as step * rows + k.
+static int sample_launch(b200_extra * e, const b200_sampling_t * sp, int rows, int step, int32_t * ids,
+                         const float * logits = nullptr) {
     const double dt = sp->temperature + 1e-5;
-    SampleArgs a{e->d_logits, e->n_vocab, dt, sp->repeat_penalty * dt, e->d_seeds, (long long) sp->first_draw + step,
+    SampleArgs a{logits ? logits : e->d_logits, e->n_vocab, dt, sp->repeat_penalty * dt, e->d_seeds, (long long) sp->first_draw + step,
                  e->d_pen, e->d_tok, ids, e->d_bad, step * rows, sp->top_k, sp->top_p};
     k_sample_rows<<<rows, 1024, 0, e->ctx.stream>>>(a);
     B200_CUDA(cudaGetLastError());
@@ -3587,50 +3724,73 @@ static int sample_finish(b200_extra * e, int rows, const int * sessions) {
     return fail(B200_EINVAL, "row %d: the logits are all -inf or overflow float64 once scaled, so they have no distribution", k);
 }
 
+// A guided call's mixing settings (b200_guidance_t's scale and smooth_factor).
+struct CfgMix { float scale, sf; };
+
 // The loop of b200_generate_greedy (sp == NULL: argmax, k_argmax_rows) and b200_generate_sample (k_sample_rows), and of
-// b200_generate_lp (lp != NULL: k_logprob_rows after each step's draw).
+// b200_generate_lp (lp != NULL: k_logprob_rows after each step's draw).  With cfg (b200_generate_cfg), sessions, counts
+// and tokens list 2 * n_seq entries, guidance session k being entry n_seq + k: every pass carries both rows of each pair,
+// the guidance row fed the id its session drew, and k_cfg_rows turns each pair's logits into the row the draw reads, in
+// d_cfg; log-probabilities still read the session's raw row.
 static int generate_locked(b200_slice * const * slices, int n_slices, b200_extra * e, const int * sessions,
                            const int * counts, int n_seq, const int32_t * tokens, int n_steps, const b200_sampling_t * sp,
-                           int32_t * ids, const b200_logprobs_t * lp) {
+                           int32_t * ids, const b200_logprobs_t * lp, const CfgMix * cfg = nullptr) {
     b200_slice * x = &e->ctx;
     B200_CUDA(cudaSetDevice(x->device));
+    const int n_rows = cfg ? 2 * n_seq : n_seq;
     int total = 0;
-    for (int k = 0; k < n_seq; k++) total += counts[k];
+    for (int k = 0; k < n_rows; k++) total += counts[k];
     int rc;
     if ((rc = extra_reserve(e, total)) || (rc = extra_reserve_ids(e, n_steps * n_seq))) return rc;
     if (lp && (rc = lp_reserve(e, n_steps * n_seq, lp->n_top))) return rc;
+    if (cfg && (rc = extra_regrow(e, e->d_cfg, e->cap_cfg, (size_t) e->n_vocab, n_seq))) return rc;
     for (int i = 0; i < n_slices; i++) B200_CUDA(cudaStreamSynchronize(slices[i]->stream));
     if (sp && (rc = sample_start(e, sp, n_seq))) return rc;
+    if (cfg && !sp) {                                    // greedy guided rows report a pair without a distribution
+        const int none = INT_MAX;
+        if ((rc = extra_reserve_sample(e, n_seq))) return rc;
+        B200_CUDA(cudaMemcpyAsync(e->d_bad, &none, 4, cudaMemcpyHostToDevice, x->stream));
+    }
     B200_CUDA(cudaMemcpyAsync(e->d_tok, tokens, (size_t) total * 4, cudaMemcpyHostToDevice, x->stream));
     {
         StreamLoan loan(slices, n_slices, x->stream);
         for (int step = 0; step < n_steps; step++) {
             // step 0: every session's prompt in one mixed pass; later steps: the id each session produced, one batched
             // step (a single session replays its captured decode graph).  Both are exact mode, as b200_mixed_forward.
-            const int N = step == 0 ? total : n_seq;
+            const int N = step == 0 ? total : n_rows;
             k_embed_rows<<<dim3((e->E + 255) / 256, N), 256, 0, x->stream>>>(e->emb_raw, e->emb_type, e->E, e->d_tok, e->n_vocab, e->d_x);
             B200_CUDA(cudaGetLastError());
             x->launches++;
             const float * cur = e->d_x;
             for (int i = 0; i < n_slices; i++) {
                 b200_slice * s = slices[i];
-                if (step == 0)       rc = pass_locked(s, sessions, counts, n_seq, cur, s->d_out, false);
-                else if (n_seq == 1) rc = forward_locked(s, cur, 1, s->d_out, false, sessions[0]);
-                else                 rc = pass_locked(s, sessions, nullptr, n_seq, cur, s->d_out, false);
+                if (step == 0)        rc = pass_locked(s, sessions, counts, n_rows, cur, s->d_out, false);
+                else if (n_rows == 1) rc = forward_locked(s, cur, 1, s->d_out, false, sessions[0]);
+                else                  rc = pass_locked(s, sessions, nullptr, n_rows, cur, s->d_out, false);
                 if (rc) return rc;
                 cur = s->d_out;
             }
-            if (step == 0 && total > n_seq) {        // each session's last prompt row, packed for the lm_head
-                for (int k = 0, end = 0; k < n_seq; k++) {
+            if (step == 0 && total > n_rows) {       // each session's last prompt row, packed for the lm_head
+                for (int k = 0, end = 0; k < n_rows; k++) {
                     end += counts[k];
                     B200_CUDA(cudaMemcpyAsync(e->d_x + (size_t) k * e->E, cur + (size_t)(end - 1) * e->E, (size_t) e->E * 4,
                                               cudaMemcpyDeviceToDevice, x->stream));
                 }
                 cur = e->d_x;
             }
-            if ((rc = extra_lmhead(e, cur, n_seq))) return rc;
+            if ((rc = extra_lmhead(e, cur, n_rows))) return rc;
             int32_t * step_ids = e->d_ids + (size_t) step * n_seq;
-            if (sp) {
+            if (cfg) {
+                // greedy: k_cfg_rows' pick is the id; sampled: k_sample_rows draws from the guided rows
+                CfgArgs c{e->d_logits, e->d_logits + (size_t) n_seq * e->n_vocab, e->n_vocab, cfg->scale, cfg->sf, e->d_cfg,
+                          sp ? nullptr : e->d_tok, sp ? nullptr : step_ids, sp ? nullptr : e->d_bad, step * n_seq};
+                k_cfg_rows<<<n_seq, kCfgThreads, 0, x->stream>>>(c);
+                B200_CUDA(cudaGetLastError());
+                x->launches++;
+                if (sp && (rc = sample_launch(e, sp, n_seq, step, step_ids, e->d_cfg))) return rc;
+                // the guidance rows of the next step take the ids their sessions drew
+                B200_CUDA(cudaMemcpyAsync(e->d_tok + n_seq, e->d_tok, (size_t) n_seq * 4, cudaMemcpyDeviceToDevice, x->stream));
+            } else if (sp) {
                 if ((rc = sample_launch(e, sp, n_seq, step, step_ids))) return rc;
             } else {
                 k_argmax_rows<<<n_seq, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, e->d_tok, step_ids);
@@ -3643,7 +3803,7 @@ static int generate_locked(b200_slice * const * slices, int n_slices, b200_extra
     B200_CUDA(cudaMemcpyAsync(ids, e->d_ids, (size_t) n_steps * n_seq * 4, cudaMemcpyDeviceToHost, x->stream));
     if (lp && (rc = lp_copy_back(e, lp, n_steps * n_seq))) return rc;
     B200_CUDA(cudaStreamSynchronize(x->stream));
-    return sp ? sample_finish(e, n_seq, sessions) : 0;
+    return sp || cfg ? sample_finish(e, n_seq, sessions) : 0;
 }
 
 }  // namespace b200
@@ -3688,6 +3848,59 @@ static int generate(const char * what, bool sampled, b200_slice_t * const * slic
         if (int rc = lp_check(lp, e->n_vocab)) return rc;
     return generate_locked(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps, sp, ids,
                            want_lp ? lp : nullptr);
+}
+
+// The mixing settings every guided call refuses before it touches a handle.
+static int cfg_mix_check(float scale, float sf) {
+    if (!std::isfinite(scale) || !(scale > 1.f))
+        return fail(B200_EINVAL, "guidance scale must be finite and > 1 (got %g): at 1 guidance is off, so do not ask for it",
+                    (double) scale);
+    if (!std::isfinite(sf)) return fail(B200_EINVAL, "guidance smooth_factor must be finite (got %g)", (double) sf);
+    return 0;
+}
+
+// b200_generate_cfg: the guidance checks, then generate_locked over the merged lists (real sessions, then guidance ones),
+// whose generate_check covers counts, ids and both contexts' room.
+static int generate_cfg(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
+                        const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps,
+                        const b200_guidance_t * g, const b200_sampling_t * sp, int32_t * ids, const b200_logprobs_t * lp) {
+    const char * what = "b200_generate_cfg";
+    if (!slices || n_slices < 1 || !e || !sessions || !prompt_counts || n_seq < 1 || !prompt_tokens || !ids)
+        return fail(B200_EINVAL, "%s: null argument or empty list", what);
+    if (!g || !g->sessions || !g->prompt_counts || !g->prompt_tokens) return fail(B200_EINVAL, "%s: null guidance", what);
+    if (int rc = cfg_mix_check(g->scale, g->smooth_factor)) return rc;
+    std::vector<std::unique_lock<std::mutex>> locks;
+    if (int rc = lock_handles(slices, n_slices, e, locks)) return rc;
+    for (int k = 0; k < n_seq; k++) {
+        const int gs = g->sessions[k];
+        for (int i = 0; i < n_slices; i++)
+            if (gs < 0 || gs >= slices[i]->n_sessions)
+                return fail(B200_EINVAL, "guidance session %d outside [0, %d) on slice %d", gs, slices[i]->n_sessions, i);
+        for (int j = 0; j < n_seq; j++) {
+            if (sessions[j] == gs) return fail(B200_EINVAL, "guidance session %d is also a listed session", gs);
+            if (j < k && g->sessions[j] == gs) return fail(B200_EINVAL, "guidance session %d listed twice", gs);
+        }
+        if (g->prompt_counts[k] < 1)
+            return fail(B200_EINVAL, "negative prompt %d has %d ids: it needs at least 1", k, g->prompt_counts[k]);
+    }
+    if (int rc = generate_check(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps)) return rc;
+    int n_prompt = 0, n_neg = 0;
+    for (int k = 0; k < n_seq; k++) { n_prompt += prompt_counts[k]; n_neg += g->prompt_counts[k]; }
+    if (int rc = check_tokens(g->prompt_tokens, n_neg, e->n_vocab, "negative prompt token")) return rc;
+    std::vector<int> all_sessions(sessions, sessions + n_seq), all_counts(prompt_counts, prompt_counts + n_seq);
+    all_sessions.insert(all_sessions.end(), g->sessions, g->sessions + n_seq);
+    all_counts.insert(all_counts.end(), g->prompt_counts, g->prompt_counts + n_seq);
+    std::vector<int32_t> all_tokens(prompt_tokens, prompt_tokens + n_prompt);
+    all_tokens.insert(all_tokens.end(), g->prompt_tokens, g->prompt_tokens + n_neg);
+    if (int rc = generate_check(slices, n_slices, e, all_sessions.data(), all_counts.data(), 2 * n_seq, all_tokens.data(), n_steps))
+        return rc;
+    if (sp)
+        if (int rc = sample_check(sp, n_seq, e->n_vocab)) return rc;
+    if (lp)
+        if (int rc = lp_check(lp, e->n_vocab)) return rc;
+    const CfgMix mix{g->scale, g->smooth_factor};
+    return generate_locked(slices, n_slices, e, all_sessions.data(), all_counts.data(), n_seq, all_tokens.data(), n_steps, sp,
+                           ids, lp, &mix);
 }
 
 // Rows the scoring loop's lm_head and k_nll_rows take at a time: its logits scratch is kScoreRows x n_vocab floats
@@ -4382,6 +4595,42 @@ int b200_extra_ppl_terms(b200_extra_t * e, const float * logits, int n_rows, con
     return 0;
 }
 
+int b200_generate_cfg(b200_slice_t * const * slices, int n_slices, b200_extra_t * e, const int * sessions,
+                      const int * prompt_counts, int n_seq, const int32_t * prompt_tokens, int n_steps,
+                      const b200_guidance_t * g, const b200_sampling_t * sp, int32_t * ids, const b200_logprobs_t * lp) {
+    return generate_cfg(slices, n_slices, e, sessions, prompt_counts, n_seq, prompt_tokens, n_steps, g, sp, ids, lp);
+}
+
+int b200_extra_cfg(b200_extra_t * e, const float * base, const float * guidance, int n_rows, float scale, float smooth_factor,
+                   float * out, int32_t * greedy) {
+    if (!e || !base || !guidance || n_rows < 1 || !out) return fail(B200_EINVAL, "b200_extra_cfg: null argument or no rows");
+    if (int rc = cfg_mix_check(scale, smooth_factor)) return rc;
+    std::lock_guard<std::mutex> lk(e->mu); B200_UNOWNED(&e->ctx);
+    const size_t V = (size_t) e->n_vocab;
+    for (const float * x : {base, guidance})
+        for (size_t i = 0; i < (size_t) n_rows * V; i++)
+            if (std::isnan(x[i]) || x[i] == INFINITY)
+                return fail(B200_EINVAL, "%s row %d has a non-finite logit at id %d (%g)", x == base ? "base" : "guidance",
+                            (int)(i / V), (int)(i % V), (double) x[i]);
+    b200_slice * s = &e->ctx;
+    B200_CUDA(cudaSetDevice(s->device));
+    int rc;
+    if ((rc = extra_reserve(e, 2 * n_rows)) || (rc = extra_reserve_ids(e, n_rows)) ||
+        (rc = extra_regrow(e, e->d_cfg, e->cap_cfg, V, n_rows)))
+        return rc;
+    B200_CUDA(cudaMemcpyAsync(e->d_logits, base, (size_t) n_rows * V * 4, cudaMemcpyHostToDevice, s->stream));
+    B200_CUDA(cudaMemcpyAsync(e->d_logits + (size_t) n_rows * V, guidance, (size_t) n_rows * V * 4, cudaMemcpyHostToDevice, s->stream));
+    CfgArgs c{e->d_logits, e->d_logits + (size_t) n_rows * V, e->n_vocab, scale, smooth_factor, e->d_cfg, e->d_ids, nullptr,
+              nullptr, 0};
+    k_cfg_rows<<<n_rows, kCfgThreads, 0, s->stream>>>(c);
+    B200_CUDA(cudaGetLastError());
+    s->launches++;
+    B200_CUDA(cudaMemcpyAsync(out, e->d_cfg, (size_t) n_rows * V * 4, cudaMemcpyDeviceToHost, s->stream));
+    if (greedy) B200_CUDA(cudaMemcpyAsync(greedy, e->d_ids, (size_t) n_rows * 4, cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    return 0;
+}
+
 int b200_extra_logprobs(b200_extra_t * e, const float * logits, int n_rows, const int32_t * ids, int n_top, double * lp,
                         int32_t * top_ids, double * top_lp) {
     if (!e || !logits || n_rows < 1 || !ids) return fail(B200_EINVAL, "b200_extra_logprobs: null argument or no rows");
@@ -4435,7 +4684,8 @@ struct b200_stream {
     int32_t * h_spec = nullptr; b200::StreamRow * h_rows = nullptr; int32_t * h_ring = nullptr;
     b200::LpRecord * h_lp = nullptr;      // mapped pinned, [regions][rows_cap]: the logprob ring beside h_ring
     struct Sess {
-        int state = 0;                    // 0 not in the stream, 1 queued, 2 admitted (its first chunk is enqueued)
+        int state = 0;                    // 0 not in the stream, 1 queued, 2 admitted (its first chunk is enqueued), 3 the
+                                          // guidance session of a guided one
         unsigned gen = 0;                 // bumped when the session leaves: rows of steps enqueued before are dropped
         std::vector<int32_t> prompt, stops;
         std::vector<int> old;             // n_past on each slice when it was added
@@ -4443,6 +4693,12 @@ struct b200_stream {
         int max_tokens = 0, enq = 0, delivered = 0;   // ids enqueued / returned by b200_stream_read
         int n_top = -1;                   // log-probabilities with n_top alternatives; -1: none
         long long first_draw = 0;
+        // classifier-free guidance: a guided session names its guidance session (state 3, owner = the guided one), which
+        // is fed neg, then the guided session's ids
+        int guide = -1, owner = -1;
+        std::vector<int32_t> neg;
+        int gfed = 0;                     // negative prompt ids enqueued
+        float scale = 0.f, sf = 0.f;
     };
     std::vector<Sess> sess;
     std::deque<int> queue;                // sessions whose prompt is not fully enqueued, in add order (the partly fed first)
@@ -4460,19 +4716,27 @@ constexpr int kStreamLookahead = 4;
 // The session leaves the stream: n_past = old + n_prompt + delivered - 1 (old when nothing was delivered) on every slice,
 // host copy now and device copy in stream order, behind any step the device still runs for it.  Those steps' rows are at
 // or above the new n_past, so they are unreachable; so are the rows of its prompt chunks when it leaves mid-prefill.
+// A guided session's guidance session leaves with it, at old + n_neg + delivered - 1 by the same rule.
 static int stream_finish(b200_stream * st, int k) {
     b200_stream::Sess & z = st->sess[k];
-    if (z.fed < (int) z.prompt.size()) st->queue.erase(std::find(st->queue.begin(), st->queue.end(), k));
+    const bool queued = z.fed < (int) z.prompt.size() || (z.guide >= 0 && z.gfed < (int) z.neg.size());
+    if (queued) st->queue.erase(std::find(st->queue.begin(), st->queue.end(), k));
     if (z.state == 2) {
-        for (size_t i = 0; i < st->slices.size(); i++) {
-            b200_slice * s = st->slices[i];
-            const int p = z.delivered ? z.old[i] + (int) z.prompt.size() + z.delivered - 1 : z.old[i];
-            if (s->past[k] == p) continue;
-            s->past[k] = p;
-            B200_CUDA(cudaMemcpyAsync(s->d_npast + k, &p, 4, cudaMemcpyHostToDevice, st->e->ctx.stream));   // staged at once
+        for (int who : {k, z.guide}) {
+            if (who < 0) continue;
+            const std::vector<int> & old = who == k ? z.old : st->sess[who].old;
+            const int n_in = who == k ? (int) z.prompt.size() : (int) z.neg.size();
+            for (size_t i = 0; i < st->slices.size(); i++) {
+                b200_slice * s = st->slices[i];
+                const int p = z.delivered ? old[i] + n_in + z.delivered - 1 : old[i];
+                if (s->past[who] == p) continue;
+                s->past[who] = p;
+                B200_CUDA(cudaMemcpyAsync(s->d_npast + who, &p, 4, cudaMemcpyHostToDevice, st->e->ctx.stream));   // staged at once
+            }
         }
     }
-    z.state = 0; z.gen++;
+    if (z.guide >= 0) { st->sess[z.guide].state = 0; st->sess[z.guide].owner = -1; st->sess[z.guide].gen++; }
+    z.state = 0; z.gen++; z.guide = -1;
     return 0;
 }
 
@@ -4480,41 +4744,82 @@ static int stream_finish(b200_stream * st, int k) {
 // fed and that still owes ids decodes one row; then the sessions with prompt ids left, in add order, each get their next
 // chunk (the whole prompt when chunk == 0) while the rows fit in max_rows; the first that does not fit ends the step.
 // Only a session whose last chunk is in the pass draws, from that chunk's last row.
+// A guided session and its guidance session are one unit: a decode row each (both take the guided session's last id),
+// and while prefilling, the next non-final chunk of each prompt; a prompt at its final chunk waits until the other's final
+// chunk goes in the same step, which draws.  The guided rows come first among the drawing rows, so the lm_head's guidance
+// rows and k_cfg_rows' output follow them in order.
 static int stream_step(b200_stream * st, bool * did) {
     *did = false;
-    std::vector<int> ses, cnt;
+    struct Entry { int session, count, src; };            // src: the session whose last id a decode row takes; -1: prompt
+    struct Draw { int k, gather, gather2; };
+    std::vector<Entry> ent;
+    std::vector<Draw> guided, plain;
     int N = 0;
     for (int k = 0; k < st->n_sess; k++) {
         const b200_stream::Sess & z = st->sess[k];
-        if (z.state == 2 && z.fed == (int) z.prompt.size() && z.enq < z.max_tokens) { ses.push_back(k); cnt.push_back(1); N++; }
+        if (z.state == 2 && z.fed == (int) z.prompt.size() && (z.guide < 0 || z.gfed == (int) z.neg.size()) &&
+            z.enq < z.max_tokens) {
+            ent.push_back({k, 1, k});
+            N++;
+            if (z.guide < 0) { plain.push_back({k, N - 1, -1}); continue; }
+            ent.push_back({z.guide, 1, k});
+            N++;
+            guided.push_back({k, N - 2, N - 1});
+        }
     }
-    const int n_decode = (int) ses.size();
+    std::vector<int> fed_now;                             // queued sessions this step feeds
+    std::vector<std::pair<int, int>> chunk_now;           // their (prompt, negative prompt) ids this step
     for (int k : st->queue) {
         const b200_stream::Sess & z = st->sess[k];
         const int left = (int) z.prompt.size() - z.fed, c = st->chunk ? std::min(st->chunk, left) : left;
-        if (N + c > st->max_rows) break;
-        ses.push_back(k); cnt.push_back(c); N += c;
+        int cn = 0;
+        bool draws = c == left;
+        int cp = c;
+        if (z.guide >= 0) {
+            const int gleft = (int) z.neg.size() - z.gfed;
+            cn = st->chunk ? std::min(st->chunk, gleft) : gleft;
+            const bool gfinal = cn == gleft;
+            draws = draws && gfinal;
+            if (!draws) {                                 // a final chunk waits for the other prompt's final chunk
+                if (c == left) cp = 0;
+                if (gfinal) cn = 0;
+            }
+        }
+        if (N + cp + cn > st->max_rows) break;
+        int gather = -1, gather2 = -1;
+        if (cp) { ent.push_back({k, cp, -1}); N += cp; gather = N - 1; }
+        if (cn) { ent.push_back({z.guide, cn, -1}); N += cn; gather2 = N - 1; }
+        fed_now.push_back(k);
+        chunk_now.emplace_back(cp, cn);
+        if (draws) (z.guide >= 0 ? guided : plain).push_back({k, gather, gather2});
     }
-    const int n = (int) ses.size();
+    const int n = (int) ent.size();
     if (n == 0) return 0;
     const int q = (int)(st->n_steps % (st->lookahead + 1));
     int32_t * spec = st->h_spec + (size_t) q * st->max_rows;
     StreamRow * rows = st->h_rows + (size_t) q * st->rows_cap;
     volatile int32_t * ring = st->h_ring + (size_t) q * st->rows_cap;
     b200_stream::Step step{q, {}, 0};
-    bool any_lp = false;
-    std::vector<int> drawing;                       // the sessions that draw, in row order of the pass
     for (int j = 0, r = 0; j < n; j++) {
-        b200_stream::Sess & z = st->sess[ses[j]];
-        if (j < n_decode) spec[r++] = ~ses[j];
-        else for (int i = z.fed; i < z.fed + cnt[j]; i++) spec[r++] = z.prompt[i];
-        if (j >= n_decode && z.fed + cnt[j] < (int) z.prompt.size()) continue;   // a non-final chunk: no draw
-        const int d = (int) drawing.size();
-        rows[d] = {z.first_draw + z.enq, ses[j], r - 1, z.n_top};
+        const Entry & en = ent[j];
+        if (en.src >= 0) { spec[r++] = ~en.src; continue; }
+        // a prompt chunk: the guided session's or its guidance session's, in the order stream_step listed them
+        const b200_stream::Sess & owner = st->sess[st->sess[en.session].state == 3 ? st->sess[en.session].owner : en.session];
+        const bool neg = st->sess[en.session].state == 3;
+        const int at = neg ? owner.gfed : owner.fed;
+        const std::vector<int32_t> & src = neg ? owner.neg : owner.prompt;
+        for (int i = at; i < at + en.count; i++) spec[r++] = src[i];
+    }
+    const int n_g = (int) guided.size();
+    std::vector<Draw> drawing(guided);
+    drawing.insert(drawing.end(), plain.begin(), plain.end());
+    bool any_lp = false;
+    for (int d = 0; d < (int) drawing.size(); d++) {
+        b200_stream::Sess & z = st->sess[drawing[d].k];
+        rows[d] = {z.first_draw + z.enq, drawing[d].k, drawing[d].gather, z.n_top, drawing[d].gather2};
         any_lp |= z.n_top >= 0;
         ring[d] = INT32_MIN;
-        step.rows.emplace_back(ses[j], z.gen);
-        drawing.push_back(ses[j]);
+        step.rows.emplace_back(drawing[d].k, z.gen);
     }
     const int n_draw = (int) drawing.size();
     if (n_draw == 0) ring[0] = INT32_MIN;
@@ -4526,11 +4831,13 @@ static int stream_step(b200_stream * st, bool * did) {
     x->launches += 2;
     // a single session decoding alone replays the slice's captured decode graph; anything else is one pass (all-1 counts:
     // the batched step).  Both are exact mode, as b200_mixed_forward.
+    std::vector<int> ses(n), cnt(n);
+    for (int j = 0; j < n; j++) { ses[j] = ent[j].session; cnt[j] = ent[j].count; }
     const float * cur = e->d_x;
     int rc;
     for (b200_slice * s : st->slices) {
-        if (N == 1 && n_decode == 1) rc = forward_locked(s, cur, 1, s->d_out, false, ses[0]);
-        else                         rc = pass_locked(s, ses.data(), cnt.data(), n, cur, s->d_out, false);
+        if (N == 1 && ent[0].src >= 0) rc = forward_locked(s, cur, 1, s->d_out, false, ses[0]);
+        else                           rc = pass_locked(s, ses.data(), cnt.data(), n, cur, s->d_out, false);
         if (rc) return rc;
         cur = s->d_out;
     }
@@ -4540,16 +4847,45 @@ static int stream_step(b200_stream * st, bool * did) {
         B200_CUDA(cudaGetLastError());
         x->launches++;
     } else {
-        if (N > n_draw) {                           // each drawing session's last row, packed for the lm_head
+        const int n_lm = n_draw + n_g;                    // the drawing rows, then the guided ones' guidance rows
+        if (N > n_lm || n_g) {                            // each drawing session's last row, packed for the lm_head
             k_gather_rows<<<dim3((e->E + 255) / 256, n_draw), 256, 0, x->stream>>>(cur, rows, e->E, e->d_x);
             B200_CUDA(cudaGetLastError());
             x->launches++;
+            if (n_g) {
+                k_gather_rows<<<dim3((e->E + 255) / 256, n_g), 256, 0, x->stream>>>(cur, rows, e->E, e->d_x + (size_t) n_draw * e->E,
+                                                                                    true);
+                B200_CUDA(cudaGetLastError());
+                x->launches++;
+            }
             cur = e->d_x;
         }
-        if ((rc = extra_lmhead(e, cur, n_draw))) return rc;
-        k_stream_draw<<<n_draw, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, rows, st->d_slots, st->d_pen, st->d_last, cells);
-        B200_CUDA(cudaGetLastError());
-        x->launches++;
+        if ((rc = extra_lmhead(e, cur, n_lm))) return rc;
+        const size_t V = (size_t) e->n_vocab;
+        if (n_g) {
+            // one guidance setting per launch: guided rows are grouped by (scale, sf) runs
+            for (int d0 = 0; d0 < n_g;) {
+                const b200_stream::Sess & z0 = st->sess[drawing[d0].k];
+                int d1 = d0 + 1;
+                while (d1 < n_g && st->sess[drawing[d1].k].scale == z0.scale && st->sess[drawing[d1].k].sf == z0.sf) d1++;
+                CfgArgs c{e->d_logits + d0 * V, e->d_logits + (n_draw + d0) * V, e->n_vocab, z0.scale, z0.sf, e->d_cfg + d0 * V,
+                          e->d_ids + d0, nullptr, nullptr, 0};
+                k_cfg_rows<<<d1 - d0, kCfgThreads, 0, x->stream>>>(c);
+                B200_CUDA(cudaGetLastError());
+                x->launches++;
+                d0 = d1;
+            }
+            k_stream_draw<<<n_g, 1024, 0, x->stream>>>(e->d_cfg, e->n_vocab, rows, st->d_slots, st->d_pen, st->d_last, cells,
+                                                       e->d_ids);
+            B200_CUDA(cudaGetLastError());
+            x->launches++;
+        }
+        if (n_draw > n_g) {
+            k_stream_draw<<<n_draw - n_g, 1024, 0, x->stream>>>(e->d_logits + n_g * V, e->n_vocab, rows + n_g, st->d_slots,
+                                                                st->d_pen, st->d_last, cells + n_g);
+            B200_CUDA(cudaGetLastError());
+            x->launches++;
+        }
         if (any_lp) {                               // publishes the rows that asked, after their records
             k_stream_logprobs<<<n_draw, 1024, 0, x->stream>>>(e->d_logits, e->n_vocab, rows, st->d_last, cells,
                                                               st->h_lp + (size_t) q * st->rows_cap);
@@ -4557,13 +4893,15 @@ static int stream_step(b200_stream * st, bool * did) {
             x->launches++;
         }
     }
-    for (int j = n_decode; j < n; j++) {
-        b200_stream::Sess & z = st->sess[ses[j]];
-        z.state = 2; z.fed += cnt[j];
+    for (size_t j = 0; j < fed_now.size(); j++) {
+        b200_stream::Sess & z = st->sess[fed_now[j]];
+        z.state = 2; z.fed += chunk_now[j].first; z.gfed += chunk_now[j].second;
     }
-    st->queue.erase(std::remove_if(st->queue.begin(), st->queue.end(),
-                                   [st](int k) { return st->sess[k].fed == (int) st->sess[k].prompt.size(); }), st->queue.end());
-    for (int k : drawing) st->sess[k].enq++;
+    st->queue.erase(std::remove_if(st->queue.begin(), st->queue.end(), [st](int k) {
+        const b200_stream::Sess & z = st->sess[k];
+        return z.fed == (int) z.prompt.size() && (z.guide < 0 || z.gfed == (int) z.neg.size());
+    }), st->queue.end());
+    for (const Draw & d : drawing) st->sess[d.k].enq++;
     st->pending.push_back(std::move(step));
     st->n_steps++; st->n_rows += N; st->most_rows = std::max(st->most_rows, N);
     *did = true;
@@ -4708,13 +5046,55 @@ int b200_stream_add(b200_stream_t * st, int session, const int32_t * prompt, int
     return b200_stream_add_lp(st, session, prompt, n_prompt, max_tokens, sp, stop_ids, n_stop, -1);
 }
 
-int b200_stream_add_lp(b200_stream_t * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
-                       const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop, int n_top) {
+}  // extern "C"
+
+namespace b200 {
+
+// The largest step a guided pair's prefill takes under stream_step's rule (chunks of c ids, 0: whole prompts; a final
+// chunk waits for the other's).
+static int cfg_unit_rows(int n_prompt, int n_neg, int c) {
+    if (!c) return n_prompt + n_neg;
+    int most = 0;
+    for (int a = n_prompt, b = n_neg; a > 0 || b > 0;) {
+        const int ca = std::min(c, a), cb = std::min(c, b);
+        const bool fa = ca == a, fb = cb == b;
+        const int rows = fa && fb ? ca + cb : (fa ? 0 : ca) + (fb ? 0 : cb);
+        most = std::max(most, rows);
+        if (!(fa && fb)) { if (!fa) a -= ca; if (!fb) b -= cb; } else { a = 0; b = 0; }
+    }
+    return most;
+}
+
+// b200_stream_add_lp, and with guide >= 0 b200_stream_add_cfg.
+static int stream_add(b200_stream * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
+                      const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop, int n_top, int guide,
+                      const int32_t * neg, int n_neg, float scale, float sf) {
     std::vector<std::unique_lock<std::mutex>> locks;
     if (int rc = stream_lock(st, locks)) return rc;
     if (session < 0 || session >= st->n_sess) return fail(B200_EINVAL, "session %d outside [0, %d)", session, st->n_sess);
     b200_stream::Sess & z = st->sess[session];
+    if (z.state == 3) return fail(B200_EINVAL, "session %d is the guidance session of session %d", session, z.owner);
     if (z.state) return fail(B200_EINVAL, "session %d is already in the stream", session);
+    if (guide >= 0 || neg) {
+        if (guide < 0 || guide >= st->n_sess) return fail(B200_EINVAL, "guidance session %d outside [0, %d)", guide, st->n_sess);
+        if (guide == session) return fail(B200_EINVAL, "session %d cannot be its own guidance session", session);
+        if (st->sess[guide].state == 3)
+            return fail(B200_EINVAL, "guidance session %d is the guidance session of session %d", guide, st->sess[guide].owner);
+        if (st->sess[guide].state) return fail(B200_EINVAL, "guidance session %d is already in the stream", guide);
+        if (!neg || n_neg < 1) return fail(B200_EINVAL, "session %d: the negative prompt needs at least one id", session);
+        if (int rc = cfg_mix_check(scale, sf)) return rc;
+        if (int rc = check_tokens(neg, n_neg, st->e->n_vocab, "negative prompt token")) return rc;
+        for (size_t i = 0; i < st->slices.size(); i++) {
+            const b200_slice * s = st->slices[i];
+            if ((long long) s->past[guide] + n_neg + max_tokens - 1 > s->n_ctx)
+                return fail(B200_ECONTEXT, "context overflow: slice %zu guidance session %d n_past %d + %d negative prompt "
+                            "tokens + %d steps > n_ctx %d", i, guide, s->past[guide], n_neg, max_tokens - 1, s->n_ctx);
+        }
+        if (n_prompt >= 1 && cfg_unit_rows(n_prompt, n_neg, st->chunk) > st->max_rows)
+            return fail(B200_EINVAL, "session %d: its prompt (%d ids) and negative prompt (%d ids) need a step of %d rows, "
+                        "more than max_rows %d", session, n_prompt, n_neg, cfg_unit_rows(n_prompt, n_neg, st->chunk),
+                        st->max_rows);
+    }
     if (!prompt || n_prompt < 1) return fail(B200_EINVAL, "session %d: the prompt needs at least one id", session);
     if (max_tokens < 1) return fail(B200_EINVAL, "session %d: max_tokens must be positive (got %d)", session, max_tokens);
     if (n_stop < 0 || (n_stop > 0 && !stop_ids)) return fail(B200_EINVAL, "session %d: bad stop list", session);
@@ -4733,6 +5113,12 @@ int b200_stream_add_lp(b200_stream_t * st, int session, const int32_t * prompt, 
     }
     if (!st->chunk && n_prompt > st->max_rows)
         return fail(B200_EINVAL, "session %d: a prompt of %d ids exceeds max_rows %d (a prompt is never split)", session, n_prompt, st->max_rows);
+    if (guide >= 0) {
+        int rc;
+        if ((rc = extra_regrow(st->e, st->e->d_cfg, st->e->cap_cfg, (size_t) st->e->n_vocab, st->rows_cap)) ||
+            (rc = extra_reserve_ids(st->e, st->rows_cap)))
+            return rc;
+    }
     // the slot's sampler state, in stream order behind any step still running for an earlier stay of the session
     const double dt = sp ? sp->temperature + 1e-5 : 1.0;
     const StreamSlot slot{sp ? sp->seeds[0] : 0, dt, sp ? sp->repeat_penalty * dt : 1.0, sp ? 1 : 0, sp ? (int) sp->top_k : 0,
@@ -4751,9 +5137,34 @@ int b200_stream_add_lp(b200_stream_t * st, int session, const int32_t * prompt, 
     for (const b200_slice * s : st->slices) z.old.push_back(s->past[session]);
     z.fed = 0; z.max_tokens = max_tokens; z.enq = 0; z.delivered = 0; z.n_top = n_top;
     z.first_draw = sp ? sp->first_draw : 0;
+    z.guide = guide; z.gfed = 0; z.scale = scale; z.sf = sf;
+    z.neg.assign(neg, neg + (guide >= 0 ? n_neg : 0));
+    if (guide >= 0) {
+        b200_stream::Sess & w = st->sess[guide];
+        w.state = 3; w.owner = session;
+        w.old.clear();
+        for (const b200_slice * s : st->slices) w.old.push_back(s->past[guide]);
+    }
     z.state = 1;
     st->queue.push_back(session);
     return 0;
+}
+
+}  // namespace b200
+
+extern "C" {
+
+int b200_stream_add_lp(b200_stream_t * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
+                       const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop, int n_top) {
+    return stream_add(st, session, prompt, n_prompt, max_tokens, sp, stop_ids, n_stop, n_top, -1, nullptr, 0, 0.f, 0.f);
+}
+
+int b200_stream_add_cfg(b200_stream_t * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
+                        const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop, int n_top, int guidance_session,
+                        const int32_t * neg, int n_neg, float scale, float smooth_factor) {
+    if (guidance_session < 0) return fail(B200_EINVAL, "guidance session %d outside [0, n_sessions)", guidance_session);
+    return stream_add(st, session, prompt, n_prompt, max_tokens, sp, stop_ids, n_stop, n_top, guidance_session, neg, n_neg,
+                      scale, smooth_factor);
 }
 
 int b200_stream_read(b200_stream_t * st, int32_t * sessions, int32_t * ids, int cap, int * n_out) {
@@ -4773,6 +5184,9 @@ int b200_stream_cancel(b200_stream_t * st, int session) {
     if (int rc = stream_lock(st, locks)) return rc;
     if (session < 0 || session >= st->n_sess || st->sess[session].state == 0)
         return fail(B200_EINVAL, "session %d is not in the stream", session);
+    if (st->sess[session].state == 3)
+        return fail(B200_EINVAL, "session %d is the guidance session of session %d: cancel that one", session,
+                    st->sess[session].owner);
     return stream_finish(st, session);
 }
 
@@ -4781,6 +5195,8 @@ int b200_stream_fork(b200_stream_t * st, int src, int dst, int n_keep) {
     if (int rc = stream_lock(st, locks)) return rc;
     for (int k : {src, dst}) {
         if (k < 0 || k >= st->n_sess) return fail(B200_EINVAL, "session %d outside [0, %d)", k, st->n_sess);
+        if (st->sess[k].state == 3)
+            return fail(B200_EINVAL, "session %d is the guidance session of session %d", k, st->sess[k].owner);
         if (st->sess[k].state) return fail(B200_EINVAL, "session %d is %s", k, st->sess[k].state == 1 ? "queued" : "active");
     }
     if (src == dst) return fail(B200_EINVAL, "b200_stream_fork: source and destination are both session %d", src);
@@ -4810,7 +5226,7 @@ int b200_stream_close(b200_stream_t * st) {
         std::vector<std::unique_lock<std::mutex>> locks;
         if ((rc = stream_lock(st, locks))) return rc;
         for (int k = 0; k < st->n_sess && !rc; k++)
-            if (st->sess[k].state) rc = stream_finish(st, k);
+            if (st->sess[k].state == 1 || st->sess[k].state == 2) rc = stream_finish(st, k);
         if (!rc && cudaStreamSynchronize(st->e->ctx.stream) != cudaSuccess) rc = fail(B200_ECUDA, "generation stream failed");
         st->loan.reset();
         for (b200_slice * s : st->slices) s->owner = nullptr;

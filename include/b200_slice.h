@@ -474,6 +474,51 @@ int b200_generate_speculative_lp(b200_slice_t * const * slices, int n_slices, b2
 int b200_extra_logprobs(b200_extra_t * e, const float * logits, int n_rows, const int32_t * ids, int n_top,
                         double * lp, int32_t * top_ids, double * top_lp);
 
+/* ---- classifier-free guidance (llama.cpp main's --cfg-negative-prompt, --cfg-scale, --cfg-smooth-factor) ---------------
+ * Each generating session k has a guidance session fed a negative prompt, then the same ids session k draws.  Before each
+ * draw, with b session k's logits and g its guidance session's (llama_sample_classifier_free_guidance, llama.cpp:2170-2225):
+ *   log_softmax(v): m = max_element(v) (v_0 when v_0 is NaN, else the first largest non-NaN value), p_i = expf(v_i - m)
+ *     with the subtraction in float, S = the p_i summed in float strictly in index order 0 .. n_vocab-1,
+ *     v_i = logf(p_i / S) with the division in float;
+ *   lb = log_softmax(b), lg = log_softmax(g), mix_i = fmaf(scale, lb_i - lg_i, lg_i), lg2 = log_softmax(mix),
+ *   out_i = fmaf(smooth_factor, lg2_i, (1 - smooth_factor) * lb_i).
+ * The two FMAs are those the reference build contracts; nothing else is fused.  expf / logf are the double functions
+ * rounded to float; glibc's, which llama.cpp calls, are not correctly rounded everywhere, and that is the one place the
+ * two can give different bits.  out replaces b as the row the draw reads:
+ *   - greedy: max_element(out) with `<` (llama_sample_token_greedy): out_0 when it is NaN, else the first largest
+ *     non-NaN value.  Where lb_i underflowed to -inf, smooth_factor 1 gives out_i = NaN (0 * -inf), and an index where
+ *     lb and lg are both -inf makes the whole row NaN (id 0);
+ *   - sampled: the Sampler of b200_generate_sample, unchanged, on out; a row holding a NaN has no distribution there;
+ *   - a pair whose b or g holds a NaN or +inf, or is all -inf, has no distribution in either mode: its id is -1 and the
+ *     call returns B200_EINVAL naming the first such step and session, after the loop (positions have moved).
+ * Log-probabilities stay those of the raw b: guidance, like temperature, penalty and truncation, is not in them.  Guidance
+ * is on only when asked for: at scale 1 the formula is not the identity bit for bit, so these calls refuse scale <= 1. */
+typedef struct b200_guidance {
+    const int * sessions;          /* [n_seq]: session k's guidance session */
+    const int * prompt_counts;     /* [n_seq], >= 1: negative prompt lengths */
+    const int32_t * prompt_tokens; /* the negative prompts, grouped in list order */
+    float scale;                   /* finite, > 1 */
+    float smooth_factor;           /* finite */
+} b200_guidance_t;
+/* b200_generate_lp's loop (sp NULL: greedy; lp NULL: no log-probabilities) over 2 * n_seq sessions: step 0 is one mixed
+ * pass of every prompt and every negative prompt, each later step one pass of 2 * n_seq decode rows, guidance row k taking
+ * the id session k drew.  The lm_head runs on both rows of each pair, then the guidance kernel, then the draw.
+ *   - Positions: session k and its guidance session end at old + count + n_steps - 1 with their own counts, so a second
+ *     call with prompt and negative prompt both [last id] (sampled: history and first_draw as b200_generate_sample)
+ *     continues the run exactly.  A session's ids are the same alone, in a batch, or split across calls.
+ *   - All-or-nothing: as b200_generate_lp, plus B200_EINVAL for a null g, a guidance session out of range, listed twice or
+ *     equal to a listed session, a negative prompt count < 1 or id outside [0, n_vocab), scale not finite or <= 1, and
+ *     smooth_factor not finite; B200_ECONTEXT when either context of a pair would overflow on some slice. */
+int b200_generate_cfg(b200_slice_t * const * slices, int n_slices, b200_extra_t * e,
+                      const int * sessions, const int * prompt_counts, int n_seq,
+                      const int32_t * prompt_tokens, int n_steps, const b200_guidance_t * g,
+                      const b200_sampling_t * sp /* NULL: greedy */, int32_t * ids, const b200_logprobs_t * lp /* NULL: none */);
+/* The guidance kernel on host rows base / guidance [n_rows][n_vocab]: out [n_rows][n_vocab] as above, and greedy[k] (may
+ * be NULL) the greedy id of row k (-1 for an all -inf input row, whose out is NaN).  A NaN or +inf input is B200_EINVAL
+ * before anything runs, as are scale and smooth_factor b200_generate_cfg refuses. */
+int b200_extra_cfg(b200_extra_t * e, const float * base, const float * guidance, int n_rows, float scale,
+                   float smooth_factor, float * out, int32_t * greedy);
+
 /* ---- generation streams: sessions join and leave between steps, ids reach the caller as they are drawn ----------------
  * A stream runs the generation loop of b200_generate_greedy / b200_generate_sample over a chain of slices on one GPU (the
  * same handle checks: contiguous layers, one device, no pipeline, the extra layers' n_embd), but open-ended:
@@ -543,6 +588,27 @@ int b200_stream_read(b200_stream_t * st, int32_t * sessions, int32_t * ids, int 
  * stores the id.  Rows that do not ask are published by the draw as before. */
 int b200_stream_add_lp(b200_stream_t * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
                        const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop, int n_top);
+/* b200_stream_add_lp (n_top -1: no log-probabilities) with classifier-free guidance (see b200_generate_cfg): session
+ * guidance_session is fed neg (n_neg ids), then every id the session draws, and each draw reads the guided row.  The pair
+ * belongs to the stream as a unit:
+ *   - each step, a decoding pair has two decode rows, both taking the session's last id; b200_stream_stats counts both;
+ *   - prefill: on a prefill_chunk 0 stream both prompts go whole into one step; with C > 0 each is cut into chunks counted
+ *     from its own first id, each step takes the pair's next non-final chunk of each prompt as one unit (the fit and
+ *     no-overtaking rule of b200_stream_open_ex), and a prompt at its final chunk waits until the other's final chunk goes
+ *     in the same step, which draws;
+ *   - contract: the ids (and log-probabilities, of the raw rows) equal b200_session_forward of each prompt's non-final
+ *     chunks on its own session, then b200_generate_cfg with the two final chunks, the same settings and n_steps =
+ *     delivered; whatever joined, ran beside it or left (so with C = 0, b200_generate_cfg with the whole prompts);
+ *   - positions: the guidance session ends with the session, at old + n_neg + delivered - 1 (old when nothing was
+ *     delivered, so also when cancelled mid-prefill);
+ *   - while the pair is in the stream, naming the guidance session in b200_stream_add, _cancel or _fork is B200_EINVAL;
+ *     cancelling the session ends both.
+ * All-or-nothing as b200_stream_add, plus B200_EINVAL for a guidance session out of range, equal to session or already in
+ * the stream, n_neg < 1, an id of neg outside [0, n_vocab), scale not finite or <= 1, smooth_factor not finite, or a pair
+ * whose largest prefill step exceeds max_rows; B200_ECONTEXT when the guidance context would overflow. */
+int b200_stream_add_cfg(b200_stream_t * st, int session, const int32_t * prompt, int n_prompt, int max_tokens,
+                        const b200_sampling_t * sp, const int32_t * stop_ids, int n_stop, int n_top, int guidance_session,
+                        const int32_t * neg, int n_neg, float scale, float smooth_factor);
 /* b200_stream_read with each id's record: lp [cap], top_ids / top_lp [cap][20], entry j < the session's n_top filled, the
  * rest -1 / NaN; a session added without log-probabilities reads back lp NaN and top_ids -1.  b200_stream_read still works on
  * any stream and drops the records. */
